@@ -1,14 +1,16 @@
 #!/usr/bin/env python3
-"""bench.py -- images/sec of the B200 int8 convolution + GEMM backend on BASELINE.json's headline workload.
+"""bench.py -- images/sec of the H100 int8 convolution + GEMM backend on BASELINE.json's headline workload.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload mobilenet_v1_int8] [--batch B] [--global-batch G]
+                  [--dump-outputs DIR]
 
 One "step" = one pass of the hot path (the whole MobileNet-v1 int8 224x224 graph: 28 convolutions + global pool,
 through tb200_graph_*) over one synthetic batch of 256 images per GPU.
   value   whole-job images/s with the batch already resident in HBM (device timing, CUDA events, max over ranks)
   e2e     the same through the reference-facing call tb200_graph_run() with HOST buffers (plain malloc'd arrays, as Tengine
           hands them over; the library page-locks them on first sight), H2D + D2H inside
-  roofline  dominant kernel: algorithmic bytes / its event-timed duration vs the measured HBM peak
+  roofline  dominant kernel: algorithmic bytes / its event-timed duration vs the HBM peak
+  --dump-outputs DIR : after the timed steps, the graph outputs of the last timed step as DIR/output<i>.npy (float32)
   cpu_baseline / --impl reference : the UNMODIFIED reference CPU backend (oracle/_ref) on this box's host cores
 Multi-GPU: ONE process drives all N GPUs through the product (a tb200 context over N GPUs): every step hands ONE batch of
 256 x N images (weak scaling) -- or --global-batch images (strong scaling, C4/C5) -- to tb200_graph_run, which shards dim 0
@@ -49,11 +51,11 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks + throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks + throttle reasons during the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -90,23 +92,6 @@ class ClockSampler(threading.Thread):
         busy = sorted(sm)[len(sm) // 2:] if sm else []
         return {"sm_mhz": float(np.median(busy)) if busy else None, "sm_max_mhz": max(mx) if mx else None,
                 "reasons": sorted(reasons), "samples": len(sm)}
-
-
-def ncu_traffic(workload, batch, family):
-    """dram__bytes_read.sum + dram__bytes_write.sum of the kernel family, summed over its launches of one step, from the
-    committed `ncu --set full` capture (profiles/rNN_ncu_traffic.json, newest round first, made by tools/ncu_traffic_json.py; not
-    measured live: ncu replays every kernel ~40x).  None when no capture is of this workload / batch."""
-    for name in ("r02_ncu_traffic.json", "r01_ncu_traffic.json"):
-        p = os.path.join(ROOT, "profiles", name)
-        if not os.path.exists(p):
-            continue
-        d = json.load(open(p))
-        if d.get("workload") != workload or d.get("batch") != batch:
-            continue
-        f = d["families"].get(family)
-        if f:
-            return float(f["dram_bytes_per_step"])
-    return None
 
 
 def build_workload(name, batch):
@@ -228,13 +213,13 @@ def run_reference_arm(args, rank):
 
 
 def int8_tensor_peak(ctx=None):
-    """(TOPS, source): the on-box tcgen05 kind::i8 peak measured live by the library's pure-MMA probe, else twice the measured
-    dense bf16 rate of MEASURED_PEAKS.json (kind::i8 issues at twice the bf16 rate), else the nominal 4500."""
+    """(TOPS, source): the on-box wgmma s8 peak measured live by the library's pure-MMA probe, else twice the measured
+    dense bf16 rate of MEASURED_PEAKS.json (int8 issues at twice the bf16 rate), else the H100 SXM data sheet's dense 1979."""
     if ctx is not None:
         try:
             t = ctx.probe_int8_tops()
             if t > 100:
-                return t, "measured live: tcgen05.mma kind::i8 128x256x32 loop, one CTA per SM (tb200_probe_int8_tops)"
+                return t, "measured live: wgmma m64n128k32 s8 loop, two warpgroups per SM (tb200_probe_int8_tops)"
         except Exception:
             pass
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
@@ -242,7 +227,7 @@ def int8_tensor_peak(ctx=None):
         d = json.load(open(p))
         if "bf16_tflops" in d:
             return 2.0 * float(d["bf16_tflops"]), "2 x measured dense bf16 (MEASURED_PEAKS.json bf16_tflops)"
-    return 4500.0, "nominal dense int8 (B200_PROFILING.md)"
+    return 1979.0, "H100 SXM data sheet, dense int8"
 
 
 # ---- rank protocol under torchrun (N > 1): a process group over gloo (CPU), so that the ranks which only wait never create a CUDA
@@ -311,13 +296,15 @@ def main():
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--impl", default="b200")
+    ap.add_argument("--impl", default="h100")
     ap.add_argument("--workload", default="mobilenet_v1_int8")
     ap.add_argument("--batch", type=int, default=0, help="images per GPU per step (0: the workload's BASELINE.json batch)")
     ap.add_argument("--global-batch", type=int, default=0, help="strong scaling: total images per step, split over the GPUs")
     ap.add_argument("--no-tensorcore", action="store_true", help="route convs through the CUDA-core cross-check kernels")
     ap.add_argument("--cpu-window", type=float, default=12.0, help="cpu_baseline: length of the fleet window in seconds; 0 disables")
     ap.add_argument("--pinned", action="store_true", help="e2e with cudaHostAlloc'd caller buffers instead of pageable ones")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the graph outputs of the last timed step to DIR/<name>.npy (float32, at most 64 MB in all)")
     ap.add_argument("--watchdog", type=float, default=780.0, help="seconds after which a stuck run dumps its Python stacks and exits (0 = off)")
     args = ap.parse_args()
     if args.watchdog > 0 and int(os.environ.get("RANK", "0")) == 0:
@@ -355,6 +342,32 @@ def main():
         run_product_arm(args, ngpu, world, lead.barrier)
     finally:
         lead.finish()  # also on an exception: the followers must not be left waiting
+
+
+DUMP_LIMIT = 64 << 20  # bytes that --dump-outputs writes at most, .npy headers included
+NPY_HEADER = 128       # bytes of a version-1 .npy header for a float32 array of up to 3 dimensions
+
+
+def dump_sample_positions(n, k, i):
+    """Flat positions (sorted) of the k elements kept of output i (n elements): a fixed seed per output index, so that a reader
+    regenerates them instead of loading them."""
+    return np.sort(np.random.default_rng(1234 + i).choice(n, k, replace=False))
+
+
+def dump_outputs(out_dir, graph, ys):
+    """The graph outputs the last timed launch left on the device (what a caller downloads), as float32 DIR/output<i>.npy in the
+    graph's output order.  Each output gets an equal share of DUMP_LIMIT; one that does not fit is stored as the 1-D array of its
+    elements at dump_sample_positions(size, kept, i)."""
+    os.makedirs(out_dir, exist_ok=True)
+    outs = [np.empty_like(y) for y in ys]
+    for i, out in enumerate(outs):
+        graph.download(i, out)
+    graph.sync()
+    keep = (DUMP_LIMIT // len(outs) - NPY_HEADER) // 4  # elements per output
+    for i, out in enumerate(outs):
+        flat = out.reshape(-1).astype(np.float32)
+        arr = flat.reshape(out.shape) if flat.size <= keep else flat[dump_sample_positions(flat.size, keep, i)]
+        np.save(os.path.join(out_dir, f"output{i}.npy"), arr)
 
 
 def run_product_arm(args, ngpu, world, barrier):
@@ -404,7 +417,7 @@ def run_product_arm(args, ngpu, world, barrier):
         verified = f"every shard's output bytes == a single-GPU context's result for the same images ({len(shards)} shards checked)"
 
     streams = [torch.cuda.ExternalStream(ctx.stream_of(i), device=devices[i]) for i in range(ngpu)]
-    flush = [torch.empty(256 << 20, dtype=torch.uint8, device=f"cuda:{d}") for d in devices]  # > 126 MB L2 each
+    flush = [torch.empty(256 << 20, dtype=torch.uint8, device=f"cuda:{d}") for d in devices]  # > 50 MB L2 each
 
     # ---------------- device-resident: `value` ----------------
     graph.upload(0, x)
@@ -433,6 +446,8 @@ def run_product_arm(args, ngpu, world, barrier):
     wall_dev = time.time() - wall0
     dev_ms = max(sum(a.elapsed_time(b_) for a, b_ in ev[i]) for i in range(ngpu))  # max over GPUs of the K-step device time
     clocks = sampler.finish()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, graph, ys)
 
     # ---------------- end to end through the reference-facing call with HOST buffers: `e2e` ----------------
     for _ in range(2):
@@ -480,7 +495,7 @@ def run_product_arm(args, ngpu, world, barrier):
     else:
         achieved = dom_bytes / (dom_ms / 1000.0) / 1e9
         roof = {"bound": "hbm", "achieved": achieved, "peak": hbm_peak, "unit": "GB/s", "frac": achieved / hbm_peak, "peak_source": hbm_src}
-    roof.update({"kernel": dom, "launches_per_step": len(fam[dom]), "traffic": ncu_traffic(args.workload, shard0, dom),
+    roof.update({"kernel": dom, "launches_per_step": len(fam[dom]), "traffic": None,  # measured DRAM bytes: no stored capture
                  "kernel_ms_per_step": dom_ms, "share_of_step": dom_ms / float(prof.sum()), "algorithmic_bytes_per_launch_set": dom_bytes,
                  "algorithmic_ops_per_launch_set": dom_ops, "arithmetic_intensity_op_per_byte": intensity, "ridge_op_per_byte": ridge,
                  "measured_on": f"cuda:{devices[0]} (its shard: {shard0} images)"})
@@ -504,7 +519,7 @@ def run_product_arm(args, ngpu, world, barrier):
                    "global_batch": total_batch,
                    "parallelism": (f"ONE process, one tb200 context over {ngpu} GPU(s): dim 0 sharded {[s[2] for s in shards]} inside tb200_graph_run; weights packed on GPU 0, "
                                    f"one {ctx.broadcast_kind} broadcast of the arena at prerun, no collective in the steady state" if ngpu > 1 else "single GPU"),
-                   "l2": "256 MiB L2 flush per GPU between timed iterations; per-step activations >> 126 MB L2",
+                   "l2": "256 MiB L2 flush per GPU between timed iterations; per-step activations >> 50 MB L2",
                    "layout": "NHWC int8 in HBM, channels padded to 16",
                    "verified": verified},
         "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": int(x.nbytes), "d2h_bytes_per_step": int(sum(y.nbytes for y in ys)),

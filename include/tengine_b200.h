@@ -1,5 +1,5 @@
 /*
- * tengine_b200.h -- C ABI of the B200 (sm_100a) int8/uint8 convolution + GEMM device backend for Tengine.
+ * tengine_b200.h -- C ABI of the H100 (sm_90a) int8/uint8 convolution + GEMM device backend for Tengine.
  *
  * Plain C, plain pointers and sizes; no CUDA, torch or Tengine types appear in any signature.
  * libtengine_b200.so exports exactly the symbols declared here.  Every entry point names the
@@ -39,7 +39,7 @@ extern "C" {
 /* ---- error codes ------------------------------------------------------------------------------- */
 #define TB200_OK 0
 #define TB200_ERR_INVALID (-1)     /* bad argument / unsupported parameter combination                 */
-#define TB200_ERR_NO_DEVICE (-2)   /* no CUDA device, or not sm_100                                    */
+#define TB200_ERR_NO_DEVICE (-2)   /* no CUDA device, or not sm_90                                     */
 #define TB200_ERR_CUDA (-3)        /* a CUDA runtime/driver call failed                                */
 #define TB200_ERR_NOMEM (-4)
 #define TB200_ERR_UNSUPPORTED (-5) /* op/dtype not implemented on device (caller must keep it on CPU)  */
@@ -141,7 +141,7 @@ typedef struct tb200_graph tb200_graph;     /* one per Tengine subgraph (subgrap
 /* ---- library / device ---------------------------------------------------------------------------- */
 TB200_API int tb200_abi_version(void);
 TB200_API const char* tb200_last_error(void);
-/* number of visible sm_100 devices (0 if none; never fails) */
+/* number of visible sm_90 devices (0 if none; never fails) */
 TB200_API int tb200_device_count(void);
 
 /* interface->init / release_device (source/device/device.h:44,65): bind one GPU. */
@@ -211,7 +211,7 @@ TB200_API int tb200_graph_postrun(tb200_graph* g);
  * batch is sharded over several GPUs (SURVEY.md 8(e)); identical layout on every rank for identical graphs. */
 TB200_API int tb200_graph_weight_arena(tb200_graph* g, void** device_ptr, size_t* bytes);
 
-/* On-box peak of the int8 tensor pipe in TOP/s: a pure tcgen05.mma kind::i8 loop (128 x 256 x 32, one CTA per SM), the measured
+/* On-box peak of the int8 tensor pipe in TOP/s: a pure wgmma m64n128k32 s8 loop (two warpgroups per SM), the measured
  * denominator of the tensor roofline that bench.py reports for compute-bound kernel families (SURVEY.md 8(d)). */
 TB200_API int tb200_probe_int8_tops(tb200_context* ctx, double* tops);
 
@@ -309,8 +309,8 @@ TB200_API int tb200k_conv_dw3x3(const void* in, const void* weight, void* out, c
  * network input; it also performs the NCHW->NHWC conversion of the graph input. */
 TB200_API int tb200k_conv_stem_nchw(const void* in_nchw, const void* weight, void* out, const tb200k_conv_shape* s,
                                     const tb200k_epilogue* e, void* stream);
-/* 1x1 convolution / FC as a tcgen05 (UMMA kind::i8) GEMM: out[M][Cout_pad] = in[M][K_pad] . weight[Cout_pad][K_pad]^T,
- * TMA-staged operands, TMEM accumulators, fused requantising epilogue.  Takes the role of
+/* 1x1 convolution / FC as a wgmma (s8 / u8) GEMM: out[M][Cout_pad] = in[M][K_pad] . weight[Cout_pad][K_pad]^T,
+ * TMA-staged operands, a shared-memory accumulator image, fused requantising epilogue.  Takes the role of
  * im2col + sgemm_i8 + sgemm_int8 epilogue (conv_kernel_x86.c:187,1008,1796) for kernel 1x1. */
 TB200_API int tb200k_gemm_i8(const void* in, const void* weight, void* out, int64_t m, int32_t k_pad, int32_t oc,
                              const tb200k_epilogue* e, void* stream);

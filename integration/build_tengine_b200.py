@@ -2,10 +2,10 @@
 """Integration build (test/demo infrastructure, not part of the product package): the reference Tengine library WITH the B200 device compiled in, exactly as its CMake would do for
 `source/device/b200/` + one `_REGISTER_DEVICE_LIST` entry (source/device/CMakeLists.txt:63-188), but driven by gcc directly.
 
-  build/tengine/libtengine-lite.so            reference objects (oracle/_ref/obj, untouched sources) + b200_device.cc
+  oracle/_ref/tengine/libtengine-lite.so            reference objects (oracle/_ref/obj, untouched sources) + b200_device.cc
                                               + source/api/c_api.c recompiled against a generated device/register.h that also lists
                                               register_b200_device()
-  build/tengine/tm_classification_int8, tm_classification_uint8, tm_benchmark   the UNMODIFIED apps, linked against it
+  oracle/_ref/tengine/tm_classification_int8, tm_classification_uint8, tm_benchmark   the UNMODIFIED apps, linked against it
 
 Needs /root/reference (headers + sources are compiled where they lie; nothing is copied into this repo).
 c_api.c, c_api.h, the serializer, examples/ and benchmark/ are byte-identical to the reference.
@@ -20,7 +20,7 @@ HERE = os.path.join(ROOT, "tengine_b200", "device")  # the device sources (would
 sys.path.insert(0, ROOT)
 from oracle import build_ref as br  # noqa: E402
 
-OUT = os.path.join(ROOT, "build", "tengine")
+OUT = os.path.join(ROOT, "oracle", "_ref", "tengine")
 
 
 def main(ref="/root/reference"):

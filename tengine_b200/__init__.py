@@ -1,4 +1,4 @@
-"""tengine_b200 -- B200 (sm_100a) int8/uint8 convolution + GEMM device backend for Tengine.
+"""tengine_b200 -- H100 (sm_90a) int8/uint8 convolution + GEMM device backend for Tengine.
 
 The product is the C-ABI library `libtengine_b200.so` (include/tengine_b200.h) built from tengine_b200/csrc/
 and the C++ Tengine device glue under tengine_b200/device/.  This package only loads that library for the

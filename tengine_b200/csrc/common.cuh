@@ -1,4 +1,4 @@
-// common.cuh -- device-side numerics shared by every kernel of the B200 backend.
+// common.cuh -- device-side numerics shared by every kernel of the H100 backend.
 //
 // The requantising epilogue reproduces the reference CPU device's float arithmetic operation for
 // operation (no FMA contraction, IEEE division, C round() = half away from zero), so that int8 results are
@@ -142,19 +142,17 @@ static __device__ __noinline__ int requant(int32_t acc, int oc, const EpiParams&
 // error is harmless; prerun proves |t| < 32000 for every reachable accumulator, else the layer takes the exact path).
 // For FC the reference itself computes roundf(x*rq) and M = rq exactly, so t == t_ref.
 //
-// The epilogues are bound by the ALU pipe (FMNMX / PRMT / LOP3 / I2FP issue at one warp instruction per two cycles per
-// SM sub-partition; measured with tools/ubench/epi_ubench.cu), so the arithmetic is arranged to keep work off it:
-//   * the float chain runs on the FMA pipe as packed FFMA2 / FADD2 (two channels per instruction),
+// The epilogues are bound by the issue rate of integer / logic instructions, so the arithmetic is arranged to keep work off them:
+//   * the float chain runs on the FMA pipe (channel pairs carried in one 64-bit value),
 //   * both clamps + the zero point are ONE DPX instruction per channel pair (VIADDMNMX.S16x2.RELU),
 //   * the tie guard is a 3-input FMNMX tree and one FSETP per 4 channels.
-// ALU-pipe instructions per element: 3.0 (was 5.75 with scalar FMNMX clamps and per-element guards).
 #define TB200_MAGIC 12582912.0f       // 1.5 * 2^23
 #define TB200_MAGIC_BITS 0x4B400000   // its bit pattern: as_float(MAGIC_BITS + i) == MAGIC + i for |i| < 2^22
 #ifndef TB200_TIE_EPS // (tools/build_nofix_lib.sh overrides it to measure what the rare path costs; never in the product build)
 #define TB200_TIE_EPS 1.220703125e-4f // 2^-13
 #endif
 
-// ---- packed fp32 pairs (sm_100 FFMA2 / FADD2 / FMUL2) ----
+// ---- fp32 pairs in one 64-bit value (two lanes, each rounded to nearest like the scalar instruction) ----
 __device__ __forceinline__ uint64_t f2_pack(float lo, float hi)
 {
     uint64_t r;
@@ -165,27 +163,27 @@ __device__ __forceinline__ void f2_unpack(uint64_t v, float& lo, float& hi) { as
 __device__ __forceinline__ void f2_unpack_bits(uint64_t v, uint32_t& lo, uint32_t& hi) { asm("mov.b64 {%0, %1}, %2;" : "=r"(lo), "=r"(hi) : "l"(v)); }
 __device__ __forceinline__ uint64_t f2_fma(uint64_t a, uint64_t b, uint64_t c)
 {
-    uint64_t r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
+    float a0, a1, b0, b1, c0, c1;
+    f2_unpack(a, a0, a1), f2_unpack(b, b0, b1), f2_unpack(c, c0, c1);
+    return f2_pack(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 __device__ __forceinline__ uint64_t f2_mul(uint64_t a, uint64_t b)
 {
-    uint64_t r;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
+    float a0, a1, b0, b1;
+    f2_unpack(a, a0, a1), f2_unpack(b, b0, b1);
+    return f2_pack(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
 __device__ __forceinline__ uint64_t f2_add(uint64_t a, uint64_t b)
 {
-    uint64_t r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
+    float a0, a1, b0, b1;
+    f2_unpack(a, a0, a1), f2_unpack(b, b0, b1);
+    return f2_pack(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
 }
 __device__ __forceinline__ uint64_t f2_sub(uint64_t a, uint64_t b)
 {
-    uint64_t r;
-    asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
+    float a0, a1, b0, b1;
+    f2_unpack(a, a0, a1), f2_unpack(b, b0, b1);
+    return f2_pack(__fsub_rn(a0, b0), __fsub_rn(a1, b1));
 }
 
 // Per-channel constants of four consecutive channels oc0..oc0+3 (oc0 % 4 == 0) in the arena's int8 layout: channel
@@ -243,7 +241,6 @@ __device__ __forceinline__ uint32_t requant_fast4_i8(const int32_t (&acc)[4], co
 // independent neighbours.  ptxas on its own schedules the chains one after the other, and with only four epilogue warps
 // per scheduler the fixed-latency stalls then halve the issue rate (ncu: stall_wait 2.2 per issue).
 // w0/w1: the two packed words (before requant_byte_fix); g0/g1: max |d| of each word for the tie guard.
-#define TB200_F2V(op, d, a, b) asm volatile(op " %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b))
 template <bool FUSE>
 __device__ __forceinline__ void requant_fast8_i8(const int32_t (&a)[8], const float4 (&p)[4], const EpiParams& e, uint32_t& w0, uint32_t& w1,
                                                  float& g0, float& g1)
@@ -259,15 +256,15 @@ __device__ __forceinline__ void requant_fast8_i8(const int32_t (&a)[8], const fl
 #pragma unroll
     for (int k = 0; k < 4; k++)
     {
-        if (FUSE) asm volatile("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(t[k]) : "l"(x[k]), "l"(f2_pack(p[k].x, p[k].y)), "l"(f2_pack(p[k].z, p[k].w)));
-        else TB200_F2V("mul.rn.f32x2", t[k], x[k], f2_pack(p[k].x, p[k].y));
+        if (FUSE) t[k] = f2_fma(x[k], f2_pack(p[k].x, p[k].y), f2_pack(p[k].z, p[k].w));
+        else t[k] = f2_mul(x[k], f2_pack(p[k].x, p[k].y));
     }
 #pragma unroll
-    for (int k = 0; k < 4; k++) TB200_F2V("add.rn.f32x2", r[k], t[k], mg);
+    for (int k = 0; k < 4; k++) r[k] = f2_add(t[k], mg);
 #pragma unroll
-    for (int k = 0; k < 4; k++) TB200_F2V("sub.rn.f32x2", s[k], r[k], mg);
+    for (int k = 0; k < 4; k++) s[k] = f2_sub(r[k], mg);
 #pragma unroll
-    for (int k = 0; k < 4; k++) TB200_F2V("sub.rn.f32x2", d[k], t[k], s[k]);
+    for (int k = 0; k < 4; k++) d[k] = f2_sub(t[k], s[k]);
     float dl[4], dh[4];
     uint32_t rl[4], rh[4];
 #pragma unroll
@@ -386,17 +383,17 @@ __device__ __forceinline__ void requant_fast8_u8(const int32_t (&a)[8], const fl
     const uint64_t S2 = f2_pack(e.in_w_scale, e.in_w_scale), R2 = f2_pack(e.fast_r, e.fast_r);
     uint64_t f[4], t[4], r[4], s[4], d[4];
 #pragma unroll
-    for (int k = 0; k < 4; k++) TB200_F2V("mul.rn.f32x2", f[k], f2_pack((float)a[2 * k], (float)a[2 * k + 1]), S2);
+    for (int k = 0; k < 4; k++) f[k] = f2_mul(f2_pack((float)a[2 * k], (float)a[2 * k + 1]), S2);
 #pragma unroll
-    for (int k = 0; k < 4; k++) TB200_F2V("add.rn.f32x2", f[k], f[k], f2_pack(bt[2 * k], bt[2 * k + 1]));
+    for (int k = 0; k < 4; k++) f[k] = f2_add(f[k], f2_pack(bt[2 * k], bt[2 * k + 1]));
 #pragma unroll
-    for (int k = 0; k < 4; k++) TB200_F2V("mul.rn.f32x2", t[k], f[k], R2);
+    for (int k = 0; k < 4; k++) t[k] = f2_mul(f[k], R2);
 #pragma unroll
-    for (int k = 0; k < 4; k++) TB200_F2V("add.rn.f32x2", r[k], t[k], mg);
+    for (int k = 0; k < 4; k++) r[k] = f2_add(t[k], mg);
 #pragma unroll
-    for (int k = 0; k < 4; k++) TB200_F2V("sub.rn.f32x2", s[k], r[k], mg);
+    for (int k = 0; k < 4; k++) s[k] = f2_sub(r[k], mg);
 #pragma unroll
-    for (int k = 0; k < 4; k++) TB200_F2V("sub.rn.f32x2", d[k], t[k], s[k]);
+    for (int k = 0; k < 4; k++) d[k] = f2_sub(t[k], s[k]);
     float dl[4], dh[4];
     uint32_t rl[4], rh[4];
 #pragma unroll

@@ -2,15 +2,15 @@
 //
 // The layers an implicit GEMM over 4-D TMA boxes serves badly: the NCHW network input (C <= 3; 3x3 and 7x7 stems, int8 and
 // uint8) and 3x3 convolutions over NHWC tensors with 16 or 32 channels (YOLOv3-tiny's second and third layer).  Their K rows
-// are 16-32 bytes per tap, and the TMA unit's cost is per row, not per byte (DESIGN.md section 5): feeding nine shifted
+// are 16-32 bytes per tap, and the TMA unit's cost is per row, not per byte: feeding nine shifted
 // 128-row boxes per tile through it left the tensor pipe idle 90% of the time, and gathering every tap from global memory
 // with bounds predicates (round 1's conv_gather_tc_kernel) cost more instructions than the whole epilogue.
 //
 // Here a CTA (128 threads = 16 x 8 output pixels) receives the input window of its tile ONCE -- one 4-D cp.async.bulk.tensor
 // load, double-buffered, out-of-image coordinates zero-filled by the TMA unit = the convolution's padding -- and every thread
 // builds its pixel's K bytes from shared memory (NHWC: one 16-byte LDS/STS pair per tap and 16 channels; NCHW: byte loads
-// packed with IMADs) as one row of `ks` SW32 K-major k-step tiles.  One thread issues ks tcgen05.mma (128 x OCp x 32), every
-// thread requantises its own TMEM lane and stores OCp contiguous bytes.  uint8: border tiles first overwrite the window's
+// packed with IMADs) as one row of `ks` SW32 K-major k-step tiles.  The warpgroup multiplies them with wgmma (64 x 16 x 32
+// per instruction) into a shared-memory accumulator image; every thread requantises its own row and stores OCp contiguous bytes.  uint8: border tiles first overwrite the window's
 // out-of-image bytes with the input zero point (such taps then contribute (zx-zx)(w-zw) = 0, exactly like the reference,
 // which skips them), each thread sums its own row with dp4a, and sum (x-zx)(w-zw) = acc - zw*sum(x) + corr[oc].
 // Takes the role of im2col + sgemm of conv_hcl_run (source/device/cpu/op/conv/x86/conv_kernel_x86.c:124-242, 1008-1631) and of
@@ -35,7 +35,6 @@ struct WindowArgs
     unsigned ntiles;
     int tiles_w, tiles_h;
     uint32_t tw_magic, th_magic; // floor(2^32 / d) + 1: q = umulhi(x, magic) is x / d for the tile counts that occur (checked by the launcher)
-    uint32_t idesc, tmem_cols;
     int box_w, box_h, xoff, in_bytes, ks;
     uint32_t fill; // uint8: the input zero point replicated x4 (0 for int8: the TMA zero fill already is the padding)
 };
@@ -52,22 +51,15 @@ __global__ void __launch_bounds__(128) conv_window_tc_kernel(const __grid_consta
     const uint32_t sA = smem_u32(sm), sB = sA + (uint32_t)a.ks * 4096u, b_tile = (uint32_t)a.ocp * 32u, sPar = sB + (uint32_t)a.ks * b_tile;
     const uint32_t in_stride = ((uint32_t)a.in_bytes + 127u) & ~127u;
     const uint32_t sIn = (sPar + (uint32_t)a.ocp * 8u + 127u) & ~127u;
-    __shared__ __align__(8) uint64_t mma_done;
+    const uint32_t pitch = acc_pitch(a.ocp), sImg = sIn + 2u * in_stride; // accumulator image [128][pitch]
     __shared__ __align__(8) uint64_t in_full[2];
-    __shared__ uint32_t tmem_slot;
-    const int tid = threadIdx.x, warp = tid >> 5;
+    const int tid = threadIdx.x;
     const int tw = tid & 15, th = tid >> 4; // the tile is 16 x 8 output pixels
 
     if (tid == 0)
     {
-        mbar_init(&mma_done, 1);
         mbar_init(&in_full[0], 1), mbar_init(&in_full[1], 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 0)
-    {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)), "r"(a.tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
     }
     __syncthreads();
     auto tile_coords = [&](unsigned tile, int& n, int& oh0, int& ow0)
@@ -103,7 +95,7 @@ __global__ void __launch_bounds__(128) conv_window_tc_kernel(const __grid_consta
     for (int c = tid; c < a.ocp; c += 128) sts_f2(sPar + c * 8, (MODE != 2 || U8) ? __ldg(e.fast_par + c) : make_float2(0.f, 0.f));
     if (LAYOUT == 2) sts_u4(sA + 4u * 4096u + sw32_offset(tid, 1), 0u, 0u, 0u, 0u); // K = 144 of 160: the last half k-step stays 0
 
-    uint32_t phase = 0, it = 0;
+    uint32_t it = 0;
     for (unsigned tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x, it++)
     {
         int n, oh0, ow0;
@@ -207,31 +199,20 @@ __global__ void __launch_bounds__(128) conv_window_tc_kernel(const __grid_consta
             }
         }
         fence_proxy_async_smem(); // the MMAs read these generic-proxy writes through the async proxy
-        tcgen05_fence_before();
-        __syncthreads(); // (first iteration: also publishes the TMEM address, the B tiles and the constants)
-        tcgen05_fence_after();
-        const uint32_t tmem_base = tmem_slot;
-        if (tid == 0)
-        {
-            // everybody has read this tile's window: prefetch the next one into the other buffer
-            if (tile + gridDim.x < a.ntiles) TB200_WIN_LOAD_TILE(tile + gridDim.x, (it + 1) & 1);
-            for (int kb = 0; kb < a.ks; kb++)
-                umma_i8(tmem_base, make_smem_desc(sA + (uint32_t)kb * 4096u, 32), make_smem_desc(sB + (uint32_t)kb * b_tile, 32), a.idesc, kb ? 1u : 0u);
-            tcgen05_commit(&mma_done);
-        }
-        mbar_wait(&mma_done, phase);
-        phase ^= 1;
-        tcgen05_fence_after();
+        __syncthreads();          // (first iteration: also publishes the B tiles and the constants)
+        // everybody has read this tile's window: prefetch the next one into the other buffer
+        if (tid == 0 && tile + gridDim.x < a.ntiles) TB200_WIN_LOAD_TILE(tile + gridDim.x, (it + 1) & 1);
+        wg_mma_to_image<U8, U8>(sA, 4096u, sB, b_tile, a.ks, 32, a.ocp, sImg, pitch);
+        __syncthreads();
 
-        // ---- epilogue: lane = pixel, 16 channels per TMEM load, OCp contiguous output bytes per pixel ----
+        // ---- epilogue: thread = pixel = accumulator row, 16 channels per load, OCp contiguous output bytes per pixel ----
         uint8_t* op = a.out + (size_t)pix * a.ocp;
-        const uint32_t tb = tmem_base + ((uint32_t)(warp * 32) << 16);
+        const uint32_t tb = sImg + (uint32_t)tid * pitch;
         const int32_t rowc = U8 ? -e.w_zero * sx : 0;
         for (int c = 0; c < a.ocp; c += 16)
         {
             uint32_t v[16];
-            tmem_ld16(tb + c, v);
-            tmem_ld_wait();
+            acc_ld16(tb + 4u * c, v);
             uint32_t w[4];
             if (U8)
             {
@@ -307,21 +288,26 @@ __global__ void __launch_bounds__(128) conv_window_tc_kernel(const __grid_consta
                 stem_unit_fast<MODE == 1>(v, sPar + c * 8, c, e, w);
             if (valid) *reinterpret_cast<uint4*>(op + c) = make_uint4(w[0], w[1], w[2], w[3]);
         }
-        // the next tile's MMAs overwrite the accumulator and its gather overwrites the A tiles (these MMAs have completed)
-        tcgen05_fence_before();
+        // the next tile's MMAs overwrite the accumulator image and its gather overwrites the A tiles
         __syncthreads();
     }
 #undef TB200_WIN_LOAD_TILE
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 0)
-    {
-        tcgen05_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_slot), "r"(a.tmem_cols) : "memory");
-    }
 }
 
 // ---- host side ------------------------------------------------------------------------------------------------------------
+static constexpr int WINDOW_SMEM_MAX = 200 * 1024;
+
+// shared memory of one CTA: A tiles, B tiles, constants, the double-buffered input window, the accumulator image
+static int window_smem_bytes(int ks, int ocp, int in_bytes)
+{
+    return ks * 4096 + ks * ocp * 32 + ocp * 8 + 128 + 2 * ((in_bytes + 127) & ~127) + 128 * (int)acc_pitch(ocp) + 1024;
+}
+
+bool window_nhwc_fits(int cp, int ocp, int stride)
+{
+    const int box_w = 15 * stride + 3, box_h = 7 * stride + 3;
+    return window_smem_bytes((9 * cp + 31) / 32, ocp, box_w * box_h * cp) <= WINDOW_SMEM_MAX;
+}
 // nhwc == 0: `in` is the NCHW network input (C <= 3); the tensor map is (W, H, C, N) with box (box_w, box_h, C, 1).
 // nhwc == 1: `in` is an NHWC tensor with cp = 16 or 32 bytes per pixel; the map is (cp, W, H, N) with box (cp, box_w, box_h, 1).
 int window_plan_create(WindowPlan* p, const void* in, const ConvShape& s, int nhwc)
@@ -357,8 +343,8 @@ int window_plan_create(WindowPlan* p, const void* in, const ConvShape& s, int nh
         const uint32_t box[4] = {(uint32_t)p->box_w, (uint32_t)p->box_h, (uint32_t)s.c, 1u};
         if (tmap_encode(p->tmap_in, in, 4, dims, strides, box, nullptr, 0)) return -1;
     }
-    p->smem_bytes = p->ks * 4096 + p->ks * s.ocp * 32 + s.ocp * 8 + 128 + 2 * ((p->in_bytes + 127) & ~127) + 1024;
-    if (p->smem_bytes > 200 * 1024) return -1;
+    p->smem_bytes = window_smem_bytes(p->ks, s.ocp, p->in_bytes);
+    if (p->smem_bytes > WINDOW_SMEM_MAX) return -1;
     p->valid = 1;
     return 0;
 }
@@ -376,10 +362,6 @@ cudaError_t launch_conv_window(const WindowPlan& p, const void* w, void* out, co
     if ((unsigned long long)a.ntiles * (unsigned)a.tiles_w >= (1ull << 32) || (unsigned long long)a.ntiles * (unsigned)a.tiles_h >= (1ull << 32)) return cudaErrorInvalidValue;
     a.tw_magic = a.tiles_w == 1 ? 0u : (uint32_t)((1ull << 32) / (unsigned)a.tiles_w) + 1u;
     a.th_magic = a.tiles_h == 1 ? 0u : (uint32_t)((1ull << 32) / (unsigned)a.tiles_h) + 1u;
-    a.idesc = make_idesc_i8(s.ocp, !e.is_uint8, !e.is_uint8);
-    uint32_t cols = 32;
-    while (cols < (uint32_t)s.ocp) cols <<= 1;
-    a.tmem_cols = cols;
     a.box_w = p.box_w, a.box_h = p.box_h, a.xoff = p.xoff, a.in_bytes = p.in_bytes, a.ks = p.ks;
     a.fill = e.is_uint8 ? ((uint32_t)(e.in_zero & 0xff) * 0x01010101u) : 0u;
     static int sms = 0;
@@ -391,8 +373,6 @@ cudaError_t launch_conv_window(const WindowPlan& p, const void* w, void* out, co
     }
     // several resident CTAs per SM overlap gather / MMA / epilogue of different tiles; each loops over its share
     int per_sm = (220 * 1024) / p.smem_bytes;
-    const int by_tmem = 512 / (int)cols;
-    if (by_tmem < per_sm) per_sm = by_tmem;
     if (per_sm > 8) per_sm = 8;
     if (per_sm < 1) per_sm = 1;
     const unsigned cap = (unsigned)(sms * per_sm);
@@ -405,7 +385,7 @@ cudaError_t launch_conv_window(const WindowPlan& p, const void* w, void* out, co
     {                                                                                                                                       \
         /* the opt-in is per device AND per context: set it before every launch (launches happen at graph capture only) */ \
         {                                                                                                                                   \
-            cudaError_t err = cudaFuncSetAttribute(conv_window_tc_kernel<MD, U, LY>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); \
+            cudaError_t err = cudaFuncSetAttribute(conv_window_tc_kernel<MD, U, LY>, cudaFuncAttributeMaxDynamicSharedMemorySize, WINDOW_SMEM_MAX); \
             if (err != cudaSuccess) return err;                                                                                             \
         }                                                                                                                                   \
         conv_window_tc_kernel<MD, U, LY><<<grid, 128, (size_t)p.smem_bytes, st>>>(tm, a, e);                                                \

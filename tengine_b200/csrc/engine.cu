@@ -244,7 +244,10 @@ int tb200_device_count(void)
     for (int i = 0; i < n; i++)
     {
         int major = 0;
-        if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, i) == cudaSuccess && major == 10) good++;
+        int minor = -1;
+        if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, i) == cudaSuccess &&
+            cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, i) == cudaSuccess && major == 9 && minor == 0)
+            good++;
     }
     return good;
 }
@@ -255,14 +258,14 @@ static int context_create_one(int cuda_device, tb200_context** out)
     if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0)
     {
         cudaGetLastError();
-        return fail(TB200_ERR_NO_DEVICE, "no CUDA device visible: the B200 backend has no CPU fallback");
+        return fail(TB200_ERR_NO_DEVICE, "no CUDA device visible: the H100 backend has no CPU fallback");
     }
     if (cuda_device < 0 || cuda_device >= n) return fail(TB200_ERR_INVALID, "cuda device %d out of range (%d)", cuda_device, n);
     int major = 0, minor = 0, sms = 0;
     CUDA_OK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, cuda_device));
     CUDA_OK(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, cuda_device));
     CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, cuda_device));
-    if (major != 10) return fail(TB200_ERR_NO_DEVICE, "device %d is sm_%d%d; this backend is built for sm_100a only", cuda_device, major, minor);
+    if (major != 9 || minor != 0) return fail(TB200_ERR_NO_DEVICE, "device %d is sm_%d%d; this backend is built for sm_90a only", cuda_device, major, minor);
     CUDA_OK(cudaSetDevice(cuda_device));
     cudaStream_t st;
     CUDA_OK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
@@ -706,7 +709,7 @@ static int prerun_one(tb200_context* ctx, const tb200_tensor_desc* tensors, int 
         TensorInfo& t = g->tensors[i];
         t.d = tensors[i];
         if (t.d.data_type != TB200_DT_INT8 && t.d.data_type != TB200_DT_UINT8)
-            return bail(fail(TB200_ERR_UNSUPPORTED, "tensor %d: data type %d not supported by the B200 backend", i, t.d.data_type));
+            return bail(fail(TB200_ERR_UNSUPPORTED, "tensor %d: data type %d not supported by the H100 backend", i, t.d.data_type));
         for (int k = 0; k < 4; k++)
             if (t.d.dims[k] <= 0) return bail(fail(TB200_ERR_INVALID, "tensor %d: dim %d is %d", i, k, t.d.dims[k]));
         t.cp = cpad(t.d.dims[1]);
@@ -766,7 +769,7 @@ static int prerun_one(tb200_context* ctx, const tb200_tensor_desc* tensors, int 
             size_t wsize;
             if (tin.input_index >= 0 && C <= 3 && L.group == 1 && !u8 && !no_tc && L.kernel_h == 3 && L.kernel_w == 3 && L.dilation_h == 1 &&
                 L.dilation_w == 1 && L.stride_h == L.stride_w && tout.cp <= 256 && !getenv("TB200_NO_STEM_TC"))
-                kind[li] = K_STEM_TC, wsize = (size_t)tout.cp * 32; // one 32-byte UMMA k-step per output channel
+                kind[li] = K_STEM_TC, wsize = (size_t)tout.cp * 32; // one 32-byte wgmma k-step per output channel
             else if (tin.input_index >= 0 && C <= 3 && L.group == 1 && !no_tc && L.kernel_h == L.kernel_w && (L.kernel_h == 7 || (u8 && L.kernel_h == 3)) &&
                      L.dilation_h == 1 && L.dilation_w == 1 && L.stride_h == L.stride_w && tout.cp <= 256 && !getenv("TB200_NO_GATHER_TC"))
                 // uint8 3x3 stems and 7x7 stems (ResNet): threads gather, taps outside the image = zero point; K padded to 32*ks
@@ -778,7 +781,7 @@ static int prerun_one(tb200_context* ctx, const tb200_tensor_desc* tensors, int 
                 kind[li] = K_GATHER_TC, wsize = (size_t)tout.cp * 160; // 16-channel input: nine 16-byte taps per pixel, five k-steps
             else if (!no_tc && L.group == 1 && tin.cp == 32 && L.kernel_h == 3 && L.kernel_w == 3 && L.dilation_h == 1 &&
                      L.dilation_w == 1 && L.stride_h == L.stride_w && (L.stride_h == 1 || L.stride_h == 2) && tout.cp <= 256 &&
-                     !getenv("TB200_NO_GATHER_TC") && !getenv("TB200_NO_WINDOW_CONV"))
+                     window_nhwc_fits(32, tout.cp, L.stride_h) && !getenv("TB200_NO_GATHER_TC") && !getenv("TB200_NO_WINDOW_CONV"))
                 kind[li] = K_GATHER_TC, wsize = (size_t)tout.cp * 288; // 32-channel input through the window kernel: nine 32-byte taps = nine k-steps
             else if (L.group == C && OC == C && C > 1)
                 kind[li] = K_CONV_DW, wsize = (size_t)L.kernel_h * L.kernel_w * tin.cp;

@@ -1,5 +1,5 @@
-// gemm_tcgen05.cu -- int8 x int8 -> int32 GEMM on the 5th-generation tensor cores (tcgen05.mma kind::i8,
-// SASS UTCIMMA) with TMA-staged operands, TMEM accumulators and the fused requantising epilogue.
+// gemm_tcgen05.cu -- int8 x int8 -> int32 GEMM on the Hopper tensor cores (wgmma.mma_async .s32.s8/.u8, m64n16k32)
+// with TMA-staged operands, a shared-memory accumulator image and the fused requantising epilogue.
 //
 //   out[m][oc] = requant( sum_k A[m][k] * B[oc][k] ),   A = NHWC activations (row = pixel, K = padded Cin),
 //                                                        B = pre-packed weights [OCp][K], both K-major.
@@ -7,18 +7,18 @@
 // (source/device/cpu/op/conv/x86/conv_kernel_x86.c:187-242, 1008-1631, 1796-1893) and of ref_fc_int8
 // (fc/fc_ref.c:209-297): with NHWC activations a 1x1 convolution IS this GEMM, no im2col pass exists.
 //
-// Structure (one persistent CTA per SM, 576 threads):
+// Structure (one persistent CTA per SM, 544 threads):
 //   warp 16   : TMA producer  (cp.async.bulk.tensor.2d -> 128B/64B/32B-swizzled smem ring, mbarrier expect_tx)
-//   warp 17   : MMA issuer    (one elected lane: tcgen05.mma.cta_group::1.kind::i8, 128 x BN x 32 per instruction;
-//                              tcgen05.commit releases smem stages / publishes the accumulator)
-//   warps 0-15: epilogue      (four warps per TMEM lane quarter; a warp owns whole "store groups" = 32 rows x 16/32/64
-//                              channels: tcgen05.ld 32x32b -> registers -> requant_fast4_i8 -> bytes -> its own swizzled
-//                              smem buffer -> ONE TMA store per group (cp.async.bulk.tensor, double-buffered).  No
-//                              barrier between epilogue warps, no address arithmetic for the stores, rows outside
-//                              the tensor are clipped by the TMA unit.)
-// Two TMEM accumulator stages (2 x BN columns) let the MMAs of tile i+1 overlap the epilogue of tile i.
-// K is small (32..1024), so these layers are bound by the epilogue's ALU-pipe issue rate, not by the tensor pipe:
-// see common.cuh (requant_fast4_i8) for the instruction budget.
+//   warps 0-15: four warpgroups that first multiply, then requantise.  MMA: warpgroup w takes rows 64*(w & 1).. and one
+//               half of the N tile's 16-column chunks, issues wgmma per ring stage, releases the stage after
+//               wgmma.wait_group and finally writes its s32 fragments into the accumulator image ([128 rows][BN] in
+//               shared memory).  Epilogue: four warps per 32-row quarter of the image; a warp owns whole "store groups"
+//               = 32 rows x 16/32/64 channels: image -> registers -> requant_fast4_i8 -> bytes -> its own swizzled smem
+//               buffer -> ONE TMA store per group (cp.async.bulk.tensor, double-buffered).  No address arithmetic for the
+//               stores, rows outside the tensor are clipped by the TMA unit.
+// The producer runs ahead through the ring while the epilogue works, so the next tile's operands are resident when its
+// MMAs start.  K is small (32..1024), so these layers are bound by the epilogue's ALU-pipe issue rate, not by the tensor
+// pipe: see common.cuh (requant_fast4_i8) for the instruction budget.
 #include <cuda.h>
 
 #include "common.cuh"
@@ -38,15 +38,14 @@ namespace tb200 {
 #endif
 
 
-static constexpr int EPI_WARPS = 16; // four per TMEM lane quarter
+static constexpr int EPI_WARPS = 16; // four warpgroups; four warps per 32-row quarter of the accumulator image
 static constexpr int EPI_THREADS = EPI_WARPS * 32;
-static constexpr int GEMM_THREADS = 64 + EPI_THREADS;
-static constexpr int SUM_WARP0 = EPI_WARPS + 2, SUM_WARPS = 2; // uint8 kernels only: two warps that add up the rows of every A tile (sum x)
+static constexpr int GEMM_THREADS = 32 + EPI_THREADS;
+static constexpr int SUM_WARP0 = EPI_WARPS + 1, SUM_WARPS = 2; // uint8 kernels only: two warps that add up the rows of every A tile (sum x)
 static constexpr int GEMM_THREADS_U8 = GEMM_THREADS + 32 * SUM_WARPS;
-// The warp scheduler favours the highest warp id of a sub-partition (B300_MICROARCH: hi-wid-first arbiter).  The two
-// single-thread roles sit on the critical path of every hand-off, so they get the highest ids; measured with the CTA
-// timeline (tools/gemm_trace.py): as warps 0/1 each of their instructions waited ~13 cycles behind the epilogue warps.
-static constexpr int PRODUCER_WARP = EPI_WARPS, MMA_WARP = EPI_WARPS + 1;
+static constexpr int PRODUCER_WARP = EPI_WARPS;
+static constexpr int ACC_COLS_MAX = 144; // columns of the accumulator image (m-tiles per stage x B tile rows)
+static constexpr int MMA_CHUNKS = 5;     // 16-column chunks of one warpgroup: half of at most 144 columns
 static constexpr int PAR_MAX = 2048; // channels whose epilogue constants stay resident in smem for the whole kernel
 static constexpr int MAX_STAGES = 24;
 static constexpr int B_RESIDENT_MAX = 96 * 1024; // weights of the CTA's N tile stay in smem when they fit in this many bytes
@@ -74,27 +73,22 @@ struct GemmArgs
     int mt;     // m-tiles (128 rows each) per accumulator stage
     uint32_t bw_rcp, bh_rcp; // ceil(65536/d): q = (x * rcp) >> 16 is exact for x < 4096, d <= 256
     int oc, ocp;
-    uint32_t idesc;
-    uint32_t tmem_cols;
     // conv mode (implicit GEMM): an m-tile is a bw x bh x bn patch of output pixels, a k-block is (tap, channel block)
     int conv, cblocks, kw_n, pad_h, pad_w, cstride, cp;
     int bw, bh, bn, tiles_w, tiles_h, oh, ow, nimg;
     uint32_t a_tx_bytes; // bytes one A load delivers (block_k * rows of the patch)
     // uint8 (unsigned A): B holds w - 128 as int8 (plain w when zw == 0), so the accumulator is sum x*(w - 128); what is left of
-    // sum x*(w - zw) is cplane * sum(x) with cplane = 128 - zw.  sum(x) of each pixel comes from a second, 16-column MMA per k-step
-    // against a constant tile of ones into 16 extra TMEM columns (8 tensor cycles), and the epilogue adds cplane * sum(x) inside the
-    // IADD3 that also adds the per-channel constant.  (A full-width second MMA against a constant tile of value 128 - zw, which
-    // would leave the epilogue identical to int8's, was measured 2.4x slower on the K = 64 layers: profiles/r02 notes.)
+    // sum x*(w - zw) is cplane * sum(x) with cplane = 128 - zw, and the epilogue adds cplane * sum(x) inside the IADD3 that also
+    // adds the per-channel constant.
     int u8, bnx, taps, in_h, in_w, b_signed, cplane;
     int sx_mode; // where sum(x) comes from when cplane != 0: 3 = two extra warps add up the rows of every A tile in shared memory (default), 0 = 16 rows of ones inside every B tile (TB200_U8_SX=0)
-    int tcols; // TMEM columns per m-tile: bnx, + 16 when a second, 16-column MMA against a tile of ones forms sum(x) (cplane != 0)
+    int tcols; // accumulator image columns per m-tile: bnx (block_n, + 16 when 16 rows of ones in B form sum(x))
     // epilogue / stores
     int cs, ngroups; // 16-column chunks per store group (1, 2 or 4) and groups per m-tile
     int rows_valid;  // rows of an m-tile that are output pixels (128, or bw*bh*bn of a smaller conv patch)
     int out_mode;    // coordinates of the output map: 0 (c, row, 0)  1 (c, pixel in image, image)  2 (c, x, image row)
     int par_all;     // the constants of every channel are resident (loaded once); else reloaded per N tile
     int b_res;       // the N tile's weights (all k-blocks) are loaded once and stay in smem; the ring carries A only
-    int teams;       // the epilogue warps form two teams, one per accumulator stage (see the epilogue)
     // deferred rare path: a guarded element is queued {m-tile, row, channel, accumulator} and recomputed literally by all threads of the
     // CTA after its last tile, instead of holding up its epilogue warp (and with it the accumulator stage); null = inline
     uint4* fixq;
@@ -119,9 +113,7 @@ struct __align__(16) GemmSmemCtl
 {
     uint64_t full[MAX_STAGES], empty[MAX_STAGES];
     uint64_t b_full; // resident-B mode: all k-blocks of the N tile's weights have landed
-    uint64_t tmem_full[2], tmem_empty[2];
-    uint32_t tmem_base;
-    uint32_t pad[3];
+    uint64_t sx_full[2], sx_empty[2]; // uint8 row sums of stage s published by the row-sum warps / read by the epilogue
 };
 
 __device__ __forceinline__ void epilogue_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory"); }
@@ -129,8 +121,7 @@ __device__ __forceinline__ void epilogue_bar_sync() { asm volatile("bar.sync 1, 
 // ---- the rare path of the fast epilogue, deferred -----------------------------------------------------------------------------
 // An element whose t sits inside the tie guard needs the literal reference arithmetic (common.cuh requant(): divisions, per-channel
 // loads, every recipe).  Done inline it occupies ONE lane of an epilogue warp for hundreds of cycles while the other fifteen warps
-// finish their groups and then wait for it at the accumulator hand-over: with ~7 guarded words per 128 x 256 stage this was 16-20 %
-// of the GEMM time (profiles/r02_rare_path.txt).  Instead the lane appends {m-tile, row, channel, accumulator} to the CTA's queue in
+// finish their groups and then wait for it at the stage hand-over.  Instead the lane appends {m-tile, row, channel, accumulator} to the CTA's queue in
 // global memory (L2) and carries on with the fast byte; after the CTA's last tile all 512 epilogue threads recompute the queued
 // elements in parallel and patch the bytes in the output tensor (the tile's TMA store has completed by then).  A full or absent
 // queue falls back to the inline computation, so the result never depends on the queue.
@@ -149,7 +140,7 @@ __device__ __forceinline__ bool fixq_push(uint32_t mtile, int oc, int32_t acc)
     if (!s_fixq.q) return false;
     const uint32_t slot = atomicAdd(&s_fixq.count, 1u);
     if (slot >= s_fixq.cap) return false;
-    const uint32_t row = ((threadIdx.x >> 5) & 3u) * 32u + (threadIdx.x & 31u); // TMEM lane of this thread = row of the m-tile
+    const uint32_t row = ((threadIdx.x >> 5) & 3u) * 32u + (threadIdx.x & 31u); // image row of this thread = row of the m-tile
     s_fixq.q[slot] = make_uint4(mtile, row | ((uint32_t)oc << 8), (uint32_t)acc, 0u);
     return true;
 }
@@ -390,9 +381,11 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
     const uint32_t stg_base = smem_u32(stg);
     GemmSmemCtl* ctl = reinterpret_cast<GemmSmemCtl*>(stg + (size_t)(CS == 8 ? EPI_WARPS / 2 : EPI_WARPS) * 2 * buf_bytes);
     const uint32_t par_base = smem_u32(ctl) + (uint32_t)sizeof(GemmSmemCtl); // [par channels] x 8 bytes (see FastPar4)
+    const int acc_cols = g.mt * g.tcols; // accumulator image columns of one stage
+    const uint32_t img_pitch = acc_pitch(acc_cols);
+    const uint32_t img_base = (par_base + (uint32_t)(g.par_all ? g.n_tiles * g.block_n : g.block_n) * 8u + 15u) & ~15u;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int acc_cols = g.mt * g.tcols; // TMEM columns of one accumulator stage
     // debug timeline: CTA 0 only, 4 logs x 1024 events of (clock << 8 | tag); plain global stores, no atomics
 #ifdef TB200_GEMM_TIMELINE
     int tl_n = 0;
@@ -407,24 +400,13 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
     if (threadIdx.x == 0)
     {
         const uint32_t sumw = (U8 && g.sx_mode == 3) ? SUM_WARPS : 0; // the row-sum warps read every operand stage and publish with the accumulators
-        for (int s = 0; s < g.stages; s++) mbar_init(&ctl->full[s], 1), mbar_init(&ctl->empty[s], 1 + sumw);
-        for (int s = 0; s < 2; s++) mbar_init(&ctl->tmem_full[s], 1 + sumw), mbar_init(&ctl->tmem_empty[s], g.teams ? EPI_WARPS / 2 : EPI_WARPS);
+        for (int s = 0; s < g.stages; s++) mbar_init(&ctl->full[s], 1), mbar_init(&ctl->empty[s], EPI_WARPS + sumw);
+        for (int s = 0; s < 2; s++) mbar_init(&ctl->sx_full[s], sumw ? sumw : 1), mbar_init(&ctl->sx_empty[s], EPI_WARPS);
         mbar_init(&ctl->b_full, 1);
         s_fixq.q = g.fixq ? g.fixq + (size_t)blockIdx.x * g.fixq_cap : nullptr, s_fixq.cap = (uint32_t)g.fixq_cap, s_fixq.count = 0;
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 0)
-    {
-        // TMEM allocation: one warp, power-of-two columns >= 32; base address is written to shared memory
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&ctl->tmem_base)),
-                     "r"(g.tmem_cols)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = ctl->tmem_base;
 
     if (warp == PRODUCER_WARP)
     {
@@ -486,46 +468,6 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
             }
         }
     }
-    else if (warp == MMA_WARP)
-    {
-        // ===================== MMA issuer =====================
-        if (lane == 0)
-        {
-            int stage = 0;
-            uint32_t phase = 0;
-            int as = 0;
-            uint32_t aphase = 0;
-            if (g.b_res) mbar_wait(&ctl->b_full, 0);
-            for (int st = blockIdx.x; st < g.num_super; st += gridDim.x)
-            {
-                const int mt0 = (st / g.n_tiles) * g.mt;
-                mbar_wait(&ctl->tmem_empty[as], aphase ^ 1); // the epilogue has drained this accumulator stage
-                tlog(1, 1);
-                tcgen05_fence_after();
-                for (int i = 0; i < g.mt && mt0 + i < g.m_tiles; i++)
-                {
-                    const uint32_t tmem_d = tmem_base + (uint32_t)(as * acc_cols + i * g.tcols);
-                    for (int kb = 0; kb < g.k_blocks; kb++)
-                    {
-                        mbar_wait(&ctl->full[stage], phase); // TMA bytes have landed
-                        tcgen05_fence_after();
-                        const uint32_t sa = smem_u32(smem + (size_t)stage * stage_bytes);
-                        const uint32_t sb = g.b_res ? smem_u32(b_region) + (uint32_t)kb * b_al : sa + a_bytes;
-                        const uint64_t da = make_smem_desc(sa, g.swizzle), db = make_smem_desc(sb, g.swizzle);
-                        for (int k = 0; k < g.block_k / 32; k++)
-                            // advance 32 bytes (one UMMA_K of int8) inside the swizzled row: +2 in 16-byte units
-                            umma_i8(tmem_d, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), g.idesc, (kb | k) ? 1u : 0u);
-                        tcgen05_commit(&ctl->empty[stage]); // smem stage reusable once these MMAs have read it
-                        tlog(1, 0);
-                        if (++stage == g.stages) stage = 0, phase ^= 1;
-                    }
-                }
-                tcgen05_commit(&ctl->tmem_full[as]); // all m-tiles of this accumulator stage are complete
-                tlog(1, 2);
-                if (++as == 2) as = 0, aphase ^= 1;
-            }
-        }
-    }
     else if (U8 && warp >= SUM_WARP0)
     {
         // ===================== row sums (uint8, warps 18 and 19) =====================
@@ -534,7 +476,7 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
         // does not care about the swizzle that permutes the 16-byte chunks inside a row.  Each of the two warps owns 64 rows (two per
         // lane), reads them with 16-byte loads (chunk order rotated per lane so that a quarter-warp covers all banks), dp4a against
         // 0x01010101, and publishes the sums through shared memory together with the accumulator stage.  This keeps the uint8 tiling
-        // identical to the int8 one: no extra B rows, no extra TMEM columns, no second MMA (DESIGN.md 5, measured alternatives).
+        // identical to the int8 one: no extra B rows, no extra accumulator columns, no second MMA.
         if (g.sx_mode == 3)
         {
             const int sw = warp - SUM_WARP0;
@@ -548,7 +490,7 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
             for (int st = blockIdx.x; st < g.num_super; st += gridDim.x)
             {
                 const int mt0 = (st / g.n_tiles) * g.mt;
-                mbar_wait(&ctl->tmem_empty[as], aphase ^ 1); // the epilogue has read this stage's sums
+                mbar_wait(&ctl->sx_empty[as], aphase ^ 1); // the epilogue has read this stage's sums
                 for (int i = 0; i < g.mt && mt0 + i < g.m_tiles; i++)
                 {
                     unsigned s0 = 0, s1 = 0;
@@ -574,22 +516,28 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
                     asm volatile("st.shared.b32 [%0], %1;" ::"r"(dst + 128u), "r"(s1) : "memory");
                 }
                 __syncwarp();
-                if (lane == 0) mbar_arrive(&ctl->tmem_full[as]); // (release) the sums of this stage are in shared memory
+                if (lane == 0) mbar_arrive(&ctl->sx_full[as]); // (release) the sums of this stage are in shared memory
                 if (++as == 2) as = 0, aphase ^= 1;
             }
         }
     }
     else
     {
-        // ===================== epilogue (warps 0..15) =====================
-        // TMEM lane quarter q (hardware rule: a warp may only touch lanes 32*(warp_id % 4)...) is served by the four
-        // warps {q, q+4, q+8, q+12}.  The work of an accumulator stage is cut into store groups (m-tile i, columns
-        // [grp*16*cs, (grp+1)*16*cs)) of 32 rows each, dealt round-robin to the quarter's warps.  A warp requantises
-        // its group chunk by chunk (16 columns per tcgen05.ld, the next chunk's load in flight), writes the bytes to
-        // its own swizzled staging buffer and hands the buffer to the TMA unit with one store.
+        // ===================== MMA + epilogue (warps 0..15) =====================
+        // Image quarter q (rows 32q..32q+31) is served by the four warps {q, q+4, q+8, q+12}.  The work of an accumulator
+        // stage is cut into store groups (m-tile i, columns [grp*16*cs, (grp+1)*16*cs)) of 32 rows each, dealt round-robin to
+        // the quarter's warps.  A warp requantises its group chunk by chunk (16 columns per load, the next chunk's load in
+        // flight), writes the bytes to its own swizzled staging buffer and hands the buffer to the TMA unit with one store.
         const int q = warp & 3;
         const int sub = warp >> 2;
         const int ngroups = g.ngroups;
+        // MMA share of this warpgroup (= sub): rows 64*mh.., chunks [c_lo, c_lo + c_n) of every B tile
+        const int mh = sub & 1, nch = g.tcols >> 4, chalf = (nch + 1) >> 1;
+        const int c_lo = (sub >> 1) ? chalf : 0, c_n = (sub >> 1) ? nch - chalf : chalf;
+        const uint32_t a_bytes_mma = BLOCK_M * g.block_k, b_al_mma = (g.bnx * g.block_k + 1023) & ~1023u;
+        int stage = 0;
+        uint32_t phase = 0;
+        if (g.b_res) mbar_wait(&ctl->b_full, 0);
         int qrows = g.rows_valid - q * 32; // rows of this quarter that are output pixels
         qrows = qrows < 0 ? 0 : (qrows > 32 ? 32 : qrows);
         const CUtensorMap* tm_out = (qrows == 32) ? &tmap_out : &tmap_out_tail;
@@ -601,11 +549,7 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
                             : CS == 4 ? (uint32_t)((lane >> 1) & 3) << 4
                                       : (CS == 2 ? (uint32_t)((lane >> 2) & 1) << 4 : 0u);
         const uint32_t row_off = (uint32_t)lane * 16u * CS;
-        // Two teams (g.teams): warps with sub 0,1 drain accumulator stage 0, warps with sub 2,3 stage 1, each warp taking every
-        // second group of its stage.  A warp then does twice the work per hand-over, and while one team waits for its stage to be
-        // refilled the other one is computing, instead of all sixteen warps idling through the same bubbles together.
-        const int team = sub >> 1;
-        const int gfirst = CS == 8 ? (sub >> 1) : (g.teams ? (sub & 1) : sub), gstep = (CS == 8 || g.teams) ? 2 : 4;
+        const int gfirst = CS == 8 ? (sub >> 1) : sub, gstep = CS == 8 ? 2 : 4;
         auto pair_sync = [&]() { asm volatile("bar.sync %0, 64;" ::"r"(2 + pair) : "memory"); };
         uint32_t ucount = 0; // groups this warp has stored (buffer parity)
         const int par_ch = g.n_tiles * g.block_n;
@@ -622,12 +566,6 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
         uint32_t aphase = 0;
         for (int st = blockIdx.x; st < g.num_super; st += gridDim.x)
         {
-            if (g.teams && as != team)
-            {
-                // the other team's stage
-                if (++as == 2) as = 0, aphase ^= 1;
-                continue;
-            }
             const int msup = st / g.n_tiles;
             const int mt0 = msup * g.mt;
             const int n0 = (st - msup * g.n_tiles) * g.block_n;
@@ -642,20 +580,55 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
                 epilogue_bar_sync();
                 par_s = par_base;
             }
-            mbar_wait(&ctl->tmem_full[as], aphase);
+            // ---- MMA: every m-tile of the stage into the accumulator image ----
+            epilogue_bar_sync(); // every warp has read the previous stage's image
+            for (int i = 0; i < mtc; i++)
+            {
+                uint32_t acc[MMA_CHUNKS][8];
+#pragma unroll
+                for (int j = 0; j < MMA_CHUNKS; j++)
+#pragma unroll
+                    for (int r = 0; r < 8; r++) acc[j][r] = 0;
+                for (int kb = 0; kb < g.k_blocks; kb++)
+                {
+                    mbar_wait(&ctl->full[stage], phase); // TMA bytes have landed
+                    const uint32_t sa = smem_u32(smem + (size_t)stage * stage_bytes);
+                    const uint32_t sb = g.b_res ? smem_u32(b_region) + (uint32_t)kb * b_al_mma : sa + a_bytes_mma;
+                    const uint64_t da = make_smem_desc(sa + (uint32_t)(mh * 64 * g.swizzle), g.swizzle);
+                    const uint64_t db = make_smem_desc(sb + (uint32_t)(c_lo * 16 * g.swizzle), g.swizzle);
+                    wgmma_fence();
+                    for (int k = 0; k < g.block_k / 32; k++)
+#pragma unroll
+                        for (int j = 0; j < MMA_CHUNKS; j++)
+                            if (j < c_n)
+                            {
+                                // +32 bytes along K inside the swizzled rows: +2 in 16-byte units; +16 rows of B: +16*swizzle bytes
+                                const uint64_t a_d = da + (uint64_t)(k * 2), b_d = db + (uint64_t)(j * g.swizzle + k * 2);
+                                if (U8 && !g.b_signed) wgmma_n16<true, true>(acc[j], a_d, b_d, 1u);
+                                else wgmma_n16<U8, false>(acc[j], a_d, b_d, 1u);
+                            }
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&ctl->empty[stage]); // this warp's MMAs have read the stage
+                    if (++stage == g.stages) stage = 0, phase ^= 1;
+                }
+#pragma unroll
+                for (int j = 0; j < MMA_CHUNKS; j++)
+                    if (j < c_n) frag_to_image(acc[j], img_base, img_pitch, mh * 64, i * g.tcols + (c_lo + j) * 16);
+            }
+            epilogue_bar_sync(); // the image is complete
+            if (U8 && g.sx_mode == 3) mbar_wait(&ctl->sx_full[as], aphase); // the row sums of this stage
             TLOG_E(0);
-            tcgen05_fence_after();
-            const uint32_t tbase = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * acc_cols);
+            const uint32_t tbase = img_base + (uint32_t)(q * 32 + lane) * img_pitch;
             if (qrows > 0)
             {
                 // groups of this warp: flattened index u = i * ngroups + grp, u = sub, sub + 4, ...
-                // (uint8: a packed FMUL2 / FADD2 epilogue -- 16 columns with spills, and 8 columns per tcgen05.ld without -- was measured
-                //  SLOWER than the scalar unit in this kernel: ResNet-50 uint8 b=512 1x1 layers 8.5 / 8.7 ms vs 7.0 ms, DESIGN.md)
                 uint32_t v0[16], v1[16];
                 int i = 0, grp = gfirst;
                 while (grp >= ngroups) grp -= ngroups, i++;
                 if (CS > 1 && i < mtc)
-                    tmem_ld16(tbase + i * g.tcols + grp * (CS * 16) + half * 64, reinterpret_cast<uint32_t(&)[16]>(v0));
+                    acc_ld16(tbase + 4u * (i * g.tcols + grp * (CS * 16) + half * 64), reinterpret_cast<uint32_t(&)[16]>(v0));
                 while (i < mtc)
                 {
                     int i2 = i, g2 = grp + gstep; // the group after this one
@@ -679,11 +652,11 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
                                 rowc = g.cplane * sx;
                             }
                             else
-                                rowc = g.cplane * (int32_t)tmem_ld1(tbase + i * g.tcols + g.block_n); // warp-collective TMEM load (ones rows in B)
+                                rowc = g.cplane * (int32_t)acc_ld1(tbase + 4u * (i * g.tcols + g.block_n)); // the column of the ones rows in B
                         }
                         if (BORDER) pad = padding_taps(g, mt0 + i, q * 32 + lane);
                     }
-                    const uint32_t tg = tbase + i * g.tcols + grp * (CS * 16) + half * 64;
+                    const uint32_t tg = tbase + 4u * (i * g.tcols + grp * (CS * 16) + half * 64);
                     const int cg0 = grp * (CS * 16); // first column of the group inside the N tile
                     const uint32_t sdst = buf + row_off;
                     auto unit = [&](const uint32_t (&v)[16], int k)
@@ -696,8 +669,7 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
                     };
                     if (CS == 1)
                     {
-                        tmem_ld16(tg, reinterpret_cast<uint32_t(&)[16]>(v0));
-                        tmem_ld_wait();
+                        acc_ld16(tg, reinterpret_cast<uint32_t(&)[16]>(v0));
                         unit(reinterpret_cast<const uint32_t(&)[16]>(v0), 0);
                     }
                     else
@@ -705,11 +677,10 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
 #pragma unroll
                         for (int k = 0; k < WCH; k++)
                         {
-                            tmem_ld_wait();
                             TLOG_E(3);
                             // the next chunk's accumulators are in flight while this one is requantised
-                            if (k + 1 < WCH) tmem_ld16(tg + (k + 1) * 16, reinterpret_cast<uint32_t(&)[16]>(*((k & 1) ? v0 : v1)));
-                            else if (i2 < mtc) tmem_ld16(tbase + i2 * g.tcols + g2 * (CS * 16) + half * 64, reinterpret_cast<uint32_t(&)[16]>(v0));
+                            if (k + 1 < WCH) acc_ld16(tg + (k + 1) * 64, reinterpret_cast<uint32_t(&)[16]>(*((k & 1) ? v0 : v1)));
+                            else if (i2 < mtc) acc_ld16(tbase + 4u * (i2 * g.tcols + g2 * (CS * 16) + half * 64), reinterpret_cast<uint32_t(&)[16]>(v0));
                             unit(reinterpret_cast<const uint32_t(&)[16]>(*((k & 1) ? v1 : v0)), k);
                             TLOG_E(4);
                         }
@@ -738,9 +709,8 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
                     i = i2, grp = g2;
                 }
             }
-            tcgen05_fence_before();
             __syncwarp();
-            if (lane == 0) mbar_arrive(&ctl->tmem_empty[as]); // accumulator drained: the MMA warp may overwrite it
+            if (lane == 0) mbar_arrive(&ctl->sx_empty[as]); // stage drained: the row-sum warps may overwrite its sums
             TLOG_E(2);
             if (++as == 2) as = 0, aphase ^= 1;
         }
@@ -753,22 +723,16 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
             fixq_drain<U8>(g, e);
         }
     }
-
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 0)
-    {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(g.tmem_cols) : "memory");
-    }
 }
 
 // ---- stem on the tensor cores ------------------------------------------------------------------------------
 // First convolution of a network: NCHW int8 input with C <= 3 channels (as the application hands it over), 3x3 filter,
-// any stride / padding -> NHWC output.  K = C*9 <= 27 is padded to ONE 32-byte UMMA k-step: the 128 threads of a CTA
-// each gather the 27 input bytes of one output pixel, write them as one row of a SW32 K-major A tile, one thread issues
-// a single tcgen05.mma (128 x OCp x 32), and every thread requantises "its" TMEM lane and writes OCp contiguous bytes.
+// any stride / padding -> NHWC output.  K = C*9 <= 27 is padded to ONE 32-byte wgmma k-step: the 128 threads of a CTA
+// each gather the 27 input bytes of one output pixel, write them as one row of a SW32 K-major A tile, the warpgroup
+// multiplies it (128 x OCp x 32) into the shared-memory accumulator image, and every thread requantises its own row and
+// writes OCp contiguous bytes.
 // Replaces ~290 dp4a per pixel of the CUDA-core stem kernel (kernels_direct.cu) by one MMA; the work left is the gather
-// (~80 instructions) and the epilogue.  Several CTAs per SM (5 KB smem, OCp TMEM columns each) overlap each other.
+// (~80 instructions) and the epilogue.  Several CTAs per SM overlap each other.
 // Takes the role of the first im2col + sgemm of conv_hcl_run (conv_kernel_x86.c:187-242).
 struct StemArgs
 {
@@ -777,7 +741,6 @@ struct StemArgs
     uint8_t* out;       // NHWC, OCp bytes per pixel
     int n, c, h, w_in, oh, ow, ocp, oc, stride, ph, pw;
     unsigned npix, ntiles;
-    uint32_t idesc, tmem_cols;
     int tiles_w, tiles_h, box_w, box_h, in_bytes; // TMA-staged input window (16 x 8 output pixels per tile)
     int xoff; // the window starts xoff bytes left of the first tap: the innermost TMA coordinate must be 16-byte aligned
 };
@@ -794,22 +757,15 @@ __global__ void __launch_bounds__(128) stem_tc_kernel(const __grid_constant__ CU
     const uint32_t sA = smem_u32(sm), sB = sA + 4096, sPar = sB + (uint32_t)a.ocp * 32u;
     const uint32_t in_stride = ((uint32_t)a.in_bytes + 127u) & ~127u;
     const uint32_t sIn = (sPar + (uint32_t)a.ocp * 8u + 127u) & ~127u;
-    __shared__ __align__(8) uint64_t mma_done;
+    const uint32_t pitch = acc_pitch(a.ocp), sImg = sIn + 2u * in_stride; // accumulator image [128][pitch]
     __shared__ __align__(8) uint64_t in_full[2];
-    __shared__ uint32_t tmem_slot;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x;
     const int tw = tid & 15, th = tid >> 4; // TMA_IN: the tile is 16 x 8 output pixels
 
     if (tid == 0)
     {
-        mbar_init(&mma_done, 1);
         mbar_init(&in_full[0], 1), mbar_init(&in_full[1], 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 0)
-    {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)), "r"(a.tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
     }
     __syncthreads();
     auto tile_coords = [&](unsigned tile, int& n, int& oh0, int& ow0)
@@ -839,8 +795,7 @@ __global__ void __launch_bounds__(128) stem_tc_kernel(const __grid_constant__ CU
     }
     for (int c = tid; c < a.ocp; c += 128) sts_f2(sPar + c * 8, (MODE != 2) ? __ldg(e.fast_par + c) : make_float2(0.f, 0.f));
 
-    uint32_t phase = 0, it = 0;
-    uint32_t tmem_base = 0;
+    uint32_t it = 0;
     for (unsigned tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x, it++)
     {
         uint32_t row[8] = {0, 0, 0, 0, 0, 0, 0, 0};
@@ -915,29 +870,19 @@ __global__ void __launch_bounds__(128) stem_tc_kernel(const __grid_constant__ CU
         sts_u4(sA + sw32_offset(tid, 0), row[0], row[1], row[2], row[3]);
         sts_u4(sA + sw32_offset(tid, 1), row[4], row[5], row[6], row[7]);
         fence_proxy_async_smem(); // the MMA reads these generic-proxy writes through the async proxy
-        tcgen05_fence_before();
-        __syncthreads(); // (first iteration: also publishes the TMEM address, the B tile and the constants)
-        tcgen05_fence_after();
-        tmem_base = tmem_slot;
-        if (tid == 0)
-        {
-            // everybody has read this tile's window: prefetch the next one into the other buffer
-            if (TMA_IN && tile + gridDim.x < a.ntiles) TB200_STEM_LOAD_TILE(tile + gridDim.x, (it + 1) & 1);
-            umma_i8(tmem_base, make_smem_desc(sA, 32), make_smem_desc(sB, 32), a.idesc, 0u);
-            tcgen05_commit(&mma_done);
-        }
-        mbar_wait(&mma_done, phase);
-        phase ^= 1;
-        tcgen05_fence_after();
+        __syncthreads();          // (first iteration: also publishes the B tile and the constants)
+        // everybody has read this tile's window: prefetch the next one into the other buffer
+        if (TMA_IN && tid == 0 && tile + gridDim.x < a.ntiles) TB200_STEM_LOAD_TILE(tile + gridDim.x, (it + 1) & 1);
+        wg_mma_to_image<false, false>(sA, 0u, sB, 0u, 1, 32, a.ocp, sImg, pitch);
+        __syncthreads();
 
-        // ---- epilogue: lane = pixel, 16 channels per TMEM load, OCp contiguous output bytes per pixel ----
+        // ---- epilogue: thread = pixel = accumulator row, 16 channels per load, OCp contiguous output bytes per pixel ----
         uint8_t* op = a.out + (size_t)pix * a.ocp;
-        const uint32_t tb = tmem_base + ((uint32_t)(warp * 32) << 16);
+        const uint32_t tb = sImg + (uint32_t)tid * pitch;
         for (int c = 0; c < a.ocp; c += 16)
         {
             uint32_t v[16];
-            tmem_ld16(tb + c, v);
-            tmem_ld_wait();
+            acc_ld16(tb + 4u * c, v);
             uint32_t w[4];
             if (MODE == 2)
             {
@@ -952,16 +897,8 @@ __global__ void __launch_bounds__(128) stem_tc_kernel(const __grid_constant__ CU
                 stem_unit_fast<MODE == 1>(v, sPar + c * 8, c, e, w);
             if (valid) *reinterpret_cast<uint4*>(op + c) = make_uint4(w[0], w[1], w[2], w[3]);
         }
-        // the next tile's MMA overwrites the accumulator and its gather overwrites the A tile (the MMA has completed)
-        tcgen05_fence_before();
+        // the next tile's MMA overwrites the accumulator image and its gather overwrites the A tile
         __syncthreads();
-    }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 0)
-    {
-        tcgen05_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_slot), "r"(a.tmem_cols) : "memory");
     }
 }
 
@@ -997,15 +934,11 @@ cudaError_t launch_stem_tc(const DwPlan& plan, const void* in, const void* w, vo
     a.in = (const uint8_t*)in, a.w = (const uint8_t*)w, a.out = (uint8_t*)out;
     a.n = s.n, a.c = s.c, a.h = s.h, a.w_in = s.w, a.oh = s.oh, a.ow = s.ow, a.ocp = s.ocp, a.oc = s.oc, a.stride = s.sh, a.ph = s.ph0, a.pw = s.pw0;
     a.npix = (unsigned)((long long)s.n * s.oh * s.ow);
-    a.idesc = make_idesc_i8(s.ocp, true, true);
-    uint32_t cols = 32;
-    while (cols < (uint32_t)s.ocp) cols <<= 1;
-    a.tmem_cols = cols;
     const bool tma = plan.valid != 0;
     a.tiles_w = (s.ow + 15) / 16, a.tiles_h = (s.oh + 7) / 8;
     a.box_w = plan.tile_cols, a.box_h = plan.tile_rows, a.in_bytes = tma ? plan.tile_cols * plan.tile_rows * s.c : 0, a.xoff = plan.gpr;
     a.ntiles = tma ? (unsigned)a.tiles_w * a.tiles_h * s.n : (a.npix + 127u) / 128u;
-    const size_t smem = 4096 + (size_t)s.ocp * 32 + (size_t)s.ocp * 8 + 128 + 2 * (size_t)((a.in_bytes + 127) & ~127) + 1024;
+    const size_t smem = 4096 + (size_t)s.ocp * 32 + (size_t)s.ocp * 8 + 128 + 2 * (size_t)((a.in_bytes + 127) & ~127) + 128 * (size_t)acc_pitch(s.ocp) + 1024;
     static int sms = 0;
     if (!sms)
     {
@@ -1019,11 +952,13 @@ cudaError_t launch_stem_tc(const DwPlan& plan, const void* in, const void* w, vo
     const int mode = !e.fast_ok ? 2 : (e.fuse_bias ? 1 : 0);
     CUtensorMap tm;
     memcpy(&tm, plan.tmap_in, sizeof tm);
-#define TB200_STEM_CASE(MD, T)                                       \
-    if (mode == MD && tma == T)                                      \
-    {                                                                \
-        stem_tc_kernel<MD, T><<<grid, 128, smem, st>>>(tm, a, e);    \
-        return cudaGetLastError();                                   \
+#define TB200_STEM_CASE(MD, T)                                                                                                 \
+    if (mode == MD && tma == T)                                                                                                \
+    {                                                                                                                          \
+        cudaError_t err = cudaFuncSetAttribute(stem_tc_kernel<MD, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
+        if (err != cudaSuccess) return err;                                                                                    \
+        stem_tc_kernel<MD, T><<<grid, 128, smem, st>>>(tm, a, e);                                                              \
+        return cudaGetLastError();                                                                                             \
     }
     TB200_STEM_CASE(0, true) TB200_STEM_CASE(1, true) TB200_STEM_CASE(2, true)
     TB200_STEM_CASE(0, false) TB200_STEM_CASE(1, false) TB200_STEM_CASE(2, false)
@@ -1033,10 +968,10 @@ cudaError_t launch_stem_tc(const DwPlan& plan, const void* in, const void* w, vo
 
 // ---- gather convolution on the tensor cores (uint8 stems, 3x3 convolutions over 16-channel NHWC tensors) ---------------
 // Same skeleton as the stem above, for the two YOLOv3-tiny layers the implicit GEMM cannot take: the uint8 NCHW stem
-// (3 -> 16 channels at 416x416) and the 3x3 convolution whose input has only 16 channels (a 32-byte UMMA k-step would
+// (3 -> 16 channels at 416x416) and the 3x3 convolution whose input has only 16 channels (a 32-byte wgmma k-step would
 // straddle two filter taps of a 4-D TMA box).  Every thread gathers the K bytes of its output pixel itself -- NCHW: 27 byte
 // loads; NHWC16: nine 16-byte loads, one per tap -- and writes them as one row of `ks` SW32 K-major k-block tiles; `ks`
-// MMAs (K = 32 each) accumulate.  uint8: taps outside the image are filled with the input zero point (they then contribute
+// k-steps (K = 32 each) accumulate.  uint8: taps outside the image are filled with the input zero point (they then contribute
 // (zx-zx)(w-zw) = 0, exactly like the reference, which skips them), padding K positions hold 0 in A and B, and the thread
 // sums its own row (dp4a) so that  sum (x-zx)(w-zw) = acc - zw*sum(x) + corr[oc]  needs no ones-row and no border table.
 // Takes the role of im2col + sgemm of conv_hcl_run for these shapes (conv_kernel_x86.c:187-242, 1008-1631).
@@ -1047,7 +982,6 @@ struct GatherArgs
     uint8_t* out;
     int n, c, h, w_in, oh, ow, ocp, oc, stride, ph, pw;
     unsigned npix, ntiles;
-    uint32_t idesc, tmem_cols;
     int ks, nhwc16;
     uint32_t fill; // byte for taps outside the image, replicated x4 (uint8: the input zero point; int8: 0)
     uint32_t fill16[4]; // NHWC16: the same for a whole 16-channel tap; pad channels (c >= C) stay 0 like in the tensor itself
@@ -1059,20 +993,8 @@ __global__ void __launch_bounds__(128) conv_gather_tc_kernel(const GatherArgs a,
     extern __shared__ __align__(1024) uint8_t gat_smem[];
     uint8_t* sm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(gat_smem) + 1023) & ~(uintptr_t)1023);
     const uint32_t sA = smem_u32(sm), sB = sA + (uint32_t)a.ks * 4096u, b_tile = (uint32_t)a.ocp * 32u, sPar = sB + (uint32_t)a.ks * b_tile;
-    __shared__ __align__(8) uint64_t mma_done;
-    __shared__ uint32_t tmem_slot;
-    const int tid = threadIdx.x, warp = tid >> 5;
-
-    if (tid == 0)
-    {
-        mbar_init(&mma_done, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 0)
-    {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)), "r"(a.tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
+    const uint32_t pitch = acc_pitch(a.ocp), sImg = (sPar + (uint32_t)a.ocp * 8u + 15u) & ~15u; // accumulator image [128][pitch]
+    const int tid = threadIdx.x;
     // B tiles (one per k-step) and the epilogue constants: identical for every CTA, L2 resident
     for (int i = tid; i < a.ks * a.ocp * 2; i += 128)
     {
@@ -1082,7 +1004,6 @@ __global__ void __launch_bounds__(128) conv_gather_tc_kernel(const GatherArgs a,
     }
     for (int c = tid; c < a.ocp; c += 128) sts_f2(sPar + c * 8, (MODE != 2 || U8) ? __ldg(e.fast_par + c) : make_float2(0.f, 0.f));
 
-    uint32_t phase = 0;
     for (unsigned tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x)
     {
         const unsigned pix = tile * 128u + (unsigned)tid;
@@ -1157,28 +1078,17 @@ __global__ void __launch_bounds__(128) conv_gather_tc_kernel(const GatherArgs a,
                 sts_u4(sA + (uint32_t)(j >> 1) * 4096u + sw32_offset(tid, j & 1), row[4 * j], row[4 * j + 1], row[4 * j + 2], row[4 * j + 3]);
         }
         fence_proxy_async_smem(); // the MMAs read these generic-proxy writes through the async proxy
-        tcgen05_fence_before();
-        __syncthreads(); // (first iteration: also publishes the TMEM address, the B tiles and the constants)
-        tcgen05_fence_after();
-        const uint32_t tmem_base = tmem_slot;
-        if (tid == 0)
-        {
-            for (int kb = 0; kb < a.ks; kb++)
-                umma_i8(tmem_base, make_smem_desc(sA + (uint32_t)kb * 4096u, 32), make_smem_desc(sB + (uint32_t)kb * b_tile, 32), a.idesc, kb ? 1u : 0u);
-            tcgen05_commit(&mma_done);
-        }
-        mbar_wait(&mma_done, phase);
-        phase ^= 1;
-        tcgen05_fence_after();
+        __syncthreads();          // (first iteration: also publishes the B tiles and the constants)
+        wg_mma_to_image<U8, U8>(sA, 4096u, sB, b_tile, a.ks, 32, a.ocp, sImg, pitch);
+        __syncthreads();
 
         uint8_t* op = a.out + (size_t)pix * a.ocp;
-        const uint32_t tb = tmem_base + ((uint32_t)(warp * 32) << 16);
+        const uint32_t tb = sImg + (uint32_t)tid * pitch;
         const int32_t rowc = U8 ? -e.w_zero * sx : 0;
         for (int c = 0; c < a.ocp; c += 16)
         {
             uint32_t v[16];
-            tmem_ld16(tb + c, v);
-            tmem_ld_wait();
+            acc_ld16(tb + 4u * c, v);
             uint32_t w[4];
             if (U8)
             {
@@ -1254,15 +1164,7 @@ __global__ void __launch_bounds__(128) conv_gather_tc_kernel(const GatherArgs a,
                 stem_unit_fast<MODE == 1>(v, sPar + c * 8, c, e, w);
             if (valid) *reinterpret_cast<uint4*>(op + c) = make_uint4(w[0], w[1], w[2], w[3]);
         }
-        tcgen05_fence_before();
-        __syncthreads(); // the next tile's gather overwrites the A tiles, its MMAs the accumulator
-    }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 0)
-    {
-        tcgen05_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_slot), "r"(a.tmem_cols) : "memory");
+        __syncthreads(); // the next tile's gather overwrites the A tiles, its MMAs the accumulator image
     }
 }
 
@@ -1274,10 +1176,6 @@ cudaError_t launch_conv_gather_tc(const void* in, const void* w, void* out, cons
     a.n = s.n, a.c = s.c, a.h = s.h, a.w_in = s.w, a.oh = s.oh, a.ow = s.ow, a.ocp = s.ocp, a.oc = s.oc, a.stride = s.sh, a.ph = s.ph0, a.pw = s.pw0;
     a.npix = (unsigned)((long long)s.n * s.oh * s.ow);
     a.ntiles = (a.npix + 127u) / 128u;
-    a.idesc = make_idesc_i8(s.ocp, !e.is_uint8, !e.is_uint8);
-    uint32_t cols = 32;
-    while (cols < (uint32_t)s.ocp) cols <<= 1;
-    a.tmem_cols = cols;
     a.ks = nhwc16 ? 5 : (s.c * s.kh * s.kw + 31) / 32, a.nhwc16 = nhwc16;
     a.fill = e.is_uint8 ? ((uint32_t)(e.in_zero & 0xff) * 0x01010101u) : 0u;
     for (int j = 0; j < 4; j++)
@@ -1286,7 +1184,7 @@ cudaError_t launch_conv_gather_tc(const void* in, const void* w, void* out, cons
         for (int t = 0; t < 4; t++)
             if (j * 4 + t < s.c) a.fill16[j] |= (a.fill & 0xffu) << (8 * t);
     }
-    const size_t smem = (size_t)a.ks * 4096 + (size_t)a.ks * s.ocp * 32 + (size_t)s.ocp * 8 + 1024;
+    const size_t smem = (size_t)a.ks * 4096 + (size_t)a.ks * s.ocp * 32 + (size_t)s.ocp * 8 + 16 + 128 * (size_t)acc_pitch(s.ocp) + 1024;
     static int sms = 0;
     if (!sms)
     {
@@ -1302,7 +1200,7 @@ cudaError_t launch_conv_gather_tc(const void* in, const void* w, void* out, cons
     {                                                                                                                              \
         /* the opt-in is per device AND per context: set it before every launch (launches happen at graph capture only) */ \
         {                                                                                                                          \
-            cudaError_t err = cudaFuncSetAttribute(conv_gather_tc_kernel<MD, U, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024); \
+            cudaError_t err = cudaFuncSetAttribute(conv_gather_tc_kernel<MD, U, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
             if (err != cudaSuccess) return err;                                                                                    \
         }                                                                                                                          \
         conv_gather_tc_kernel<MD, U, K><<<grid, 128, smem, st>>>(a, e);                                                            \
@@ -1317,17 +1215,15 @@ cudaError_t launch_conv_gather_tc(const void* in, const void* w, void* out, cons
 // ---- small-K pointwise GEMM: many small CTAs instead of one warp-specialised persistent CTA ---------------------------
 // For K <= 256 (the first pointwise layers: K = 32..128, one or two k-blocks) the persistent kernel above spends more
 // time in hand-overs between its roles than in work (timeline: the epilogue warps idle ~50% of the time).  Here a CTA is
-// four warps = the four TMEM lane quarters; it keeps the N tile's weights in shared memory, double-buffers the A tile
-// (TMA), and per m-tile does: wait A -> one elected thread issues the MMAs -> everybody requantises its own accumulator
-// row and writes its bn contiguous output bytes straight to global memory.  There is no pipelining inside a CTA beyond the
-// A prefetch; 4-8 CTAs are resident per SM (bounded by TMEM columns and shared memory) and overlap each other, the way the
-// tensor-core stem above does (8.2 output bytes/clk/SM vs 4.2 for the persistent kernel on the same layer shape).
+// one warpgroup; it keeps the N tile's weights in shared memory, double-buffers the A tile (TMA), and per m-tile does:
+// wait A -> the warpgroup's MMAs into the accumulator image -> everybody requantises its own accumulator row and writes its
+// bn contiguous output bytes straight to global memory.  There is no pipelining inside a CTA beyond the A prefetch; several
+// CTAs are resident per SM (bounded by shared memory) and overlap each other, the way the tensor-core stem above does.
 struct SimpleArgs
 {
     uint8_t* out;
     long long m;
     int m_tiles, n_tiles, k_blocks, block_n, block_k, swizzle, ocp, oc, ldo;
-    uint32_t idesc, tmem_cols;
 };
 
 template <int MODE> // 0 fast, 1 fast + fused bias, 2 exact
@@ -1340,21 +1236,16 @@ __global__ void __launch_bounds__(128) gemm_simple_kernel(const __grid_constant_
     uint8_t* sA = sm;                                               // [2][k_blocks][a_bytes]
     uint8_t* sB = sA + 2u * (size_t)g.k_blocks * a_bytes;           // [k_blocks][b_al]
     const uint32_t sPar = smem_u32(sB) + (uint32_t)g.k_blocks * b_al; // [block_n] x 8 bytes
-    __shared__ __align__(8) uint64_t a_full[2], b_full, mma_done;
-    __shared__ uint32_t tmem_slot;
-    const int tid = threadIdx.x, warp = tid >> 5;
+    const uint32_t pitch = acc_pitch(g.block_n), sImg = sPar + (uint32_t)g.block_n * 8u; // accumulator image [128][pitch]
+    __shared__ __align__(8) uint64_t a_full[2], b_full;
+    const int tid = threadIdx.x;
     const int ntile = blockIdx.x % g.n_tiles, n0 = ntile * g.block_n;
     const int mfirst = blockIdx.x / g.n_tiles, mstep = gridDim.x / g.n_tiles; // the grid is a multiple of n_tiles
 
     if (tid == 0)
     {
-        mbar_init(&a_full[0], 1), mbar_init(&a_full[1], 1), mbar_init(&b_full, 1), mbar_init(&mma_done, 1);
+        mbar_init(&a_full[0], 1), mbar_init(&a_full[1], 1), mbar_init(&b_full, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 0)
-    {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)), "r"(g.tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
     }
     __syncthreads();
     if (tid == 0)
@@ -1369,49 +1260,35 @@ __global__ void __launch_bounds__(128) gemm_simple_kernel(const __grid_constant_
     }
     for (int c = tid; c < g.block_n; c += 128)
         sts_f2(sPar + c * 8, (MODE != 2 && n0 + c < g.ocp) ? __ldg(e.fast_par + n0 + c) : make_float2(0.f, 0.f));
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = tmem_slot;
-    const uint32_t tb = tmem_base + ((uint32_t)(warp * 32) << 16);
+    const uint32_t tb = sImg + (uint32_t)tid * pitch;
 
     uint32_t it = 0;
     for (int mt = mfirst; mt < g.m_tiles; mt += mstep, it++)
     {
         const int buf = it & 1;
-        if (tid == 0)
+        // the other buffer was read by the MMAs of the previous tile, which have completed: prefetch the next tile
+        if (tid == 0 && mt + mstep < g.m_tiles)
         {
-            // the other buffer was read by the MMAs of the previous tile, which have completed: prefetch the next tile
-            if (mt + mstep < g.m_tiles)
-            {
-                mbar_expect_tx(&a_full[buf ^ 1], (uint32_t)g.k_blocks * a_bytes);
-                for (int kb = 0; kb < g.k_blocks; kb++)
-                    tma_load_2d(&tmap_a, &a_full[buf ^ 1], sA + ((size_t)(buf ^ 1) * g.k_blocks + kb) * a_bytes, kb * g.block_k, (mt + mstep) * BLOCK_M);
-            }
-            if (it == 0) mbar_wait(&b_full, 0);
-            mbar_wait(&a_full[buf], (it >> 1) & 1);
-            tcgen05_fence_after();
+            mbar_expect_tx(&a_full[buf ^ 1], (uint32_t)g.k_blocks * a_bytes);
             for (int kb = 0; kb < g.k_blocks; kb++)
-            {
-                const uint64_t da = make_smem_desc(smem_u32(sA + ((size_t)buf * g.k_blocks + kb) * a_bytes), g.swizzle);
-                const uint64_t db = make_smem_desc(smem_u32(sB + (size_t)kb * b_al), g.swizzle);
-                for (int k = 0; k < g.block_k / 32; k++) umma_i8(tmem_base, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), g.idesc, (kb | k) ? 1u : 0u);
-            }
-            tcgen05_commit(&mma_done);
+                tma_load_2d(&tmap_a, &a_full[buf ^ 1], sA + ((size_t)(buf ^ 1) * g.k_blocks + kb) * a_bytes, kb * g.block_k, (mt + mstep) * BLOCK_M);
         }
-        mbar_wait(&mma_done, it & 1);
-        tcgen05_fence_after();
+        if (it == 0) mbar_wait(&b_full, 0);
+        mbar_wait(&a_full[buf], (it >> 1) & 1);
+        wg_mma_to_image<false, false>(smem_u32(sA + (size_t)buf * g.k_blocks * a_bytes), a_bytes, smem_u32(sB), b_al, g.k_blocks, g.swizzle,
+                                      g.block_n, sImg, pitch);
+        __syncthreads();
 
-        // ---- epilogue: lane = output row, 16 channels per TMEM load, straight to global memory ----
+        // ---- epilogue: thread = output row, 16 channels per load, straight to global memory ----
         const long long row = (long long)mt * BLOCK_M + tid;
         uint8_t* op = g.out + (size_t)(row < g.m ? row : 0) * g.ldo + n0;
         uint32_t v0[16], v1[16];
-        tmem_ld16(tb, v0);
+        acc_ld16(tb, v0);
         const int nch = g.block_n >> 4;
         for (int c = 0; c < nch; c += 2)
         {
-            tmem_ld_wait();
-            if (c + 1 < nch) tmem_ld16(tb + (c + 1) * 16, v1);
+            if (c + 1 < nch) acc_ld16(tb + (c + 1) * 64, v1);
             {
                 uint32_t w[4];
                 if (MODE == 2)
@@ -1428,8 +1305,7 @@ __global__ void __launch_bounds__(128) gemm_simple_kernel(const __grid_constant_
                 if (row < g.m && n0 + c * 16 < g.ocp) *reinterpret_cast<uint4*>(op + c * 16) = make_uint4(w[0], w[1], w[2], w[3]);
             }
             if (c + 1 >= nch) break;
-            tmem_ld_wait();
-            if (c + 2 < nch) tmem_ld16(tb + (c + 2) * 16, v0);
+            if (c + 2 < nch) acc_ld16(tb + (c + 2) * 64, v0);
             {
                 uint32_t w[4];
                 if (MODE == 2)
@@ -1446,68 +1322,51 @@ __global__ void __launch_bounds__(128) gemm_simple_kernel(const __grid_constant_
                 if (row < g.m && n0 + (c + 1) * 16 < g.ocp) *reinterpret_cast<uint4*>(op + (c + 1) * 16) = make_uint4(w[0], w[1], w[2], w[3]);
             }
         }
-        // the next tile's MMAs overwrite the accumulator
-        tcgen05_fence_before();
+        // the next tile's MMAs overwrite the accumulator image
         __syncthreads();
-        tcgen05_fence_after();
-    }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 0)
-    {
-        tcgen05_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_slot), "r"(g.tmem_cols) : "memory");
     }
 }
 
 // ---- on-box peak of the int8 tensor pipe (SURVEY.md 8(d): "replace the nominal numbers by on-box microbenchmark peaks") ---------
-// One CTA per SM; one thread issues `iters` x 4 tcgen05.mma.kind::i8 of 128 x 256 x 32 on fixed shared-memory tiles (contents
-// irrelevant), alternating between two TMEM accumulators; no loads, no epilogue.  ops = CTAs * iters * 4 * 2 * 128 * 256 * 32.
-__global__ void __launch_bounds__(128) i8_mma_peak_kernel(int iters, uint32_t idesc)
+// One CTA of two warpgroups per SM; each warpgroup issues `iters` x 4 wgmma m64n128k32 s8 on fixed shared-memory tiles (contents
+// irrelevant) into its own registers; no loads, no epilogue.  ops = CTAs * 2 * iters * 4 * 2 * 64 * 128 * 32.
+__device__ __forceinline__ void wgmma_n128_ss(uint32_t (&d)[64], uint64_t desc_a, uint64_t desc_b)
+{
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\twgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p;\n\t}"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+                 : "l"(desc_a), "l"(desc_b)
+                 : "memory");
+}
+__global__ void __launch_bounds__(256) i8_mma_peak_kernel(int iters)
 {
     extern __shared__ __align__(1024) uint8_t peak_smem[];
     uint8_t* sm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(peak_smem) + 1023) & ~(uintptr_t)1023);
-    __shared__ __align__(8) uint64_t done;
-    __shared__ uint32_t tmem_slot;
-    for (int i = threadIdx.x; i < (16384 + 32768) / 16; i += 128) sts_u4(smem_u32(sm) + i * 16, 0x01010101u, 0x01020304u, 0x7f7f0101u, 0u);
+    for (int i = threadIdx.x; i < (16384 + 32768) / 16; i += 256) sts_u4(smem_u32(sm) + i * 16, 0x01010101u, 0x01020304u, 0x7f7f0101u, 0u);
     fence_proxy_async_smem();
-    if (threadIdx.x == 0)
-    {
-        mbar_init(&done, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (threadIdx.x < 32)
-    {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)), "r"(512u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem = tmem_slot;
-    if (threadIdx.x == 0)
-    {
-        const uint64_t da = make_smem_desc(smem_u32(sm), 128), db = make_smem_desc(smem_u32(sm) + 16384u, 128);
-        for (int it = 0; it < iters; it++)
+    uint32_t d[64];
 #pragma unroll
-            for (int k = 0; k < 4; k++) umma_i8(tmem + (uint32_t)(it & 1) * 256u, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc, 1u);
-        tcgen05_commit(&done);
-        mbar_wait(&done, 0);
-    }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (threadIdx.x < 32)
+    for (int i = 0; i < 64; i++) d[i] = 0;
+    const uint64_t da = make_smem_desc(smem_u32(sm) + (uint32_t)(threadIdx.x >> 7) * 8192u, 128), db = make_smem_desc(smem_u32(sm) + 16384u, 128);
+    wgmma_fence();
+    for (int it = 0; it < iters; it++)
     {
-        tcgen05_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512u) : "memory");
+#pragma unroll
+        for (int k = 0; k < 4; k++) wgmma_n128_ss(d, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2));
+        wgmma_commit();
+        wgmma_wait<1>();
     }
+    wgmma_wait<0>();
+    uint32_t x = 0;
+#pragma unroll
+    for (int i = 0; i < 64; i++) x ^= d[i];
+    if (x == 0x9e3779b9u) sts_u4(smem_u32(sm), x, x, x, x); // keeps the accumulators live
 }
 
 cudaError_t probe_int8_mma_peak(int num_sms, double* tops, cudaStream_t st)
 {
     cudaError_t err = cudaFuncSetAttribute(i8_mma_peak_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024);
     if (err != cudaSuccess) return err;
-    const uint32_t idesc = make_idesc_i8(256, true, true);
     cudaEvent_t a, b;
     cudaEventCreate(&a), cudaEventCreate(&b);
     const int iters = 20000;
@@ -1515,12 +1374,12 @@ cudaError_t probe_int8_mma_peak(int num_sms, double* tops, cudaStream_t st)
     for (int rep = 0; rep < 4; rep++)
     {
         cudaEventRecord(a, st);
-        i8_mma_peak_kernel<<<num_sms, 128, 16384 + 32768 + 1024, st>>>(iters, idesc);
+        i8_mma_peak_kernel<<<num_sms, 256, 16384 + 32768 + 1024, st>>>(iters);
         cudaEventRecord(b, st);
         if ((err = cudaEventSynchronize(b)) != cudaSuccess) break;
         float ms = 0;
         cudaEventElapsedTime(&ms, a, b);
-        const double t = (double)num_sms * iters * 4.0 * 2.0 * 128 * 256 * 32 / (ms * 1e-3) / 1e12;
+        const double t = (double)num_sms * 2.0 * iters * 4.0 * 2.0 * 64 * 128 * 32 / (ms * 1e-3) / 1e12;
         if (rep > 0 && t > best) best = t; // the first repetition is the warm-up
     }
     cudaEventDestroy(a), cudaEventDestroy(b);
@@ -1575,9 +1434,7 @@ static int encode_2d(void* tmap, const void* base, uint64_t inner, uint64_t rows
 }
 
 // Where the uint8 path's sum(x) comes from (TB200_U8_SX, A/B switch): 3 (default) = two extra warps add up the rows of the A tiles,
-// 0 = 16 rows of ones in every B tile (sum(x) is then a 17th..32nd accumulator column; costs TMEM columns and smaller N tiles).
-// Measured and dropped: a second MMA per k-step against a tile of ones (interleaved or after the k-block) -- no better than the ones
-// rows, the cost was the smaller accumulator stages, not the MMAs (DESIGN.md 5).
+// 0 = 16 rows of ones in every B tile (sum(x) is then a 17th..32nd accumulator column; costs image columns and m-tiles per stage).
 int gemm_sx_mode()
 {
     static const int mode = [] { const char* e = getenv("TB200_U8_SX"); return (e && atoi(e) == 0) ? 0 : 3; }();
@@ -1589,13 +1446,15 @@ int gemm_tile_rows(int ocp, int u8) { return gemm_block_n(ocp, u8) + ((u8 > 1 &&
 
 int gemm_block_n(int ocp, int u8)
 {
-    // ones-rows mode: 16 extra TMEM columns per m-tile hold sum(x), and two accumulator stages must fit 512 columns
-    if (u8 && gemm_sx_mode() == 0) return ocp <= 240 ? ocp : 128;
-    return ocp <= 256 ? ocp : 128;
+    // N tiles of at most 128 channels (+ 16 ones rows in mode 0): the accumulator image of a stage shares shared memory with
+    // the operand ring; the channels are dealt evenly to the fewest such tiles
+    (void)u8;
+    const int nt = (ocp + 127) / 128;
+    return ((ocp + nt - 1) / nt + 15) & ~15;
 }
 
 // Store-group width and output tensor maps.  A group is 32 rows x 16*cs channels; cs is the largest of 4 / 2 / 1 that
-// divides the N tile's chunk count and deals the stage's groups evenly to the four warps of a TMEM lane quarter.
+// divides the N tile's chunk count and deals the stage's groups evenly to the four warps of a 32-row image quarter.
 static void plan_store_groups(GemmPlan* p)
 {
     const int nch = p->block_n / 16;
@@ -1636,7 +1495,8 @@ static int plan_epilogue(GemmPlan* p, const void* out, uint64_t d1, uint64_t d2)
 static int epilogue_smem_bytes(const GemmPlan* p)
 {
     const int par_ch = p->n_tiles * p->block_n;
-    return EPI_WARPS * 2 * 512 * (p->cs == 8 ? 4 : p->cs) + (par_ch <= PAR_MAX ? par_ch : p->block_n) * 8 + (int)sizeof(GemmSmemCtl) + 2048;
+    return EPI_WARPS * 2 * 512 * (p->cs == 8 ? 4 : p->cs) + (par_ch <= PAR_MAX ? par_ch : p->block_n) * 8 + (int)sizeof(GemmSmemCtl) + 2048 +
+           128 * (int)acc_pitch(p->mt * p->bnx) + 16;
 }
 
 // Operand ring depth and the resident-B decision.  With the N tile's weights resident the ring carries A tiles only,
@@ -1672,13 +1532,13 @@ int gemm_plan_create(GemmPlan* p, const void* a, long long lda, const void* b, v
     p->taps = 1;
     p->n_tiles = (ocp + p->block_n - 1) / p->block_n;
     p->m_tiles = (m + BLOCK_M - 1) / BLOCK_M;
-    // m-tiles per accumulator stage: amortise the per-stage synchronisation over ~256 TMEM columns of work
+    // m-tiles per accumulator stage: amortise the per-stage synchronisation over up to ACC_COLS_MAX image columns of work
     p->mt = 1;
     {
         // several m-tiles per stage when the CTA stays on one N tile anyway (single tile, or resident weights)
         const bool resident = (long long)p->k_blocks * ((p->bnx * p->block_k + 1023) & ~1023) <= B_RESIDENT_MAX;
         if (p->n_tiles == 1 || (resident && getenv("TB200_GEMM_PAIR")))
-            while (p->mt < 4 && 2 * (p->mt * 2) * p->bnx <= 512 && (long long)(p->mt * 2) * 148 <= p->m_tiles * (p->n_tiles == 1 ? 148 : 1)) p->mt *= 2;
+            while (p->mt < 4 && (p->mt * 2) * p->bnx <= ACC_COLS_MAX && (long long)(p->mt * 2) * 132 <= p->m_tiles * (p->n_tiles == 1 ? 132 : 1)) p->mt *= 2;
     }
     plan_store_groups(p);
     int rc = plan_ring(p);
@@ -1693,15 +1553,13 @@ int gemm_plan_create(GemmPlan* p, const void* a, long long lda, const void* b, v
     // small-K layers: the many-small-CTAs kernel (gemm_simple_kernel), N tiles of at most 128 channels
     p->simple = 0;
     static const int maxk = getenv("TB200_GEMM_SIMPLE_MAXK") ? atoi(getenv("TB200_GEMM_SIMPLE_MAXK")) : 256;
-    // Opt-in (TB200_GEMM_SIMPLE=1): measured slower than the persistent kernel on every MobileNet-v1 layer it applies to
-    // (batch 256: 148 vs 134 us for K=32/N=64, 84 vs 71 us for K=64/N=128, 72 vs 44 us for K=256/N=256); kept as the
-    // cross-check implementation of the same contraction and for the record of the experiment.
+    // Opt-in (TB200_GEMM_SIMPLE=1): the cross-check implementation of the same contraction.
     if (!u8 && k <= maxk && getenv("TB200_GEMM_SIMPLE"))
     {
         const int bn = ocp <= 128 ? ocp : 128;
         const int a_bytes = BLOCK_M * p->block_k, b_al = (bn * p->block_k + 1023) & ~1023;
-        const int smem = p->k_blocks * (2 * a_bytes + b_al) + bn * 8 + 2048;
-        if (smem <= 112 * 1024 &&
+        const int smem = p->k_blocks * (2 * a_bytes + b_al) + bn * 8 + 128 * (int)acc_pitch(bn) + 2048;
+        if (smem <= 200 * 1024 &&
             encode_2d(p->tmap_b_s, b, (uint64_t)k, (uint64_t)ocp, (uint64_t)k, p->block_k, bn, p->swizzle) == 0)
             p->simple = 1, p->s_block_n = bn, p->s_n_tiles = (ocp + bn - 1) / bn, p->s_smem = smem, p->out = out;
     }
@@ -1754,7 +1612,7 @@ int gemm_plan_create_conv(GemmPlan* p, const void* in, const void* w, void* out,
         // several m-tiles per stage when the CTA stays on one N tile anyway (single tile, or resident weights)
         const bool resident = (long long)p->k_blocks * ((p->bnx * p->block_k + 1023) & ~1023) <= B_RESIDENT_MAX;
         if (p->n_tiles == 1 || (resident && getenv("TB200_GEMM_PAIR")))
-            while (p->mt < 4 && 2 * (p->mt * 2) * p->bnx <= 512 && (long long)(p->mt * 2) * 148 <= p->m_tiles * (p->n_tiles == 1 ? 148 : 1)) p->mt *= 2;
+            while (p->mt < 4 && (p->mt * 2) * p->bnx <= ACC_COLS_MAX && (long long)(p->mt * 2) * 132 <= p->m_tiles * (p->n_tiles == 1 ? 132 : 1)) p->mt *= 2;
     }
     plan_store_groups(p);
     int rc = plan_ring(p);
@@ -1800,8 +1658,8 @@ static void gemm_trace_report(const GemmPlan& p, const GemmArgs& g, int grid, cu
     for (int i = 0; i < 4 * 1024; i++)
         if (h[i] && (h[i] >> 8) < t0) t0 = h[i] >> 8;
     static const char* role[4] = {"P", "M", "E0", "E15"};
-    static const char* tagM[3] = {"kblock mma issued", "got tmem_empty", "commit tmem_full"};
-    static const char* tagE[5] = {"got tmem_full", "group stored", "arrive tmem_empty", "tmem ld done", "unit done"};
+    static const char* tagM[3] = {"kblock mma issued", "got sx_empty", "commit sx_full"};
+    static const char* tagE[5] = {"got sx_full", "group stored", "arrive sx_empty", "tmem ld done", "unit done"};
     for (int r = 0; r < 4; r++)
         for (int i = 0; i < 1024 && h[r * 1024 + i]; i++)
         {
@@ -1817,13 +1675,7 @@ static cudaError_t launch_gemm_simple(const GemmPlan& p, const EpiParams& e, int
     SimpleArgs g;
     g.out = (uint8_t*)p.out, g.m = p.m, g.m_tiles = (int)p.m_tiles, g.n_tiles = p.s_n_tiles, g.k_blocks = p.k_blocks, g.block_n = p.s_block_n;
     g.block_k = p.block_k, g.swizzle = p.swizzle, g.ocp = p.ocp, g.oc = p.oc, g.ldo = p.ldo;
-    g.idesc = make_idesc_i8(p.s_block_n, true, true);
-    uint32_t cols = 32;
-    while (cols < (uint32_t)p.s_block_n) cols <<= 1;
-    g.tmem_cols = cols;
-    int per_sm = (int)(512 / cols);
-    const int by_smem = (220 * 1024) / (p.s_smem + 1024);
-    if (by_smem < per_sm) per_sm = by_smem;
+    int per_sm = (220 * 1024) / (p.s_smem + 1024);
     if (per_sm > 16) per_sm = 16;
     if (per_sm < 1) per_sm = 1;
     long long want = p.m_tiles * p.s_n_tiles, cap = (long long)num_sms * per_sm;
@@ -1840,7 +1692,7 @@ static cudaError_t launch_gemm_simple(const GemmPlan& p, const EpiParams& e, int
     {                                                                                                                          \
         /* the opt-in is per device AND per context: set it before every launch (launches happen at graph capture only) */ \
         {                                                                                                                      \
-            cudaError_t err = cudaFuncSetAttribute(gemm_simple_kernel<MD>, cudaFuncAttributeMaxDynamicSharedMemorySize, 116 * 1024); \
+            cudaError_t err = cudaFuncSetAttribute(gemm_simple_kernel<MD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
             if (err != cudaSuccess) return err;                                                                                \
         }                                                                                                                      \
         gemm_simple_kernel<MD><<<grid, 128, smem, st>>>(ta, tb, g, e);                                                         \
@@ -1869,20 +1721,14 @@ cudaError_t launch_gemm_i8(const GemmPlan& p, const EpiParams& e, const int32_t*
     g.bw_rcp = p.conv ? (65536u + (uint32_t)p.bw - 1) / (uint32_t)p.bw : 0;
     g.bh_rcp = p.conv ? (65536u + (uint32_t)p.bh - 1) / (uint32_t)p.bh : 0;
     g.block_k = p.block_k, g.stages = p.stages, g.swizzle = p.swizzle, g.oc = p.oc, g.ocp = p.ocp;
-    g.idesc = make_idesc_i8(p.bnx, !p.u8, p.b_signed != 0);
-    uint32_t cols = 32;
-    while (cols < (uint32_t)(2 * p.mt * g.tcols)) cols <<= 1;
-    g.tmem_cols = cols;
     g.cs = p.cs, g.ngroups = p.ngroups, g.rows_valid = p.rows_valid, g.out_mode = p.out_mode;
     const int par_ch = p.n_tiles * p.block_n;
     g.par_all = par_ch <= PAR_MAX ? 1 : 0;
     const int a_bytes = BLOCK_M * p.block_k, b_bytes = (p.bnx * p.block_k + 1023) & ~1023;
     g.b_res = p.b_res;
-    static const int teams_env = getenv("TB200_GEMM_TEAMS") ? atoi(getenv("TB200_GEMM_TEAMS")) : 0;
-    g.teams = (teams_env && p.cs != 8 && p.n_tiles * p.block_n <= PAR_MAX) ? 1 : 0;
     const size_t smem = (size_t)p.stages * (a_bytes + (p.b_res ? 0 : b_bytes)) + (p.b_res ? (size_t)p.k_blocks * b_bytes : 0) + (p.cplane ? 4096 : 0) +
                         (size_t)EPI_WARPS * 2 * 512 * (p.cs == 8 ? 4 : p.cs) + sizeof(GemmSmemCtl) +
-                        (size_t)(g.par_all ? par_ch : p.block_n) * 8 + 1024;
+                        (size_t)(g.par_all ? par_ch : p.block_n) * 8 + 16 + 128 * (size_t)acc_pitch(p.mt * g.tcols) + 1024;
     static const bool trace_on = getenv("TB200_GEMM_TRACE") != nullptr;
     static const bool launch_dbg = getenv("TB200_DEBUG_LAUNCH") != nullptr;
     static unsigned long long* trace_buf = nullptr;

@@ -97,9 +97,10 @@ struct WindowPlan
     int box_w, box_h, xoff, in_bytes, ks, smem_bytes;
 };
 int window_plan_create(WindowPlan* plan, const void* in, const ConvShape& s, int nhwc); // < 0: not applicable
+bool window_nhwc_fits(int cp, int ocp, int stride); // a 3x3 conv over an NHWC input of cp bytes per pixel fits the kernel's shared memory
 cudaError_t launch_conv_window(const WindowPlan& plan, const void* w, void* out, const ConvShape& s, const EpiParams& e, cudaStream_t st);
 
-// ---- tcgen05 GEMM (gemm_tcgen05.cu) ------------------------------------------------------------------
+// ---- wgmma GEMM (gemm_tcgen05.cu) --------------------------------------------------------------------
 // out[M][ldo] (bytes) = requant( A[M][K] (row pitch lda bytes) . B[OCp][K]^T )
 struct GemmPlan
 {
@@ -152,7 +153,7 @@ cudaError_t launch_stem_tc(const DwPlan& plan, const void* in, const void* w, vo
 // 3x3 convolutions whose K the threads gather themselves (uint8 NCHW stems, 16-channel NHWC inputs), gemm_tcgen05.cu
 cudaError_t launch_conv_gather_tc(const void* in, const void* w, void* out, const ConvShape& s, const EpiParams& e, int nhwc16, cudaStream_t st);
 cudaError_t launch_gemm_i8(const GemmPlan& plan, const EpiParams& e, const int32_t* btab, int num_sms, cudaStream_t st);
-// measured peak of tcgen05.mma kind::i8 (cta_group::1, 128 x 256 x 32) on this GPU, in TOP/s: the tensor roofline's denominator
+// measured peak of wgmma m64n128k32 s8 (two warpgroups per SM) on this GPU, in TOP/s: the tensor roofline's denominator
 cudaError_t probe_int8_mma_peak(int num_sms, double* tops, cudaStream_t st);
 
 } // namespace tb200

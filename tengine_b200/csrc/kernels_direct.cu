@@ -1,9 +1,9 @@
-// kernels_direct.cu -- CUDA-core (dp4a) kernels of the B200 backend: generic direct convolution, depthwise,
+// kernels_direct.cu -- CUDA-core (dp4a) kernels of the H100 backend: generic direct convolution, depthwise,
 // NCHW stem, and the HBM-bound glue ops (pool / relu / eltwise / concat / upsample / layout).
 //
 // Device layout: activations NHWC, channels padded to a multiple of 16 (pad lanes hold 0), 1 byte/element.
 // These kernels are the general path (any kernel/stride/pad/dilation/group) and the on-device cross-check
-// for the tcgen05 GEMM path; the dense 1x1 / FC contractions run in gemm_tcgen05.cu.
+// for the tensor-core GEMM path; the dense 1x1 / FC contractions run in gemm_tcgen05.cu.
 #include "common.cuh"
 #include "kernels.h"
 

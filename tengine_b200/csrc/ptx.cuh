@@ -1,4 +1,4 @@
-// ptx.cuh -- inline-PTX wrappers shared by the TMA / tcgen05 kernels (mbarrier, cp.async.bulk.tensor, tcgen05.*).
+// ptx.cuh -- inline-PTX wrappers shared by the TMA / wgmma kernels (mbarrier, cp.async.bulk.tensor, wgmma.*).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -53,36 +53,39 @@ __device__ __forceinline__ void tma_load_2d(const void* tmap, uint64_t* bar, voi
         "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
         : "memory");
 }
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_commit(uint64_t* bar)
+// ---- warpgroup MMA (wgmma, sm_90a): 64 x 16 x 32 int8 / uint8 products accumulated in s32 registers -------------------
+// Accumulator fragment of one m64n16 product (PTX ISA "wgmma .m64nNk32 D matrix"): warp w of the warpgroup holds rows
+// 16w..16w+15; lane l holds d[0..1] = (row l/4, cols 2(l%4)+{0,1}), d[2..3] = (row l/4+8, same cols), d[4..7] = the same for
+// cols 8 + 2(l%4)+{0,1}.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait()
 {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void umma_i8(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate)
+#define TB200_WGMMA_N16(NAME, AT, BT)                                                                                           \
+    __device__ __forceinline__ void NAME(uint32_t (&d)[8], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate)              \
+    {                                                                                                                          \
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"                                                      \
+                     "wgmma.mma_async.sync.aligned.m64n16k32.s32." AT "." BT " {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p;\n\t}"               \
+                     : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7])            \
+                     : "l"(desc_a), "l"(desc_b), "r"(accumulate)                                                               \
+                     : "memory");                                                                                              \
+    }
+TB200_WGMMA_N16(wgmma_n16_ss, "s8", "s8")
+TB200_WGMMA_N16(wgmma_n16_us, "u8", "s8")
+TB200_WGMMA_N16(wgmma_n16_su, "s8", "u8")
+TB200_WGMMA_N16(wgmma_n16_uu, "u8", "u8")
+#undef TB200_WGMMA_N16
+// AU / BU: A / B operand unsigned
+template <bool AU, bool BU>
+__device__ __forceinline__ void wgmma_n16(uint32_t (&d)[8], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate)
 {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16])
-{
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t (&v)[8])
-{
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-                 : "r"(taddr)
-                 : "memory");
+    if (AU && BU) wgmma_n16_uu(d, desc_a, desc_b, accumulate);
+    else if (AU) wgmma_n16_us(d, desc_a, desc_b, accumulate);
+    else if (BU) wgmma_n16_su(d, desc_a, desc_b, accumulate);
+    else wgmma_n16_ss(d, desc_a, desc_b, accumulate);
 }
 __device__ __forceinline__ void sts_u2(uint32_t addr, uint32_t a, uint32_t b)
 {
@@ -114,14 +117,34 @@ __device__ __forceinline__ void sts_f2(uint32_t addr, float2 v)
 {
     asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(v.x), "f"(v.y) : "memory");
 }
-__device__ __forceinline__ uint32_t tmem_ld1(uint32_t taddr)
+
+// ---- accumulator image: the s32 accumulators of a 128-row tile as [row][pitch bytes] in shared memory --------------------
+// The MMA warpgroups write their fragments here; the epilogues read one row per thread, 16 consecutive columns at a time.
+__device__ __forceinline__ void frag_to_image(const uint32_t (&d)[8], uint32_t img, uint32_t pitch, int row0, int col0)
+{
+    const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
+    const uint32_t r = (uint32_t)(row0 + 16 * w + (lane >> 2)), c = (uint32_t)(col0 + 2 * (lane & 3));
+    const uint32_t p0 = img + r * pitch + c * 4u, p1 = p0 + 8u * pitch;
+    sts_u2(p0, d[0], d[1]);
+    sts_u2(p1, d[2], d[3]);
+    sts_u2(p0 + 32u, d[4], d[5]);
+    sts_u2(p1 + 32u, d[6], d[7]);
+}
+__device__ __forceinline__ void acc_ld16(uint32_t addr, uint32_t (&v)[16])
+{
+#pragma unroll
+    for (int j = 0; j < 4; j++)
+    {
+        const uint4 u = lds_u4(addr + 16u * j);
+        v[4 * j] = u.x, v[4 * j + 1] = u.y, v[4 * j + 2] = u.z, v[4 * j + 3] = u.w;
+    }
+}
+__device__ __forceinline__ uint32_t acc_ld1(uint32_t addr)
 {
     uint32_t v;
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(v) : "r"(taddr) : "memory");
+    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr));
     return v;
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
 
 __device__ __forceinline__ void tma_load_4d(const void* tmap, uint64_t* bar, void* smem, int c0, int c1, int c2, int c3)
 {

@@ -1,5 +1,5 @@
-// tc_common.cuh -- device helpers shared by the tcgen05 kernels (gemm_tcgen05.cu, conv_window.cu): UMMA shared-memory and
-// instruction descriptors, the SW32 tile addressing of the thread-built A tiles, the per-lane fast epilogue unit.
+// tc_common.cuh -- device helpers shared by the tensor-core kernels (gemm_tcgen05.cu, conv_window.cu): wgmma shared-memory
+// descriptors, the accumulator image, the SW32 tile addressing of the thread-built A tiles, the per-lane fast epilogue unit.
 #pragma once
 #include "common.cuh"
 #include "ptx.cuh"
@@ -8,31 +8,58 @@ namespace tb200 {
 
 static constexpr int BLOCK_M = 128;
 
-// K-major operand tile in shared memory, rows of `swizzle` bytes, 8-row groups `8*swizzle` bytes apart
-// (cute/atom/mma_traits_sm100.hpp: canonical layout ((8,n),2):((swizzle/16,SBO),1), LBO = 1, version 1).
+// K-major operand tile in shared memory, rows of `swizzle` bytes, 8-row groups `8*swizzle` bytes apart: the wgmma matrix
+// descriptor (PTX ISA "Matrix Descriptor Format" for sm_90a: start >> 4, leading byte offset >> 4 (unused for swizzled K-major),
+// stride byte offset >> 4, base offset 0 (tiles are aligned to the swizzle repeat), layout 1 = 128B, 2 = 64B, 3 = 32B swizzle).
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, int swizzle)
 {
-    const uint64_t layout = (swizzle == 128) ? 2ull : (swizzle == 64) ? 4ull : 6ull;
+    const uint64_t layout = (swizzle == 128) ? 1ull : (swizzle == 64) ? 2ull : 3ull;
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr >> 4) & 0x3fff);
-    d |= (uint64_t)1 << 16;                              // leading byte offset (unused for swizzled K-major)
-    d |= (uint64_t)(((8 * swizzle) >> 4) & 0x3fff) << 32; // stride byte offset between 8-row groups
-    d |= (uint64_t)1 << 46;                              // descriptor version (Blackwell)
-    d |= layout << 61;
+    d |= (uint64_t)1 << 16;
+    d |= (uint64_t)(((8 * swizzle) >> 4) & 0x3fff) << 32;
+    d |= layout << 62;
     return d;
 }
 
-// UMMA instruction descriptor (cute/arch/mma_sm100_desc.hpp InstrDescriptor): S32 accumulate, A/B int8 or uint8,
-// both K-major, M = 128, N = block_n.
-__host__ __device__ inline uint32_t make_idesc_i8(int block_n, bool a_signed, bool b_signed)
+// bytes of one row of an accumulator image of `cols` s32 columns (16 bytes of padding: the epilogue's 16-byte row loads of
+// 32 consecutive rows then hit distinct banks)
+__host__ __device__ inline uint32_t acc_pitch(int cols) { return (uint32_t)cols * 4u + 16u; }
+
+// The CTA's first warpgroup: D[128 x ncols] = sum over nkb k-blocks of A[128 x swizzle] . B[ncols x swizzle]^T into the
+// accumulator image.  Operands are K-major swizzled tiles (A: 128 rows, B: ncols rows; one tile per k-block, a_kb / b_kb bytes
+// apart).  The two 64-row halves and column groups of at most 128 run one after the other so that the fragment stays at 64
+// registers.  The image is complete for the warpgroup when this returns; other threads need a barrier.
+template <bool AU, bool BU>
+__device__ __forceinline__ void wg_mma_to_image(uint32_t sA, uint32_t a_kb, uint32_t sB, uint32_t b_kb, int nkb, int swizzle, int ncols,
+                                                uint32_t img, uint32_t pitch)
 {
-    uint32_t d = 0;
-    d |= 2u << 4;                        // c_format = S32
-    d |= (a_signed ? 1u : 0u) << 7;      // a_format
-    d |= (b_signed ? 1u : 0u) << 10;     // b_format
-    d |= (uint32_t)(block_n >> 3) << 17; // n_dim
-    d |= (uint32_t)(BLOCK_M >> 4) << 24; // m_dim
-    return d;
+    const int nch = ncols >> 4, ksteps = swizzle >> 5;
+    for (int mh = 0; mh < 2; mh++)
+        for (int c0 = 0; c0 < nch; c0 += 8)
+        {
+            uint32_t acc[8][8];
+#pragma unroll
+            for (int j = 0; j < 8; j++)
+#pragma unroll
+                for (int r = 0; r < 8; r++) acc[j][r] = 0;
+            wgmma_fence();
+            for (int kb = 0; kb < nkb; kb++)
+            {
+                const uint64_t da = make_smem_desc(sA + (uint32_t)kb * a_kb + (uint32_t)(mh * 64 * swizzle), swizzle);
+                const uint64_t db = make_smem_desc(sB + (uint32_t)kb * b_kb + (uint32_t)(c0 * 16 * swizzle), swizzle);
+                for (int k = 0; k < ksteps; k++)
+#pragma unroll
+                    for (int j = 0; j < 8; j++)
+                        // +32 bytes along K inside the swizzled rows: +2 in 16-byte units; +16 rows of B: +16*swizzle bytes
+                        if (c0 + j < nch) wgmma_n16<AU, BU>(acc[j], da + (uint64_t)(k * 2), db + (uint64_t)(j * swizzle + k * 2), 1u);
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+#pragma unroll
+            for (int j = 0; j < 8; j++)
+                if (c0 + j < nch) frag_to_image(acc[j], img, pitch, mh * 64, (c0 + j) * 16);
+        }
 }
 
 template <bool FUSE>

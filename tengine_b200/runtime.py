@@ -20,7 +20,7 @@ class TB200Error(RuntimeError):
 
 
 def build(verbose=False):
-    """Compile tengine_b200/csrc for sm_100a (nvcc cross-compiles without a GPU)."""
+    """Compile tengine_b200/csrc for sm_90a (nvcc cross-compiles without a GPU)."""
     r = subprocess.run(["make", "-C", os.path.join(_HERE, "csrc")], capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("building libtengine_b200.so failed:\n" + r.stdout[-3000:] + r.stderr[-3000:])
@@ -34,7 +34,7 @@ def lib():
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise ImportError(f"{LIB_PATH} not found: run `python -c 'import __graft_entry__ as g; g.build()'` "
-                              "(the B200 backend has no CPU fallback)")
+                              "(the H100 backend has no CPU fallback)")
         L = C.CDLL(LIB_PATH)
         L.tb200_last_error.restype = C.c_char_p
         L.tb200_graph_layer_kernel.restype = C.c_char_p

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run with -m gpu)")
     # On a multi-GPU box some tests reach the library's NCCL path through the Tengine runtime (not through tengine_b200/runtime.py,
     # which maps torch's bundled NCCL first): do the same here, once, so that a later `import torch` in this process still finds
     # the NCCL build it was linked against (a process can hold only one libnccl.so.2).

@@ -43,7 +43,7 @@ def test_no_cpu_fallback_without_gpu():
     from tengine_b200 import runtime as rt
 
     if rt.device_count() > 0:
-        pytest.skip("a B200 is visible")
+        pytest.skip("an H100 is visible")
     with pytest.raises(rt.TB200Error) as e:
         rt.Context(0)
     assert e.value.code == abi.ERR_NO_DEVICE

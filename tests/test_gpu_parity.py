@@ -1,6 +1,6 @@
 """Parity of the CUDA path against the CPU oracle and the committed reference fixtures, through the C ABI
 (tb200_graph_prerun / run / read_tensor).  Bar: bit-exact for int8; uint8 bit-exact against the exact-integer
-oracle (mode 0) and within +-1 LSB of the reference's fp32 simulation.  Needs a B200: run with `-m gpu`."""
+oracle (mode 0) and within +-1 LSB of the reference's fp32 simulation.  Needs an H100: run with `-m gpu`."""
 import numpy as np
 import pytest
 
@@ -160,6 +160,9 @@ CONV_CASES = [
     (2, 32, 21, 19, 64, 3, 1, 1, 1),    # 32-channel 3x3 (window kernel, NHWC 32 B/pixel), ragged tiles
     (2, 24, 18, 18, 40, 3, 2, 1, 1),    # 24 real channels in a 32-byte pixel: pad lanes must stay out of the uint8 sums
     (1, 12, 20, 20, 16, 3, 1, 1, 1),    # 12 real channels in a 16-byte pixel
+    (2, 32, 18, 18, 256, 3, 2, 1, 1),   # 32-channel 3x3 whose window kernel would not fit shared memory (implicit GEMM)
+    (1, 32, 17, 17, 192, 3, 1, 1, 1),   # the same at stride 1
+    (1, 16, 14, 14, 256, 3, 2, 1, 1),   # 16-channel 3x3, wide output: the global-memory gather kernel
 ]
 
 

@@ -33,18 +33,6 @@ def test_inplace_scales_mirror_the_quantisation_tool():
     assert any(L["op"] == abi.OP_POOL and g3.tensors[L["inputs"][0]]["scale"] != g3.tensors[L["output"]]["scale"] for L in g3.layers)
 
 
-def test_bench_traffic_comes_from_the_committed_capture():
-    sys.path.insert(0, ROOT)
-    import bench
-
-    newest = [n for n in ("r02_ncu_traffic.json", "r01_ncu_traffic.json") if os.path.exists(os.path.join(ROOT, "profiles", n))][0]
-    d = json.load(open(os.path.join(ROOT, "profiles", newest)))
-    fam = next(iter(d["families"]))
-    assert bench.ncu_traffic(d["workload"], d["batch"], fam) == pytest.approx(d["families"][fam]["dram_bytes_per_step"])
-    assert bench.ncu_traffic(d["workload"], d["batch"] + 1, fam) is None  # another batch: no claim
-    assert bench.ncu_traffic("resnet50_int8", d["batch"], fam) is None
-
-
 def test_reference_worker_is_torch_free_and_reports_json(tmp_path):
     """bench.py's reference arm runs `python -m oracle.ref_worker` once per CPU: it must not import torch (start-up time x
     128 processes) and must print one JSON line."""
@@ -66,18 +54,51 @@ def test_reference_worker_is_torch_free_and_reports_json(tmp_path):
     assert out["images"] == 2 and out["loop_s"] > 0 and out["min_ms"] > 0
 
 
-def test_ncu_traffic_tool_reproduces_the_committed_traffic_file(tmp_path):
-    """tools/ncu_traffic_json.py on the committed per-launch summary of round 1's whole-step capture gives the committed per-family
-    DRAM bytes (the numbers bench.py reports as roofline.traffic)."""
+def test_ncu_traffic_tool_reproduces_the_stored_traffic_file(tmp_path):
+    """tools/ncu_traffic_json.py on a stored per-launch summary of one whole MobileNet-v1 int8 step (batch 256) gives the stored
+    per-family DRAM bytes and launch counts (tests/golden/ncu_*: an Nsight Compute capture of an earlier build, used as input data)."""
     import subprocess
 
     out = tmp_path / "t.json"
-    r = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "ncu_traffic_json.py"), os.path.join(ROOT, "profiles", "r01_final_ncu_full_summary.csv"),
-                        str(out), "mobilenet_v1_int8", "256"], capture_output=True, text=True)
+    r = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "ncu_traffic_json.py"),
+                        os.path.join(ROOT, "tests", "golden", "ncu_summary_mobilenet_v1_int8_b256.csv"), str(out), "mobilenet_v1_int8", "256"],
+                       capture_output=True, text=True)
     assert r.returncode == 0, r.stderr
     got = json.load(open(out))
-    want = json.load(open(os.path.join(ROOT, "profiles", "r01_ncu_traffic.json")))
+    want = json.load(open(os.path.join(ROOT, "tests", "golden", "ncu_traffic_mobilenet_v1_int8_b256.json")))
     for fam, f in want["families"].items():
         assert fam in got["families"], fam
         assert got["families"][fam]["launches_per_step"] == f["launches_per_step"]
         assert got["families"][fam]["dram_bytes_per_step"] == pytest.approx(f["dram_bytes_per_step"], rel=1e-6)
+
+
+def test_dump_outputs_stays_within_the_limit_and_is_reproducible(tmp_path, monkeypatch):
+    """bench.py --dump-outputs: the files of all outputs together never exceed DUMP_LIMIT bytes, small outputs are stored whole and
+    in shape, an output over its share holds exactly the elements at dump_sample_positions (YOLOv5s-like head sizes, scaled down)."""
+    sys.path.insert(0, ROOT)
+    import bench
+
+    monkeypatch.setattr(bench, "DUMP_LIMIT", 1 << 20)
+    rng = np.random.default_rng(0)
+    ys = [rng.integers(-127, 128, s, dtype=np.int8) for s in ((2, 255, 40, 40), (2, 255, 20, 20), (2, 255, 10, 10))]
+
+    class FakeGraph:
+        def download(self, i, out):
+            out[...] = ys[i]
+
+        def sync(self):
+            pass
+
+    for d in ("a", "b"):
+        bench.dump_outputs(str(tmp_path / d), FakeGraph(), [np.empty_like(y) for y in ys])
+    files = sorted(os.listdir(tmp_path / "a"))
+    assert files == ["output0.npy", "output1.npy", "output2.npy"]
+    assert sum(os.path.getsize(tmp_path / "a" / f) for f in files) <= bench.DUMP_LIMIT
+    for i, (f, y) in enumerate(zip(files, ys)):
+        a, b = np.load(tmp_path / "a" / f), np.load(tmp_path / "b" / f)
+        assert a.dtype == np.float32 and np.array_equal(a, b)
+        if a.shape == y.shape:
+            assert np.array_equal(a, y.astype(np.float32))
+        else:
+            assert a.ndim == 1 and np.array_equal(a, y.reshape(-1)[bench.dump_sample_positions(y.size, a.size, i)].astype(np.float32))
+    assert np.load(tmp_path / "a" / "output0.npy").ndim == 1  # the large head was sampled

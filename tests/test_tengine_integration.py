@@ -1,5 +1,5 @@
 """The drop-in boundary, end to end: the REAL Tengine runtime (unmodified reference sources + the B200 nn_device of
-tengine_b200/device/, built by integration/build_tengine_b200.py into build/tengine/) executes graphs on device "B200"
+tengine_b200/device/, built by integration/build_tengine_b200.py into oracle/_ref/tengine/) executes graphs on device "B200"
 through init_tengine()/create_graph()/prerun_graph_multithread()/run_graph(), and the UNMODIFIED example binaries
 tm_classification_int8 / tm_benchmark run against it.  Results are compared with the same library's CPU device."""
 import os
@@ -10,7 +10,7 @@ import numpy as np
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-BUILD = os.path.join(ROOT, "build", "tengine")
+BUILD = os.path.join(ROOT, "oracle", "_ref", "tengine")
 MODELS = os.path.join(ROOT, "oracle", "_ref", "models")
 
 
@@ -40,7 +40,7 @@ def test_integration_library_registers_b200_and_fails_loudly_without_gpu(tmp_pat
     from tengine_b200 import runtime as rt
 
     if rt.device_count() > 0:
-        pytest.skip("a B200 is visible")
+        pytest.skip("an H100 is visible")
     out = tmp_path / "o.npz"
     r = subprocess.run([sys.executable, os.path.join(ROOT, "integration", "run_fixture.py"), "ref_tiny_int8", "B200", str(out)],
                        capture_output=True, text=True)
@@ -161,7 +161,6 @@ def test_full_size_tmfile_through_run_graph_on_b200(oracle, tmp_path, name, gpus
     (The file is written HERE from the graph the oracle gets: the workloads' activation scales come from a torch fp32
     calibration pass whose last bit depends on the host CPU, so a file made on another machine describes a slightly different
     network -- that, not the device, was the 1-LSB difference this test showed with pre-generated files.)"""
-    from oracle.pyoracle import Reference, run_tmfile, save_tmfile
     from tengine_b200 import runtime as rt
 
     if not _have_integration():
@@ -169,10 +168,28 @@ def test_full_size_tmfile_through_run_graph_on_b200(oracle, tmp_path, name, gpus
     g, b, outs = _tmfile_case(name)
     x = b.random_input(21)
     path = str(tmp_path / (name + ".tmfile"))
-    ref = Reference(libdir=BUILD)  # one Tengine library in the process: it writes the file and runs it
-    save_tmfile(ref, g, path)
+    # A fresh process holds ONE Tengine library, the integration build: it writes the file and runs it.  (In this process another
+    # test may already have mapped the plain reference library, whose soname is the same, so the dynamic loader would hand that
+    # one -- without the B200 device -- to the integration build's shim.)
+    d = g.to_dict()
+    d["input"] = x
+    npz, out_npz = str(tmp_path / "case.npz"), str(tmp_path / "got.npz")
+    np.savez(npz, **d)
     env = {"TG_B200_GPU_LIST": "0,0"} if (gpus == 2 and rt.device_count() < 2) else {}
-    got, ms = run_tmfile(ref, path, x, [g.dims(t) for t in outs], device="B200", num_gpus=gpus if gpus > 1 else 0, env=env, warmup=1, loops=2)
+    code = ("import sys, numpy as np\n"
+            "from oracle.pyoracle import Reference, run_tmfile, save_tmfile\n"
+            "from tengine_b200.graphdef import GraphDef\n"
+            "npz, path, out, libdir, gpus = sys.argv[1:6]\n"
+            "d = dict(np.load(npz)); g = GraphDef.from_dict(d)\n"
+            "ref = Reference(libdir=libdir)\n"
+            "save_tmfile(ref, g, path)\n"
+            "got, ms = run_tmfile(ref, path, d['input'], [g.dims(t) for t in g.outputs], device='B200', num_gpus=int(gpus), env=%r, warmup=1, loops=2)\n"
+            "np.savez(out, *got)\n" % env)
+    r = subprocess.run([sys.executable, "-c", code, npz, path, out_npz, BUILD, str(gpus if gpus > 1 else 0)], cwd=ROOT,
+                       env=dict(os.environ, PYTHONPATH=ROOT), capture_output=True, text=True, timeout=600)
+    assert r.returncode == 0, r.stderr[-2000:]
+    saved = np.load(out_npz)
+    got = [saved[f"arr_{i}"] for i in range(len(outs))]
     want = oracle.run(g, [x], uint8_mode=0)
     for o, t in zip(got, outs):
         assert np.array_equal(o, want[t]), (name, t, int(np.abs(o.astype(int) - want[t].astype(int)).max()))

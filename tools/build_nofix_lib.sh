@@ -5,8 +5,8 @@
 set -e
 cd "$(dirname "$0")/../tengine_b200/csrc"
 mkdir -p ../../build/nofix
-FLAGS="-gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-fvisibility=hidden --expt-relaxed-constexpr -DTB200_TIE_EPS=-1.0f"
+FLAGS="-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-fvisibility=hidden --expt-relaxed-constexpr -DTB200_TIE_EPS=-1.0f"
 for f in engine kernels_direct gemm_tcgen05 dw_tma conv_window yolo_detect conv_fp32; do nvcc $FLAGS -c $f.cu -o ../../build/nofix/$f.o & done
 wait
-nvcc -gencode arch=compute_100a,code=sm_100a -shared -o ../../build/nofix/libtengine_b200_nofix.so ../../build/nofix/*.o -ldl
+nvcc -gencode arch=compute_90a,code=sm_90a -shared -o ../../build/nofix/libtengine_b200_nofix.so ../../build/nofix/*.o -ldl
 echo built build/nofix/libtengine_b200_nofix.so

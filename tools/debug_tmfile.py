@@ -29,7 +29,7 @@ def run(route):
         print("kernels:", gr.layer_kernels(), file=sys.stderr)
         gr.close()
     else:
-        ref = Reference(libdir=os.path.join(ROOT, "build", "tengine"))
+        ref = Reference(libdir=os.path.join(ROOT, "oracle", "_ref", "tengine"))
         got, _ = run_tmfile(ref, os.path.join(ROOT, "oracle/_ref/models/resnet50_uint8.tmfile"), x, [g.dims(t) for t in outs], device="B200")
     for o, t, nm in zip(got, outs, ("prob", "fc")):
         d = np.abs(o.astype(int) - want[t].astype(int))

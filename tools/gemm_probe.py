@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""On-GPU probe of the tcgen05 GEMM path: for each 1x1-conv shape run the tensor-core path and the CUDA-core
+"""On-GPU probe of the tensor-core GEMM path: for each 1x1-conv shape run the tensor-core path and the CUDA-core
 cross-check path through the C ABI and compare bytes.  Each shape runs in its own subprocess so that a device trap in one
 configuration does not poison the others.  Usage: python tools/gemm_probe.py [--one n,c,h,w,oc]"""
 import os
@@ -46,7 +46,7 @@ def one(shape):
     got = gr.run([xin])[0]
     gr.close()
     bad = got != ref
-    print(f"  tcgen05 vs cudacore mismatches {bad.sum()} / {ref.size}", flush=True)
+    print(f"  tensor-core vs cudacore mismatches {bad.sum()} / {ref.size}", flush=True)
     if bad.any():
         idx = np.argwhere(bad)
         print("  first bad (n,oc,h,w):", idx[:6].tolist(), "got", got[bad][:6].tolist(), "want", ref[bad][:6].tolist())

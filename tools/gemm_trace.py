@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Per-role waiting time of every tcgen05 GEMM launch of a workload (debug aid; TB200_GEMM_TRACE=1 makes the launcher
+"""Per-role waiting time of every tensor-core GEMM launch of a workload (debug aid; TB200_GEMM_TRACE=1 makes the launcher
 synchronise and print cycle counters, so the graph is built without CUDA-graph capture)."""
 import os
 import sys

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
-"""Summarise an .ncu-rep (ncu -i ... --page raw --csv) into one CSV row per kernel launch: the columns the DESIGN.md
-roofline table and bench.py's `roofline.traffic` are derived from.  usage: ncu_summary.py <rep> [out.csv]"""
+"""Summarise an .ncu-rep (ncu -i ... --page raw --csv) into one CSV row per kernel launch (time, DRAM bytes, pipe
+utilisation, stall reasons); tools/ncu_traffic_json.py condenses it per kernel family.  usage: ncu_summary.py <rep> [out.csv]"""
 import csv
 import subprocess
 import sys

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
-"""Condense an ncu_summary.py CSV of ONE whole-batch step into profiles/rNN_ncu_traffic.json -- per kernel family (bench.py's
-`graph.layer_kernels()` names) the DRAM bytes and ncu time of its launches -- which bench.py's `roofline.traffic` reads.
+"""Condense an ncu_summary.py CSV of ONE whole-batch step into a JSON file -- per kernel family (bench.py's
+`graph.layer_kernels()` names) the DRAM bytes and ncu time of its launches.
 usage: ncu_traffic_json.py <summary.csv> <out.json> <workload> <batch> [first_row] [n_rows]   (rows select one step of the capture)"""
 import csv
 import json
