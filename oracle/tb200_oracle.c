@@ -481,10 +481,10 @@ ORACLE_API int tb200_oracle_concat(const tb200_tensor_desc* const* tins, const v
                 const size_t src = (size_t)n * C * HW + i, dst = ((size_t)n * OC + coff) * HW + i;
                 if (is_u8)
                 {
-                    /* concat_kernel_ref_uint8.c: dequant with input (scale,zp), requant with output (scale,zp) */
+                    /* concat_kernel_ref_uint8.c:82: roundf((q - zp_in) * (s_in/s_out) + zp_out) -- zp inside the rounding */
                     uint8_t q = ((const uint8_t*)xs[k])[src];
-                    float f = ((float)q - (float)t->zero_point) * t->scale;
-                    int u = round(f / tout->scale) + tout->zero_point;
+                    float rescale = t->scale / tout->scale;
+                    int u = roundf((float)((int)q - t->zero_point) * rescale + (float)tout->zero_point);
                     if (u > 255) u = 255;
                     else if (u < 0) u = 0;
                     ((uint8_t*)y)[dst] = (uint8_t)u;

@@ -22,6 +22,7 @@
 #include "ptx.cuh"
 #include "tc_common.cuh"
 
+#include <cstdio>
 #include <cstdlib>
 #include <cstring>
 
@@ -388,6 +389,7 @@ cudaError_t launch_conv_window(const WindowPlan& p, const void* w, void* out, co
             cudaError_t err = cudaFuncSetAttribute(conv_window_tc_kernel<MD, U, LY>, cudaFuncAttributeMaxDynamicSharedMemorySize, WINDOW_SMEM_MAX); \
             if (err != cudaSuccess) return err;                                                                                             \
         }                                                                                                                                   \
+        if (debug_launch()) fprintf(stderr, "tengine_b200: launch conv_window_tc_kernel<MODE=%d,U8=%d,LAYOUT=%d>\n", MD, (int)U, LY);     \
         conv_window_tc_kernel<MD, U, LY><<<grid, 128, (size_t)p.smem_bytes, st>>>(tm, a, e);                                                \
         return cudaGetLastError();                                                                                                          \
     }

@@ -27,7 +27,7 @@ using namespace tb200;
 
 #define TB200_OP_NOP_ (-1)  // planner-internal: a node folded into its producer
 #define TB200_OP_LUT2_ (-2) // planner-internal: Sigmoid + Eltwise-PROD with the Sigmoid's input, as one byte table
-#define TB200_PACK_FORMAT 3  // bump whenever the layout of the packed weight arena changes (pack cache key)
+#define TB200_PACK_FORMAT 4  // bump whenever the layout or content of the packed weight arena changes (pack cache key)
 
 // ---- packed-weight cache directory (SURVEY.md 8(f)-3): tb200_pack_cache_dir() or the environment ----
 static std::string g_pack_cache_dir;
@@ -1110,7 +1110,8 @@ static int prerun_one(tb200_context* ctx, const tb200_tensor_desc* tensors, int 
             if (kind[li] == K_CONCAT_PART)
             {
                 // per-input requantisation of concat_kernel_ref_int8.c:70-80 (roundf(q * (s_in / s_out)), including its clamp of
-                // values below -127 to +127) and concat_kernel_ref_uint8.c (dequantise, round(f / s_out) + zp, clamp) as byte tables
+                // values below -127 to +127) and concat_kernel_ref_uint8.c:82 (roundf((q - zp_in) * (s_in / s_out) + zp_out), the zero
+                // point inside the rounding, clamp) as byte tables
                 const tb200_tensor_desc& to = g->tensors[L.output].d;
                 for (int k = 0; k < L.num_inputs && k < 4; k++)
                 {
@@ -1121,9 +1122,10 @@ static int prerun_one(tb200_context* ctx, const tb200_tensor_desc* tensors, int 
                         int q;
                         if (ti.data_type == TB200_DT_UINT8)
                         {
-                            volatile float f = ((float)b - (float)ti.zero_point) * ti.scale;
-                            volatile float t = f / to.scale;
-                            q = (int)roundf(t) + to.zero_point;
+                            volatile float rs = ti.scale / to.scale;
+                            volatile float f = (float)(b - ti.zero_point) * rs;
+                            volatile float t = f + (float)to.zero_point;
+                            q = (int)roundf(t);
                             q = q > 255 ? 255 : (q < 0 ? 0 : q);
                         }
                         else

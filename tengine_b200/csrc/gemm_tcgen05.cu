@@ -957,6 +957,7 @@ cudaError_t launch_stem_tc(const DwPlan& plan, const void* in, const void* w, vo
     {                                                                                                                          \
         cudaError_t err = cudaFuncSetAttribute(stem_tc_kernel<MD, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
         if (err != cudaSuccess) return err;                                                                                    \
+        if (debug_launch()) fprintf(stderr, "tengine_b200: launch stem_tc_kernel<MODE=%d,TMA_IN=%d>\n", MD, (int)T);         \
         stem_tc_kernel<MD, T><<<grid, 128, smem, st>>>(tm, a, e);                                                              \
         return cudaGetLastError();                                                                                             \
     }
@@ -1203,6 +1204,7 @@ cudaError_t launch_conv_gather_tc(const void* in, const void* w, void* out, cons
             cudaError_t err = cudaFuncSetAttribute(conv_gather_tc_kernel<MD, U, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
             if (err != cudaSuccess) return err;                                                                                    \
         }                                                                                                                          \
+        if (debug_launch()) fprintf(stderr, "tengine_b200: launch conv_gather_tc_kernel<MODE=%d,U8=%d,KHW=%d>\n", MD, (int)U, K);  \
         conv_gather_tc_kernel<MD, U, K><<<grid, 128, smem, st>>>(a, e);                                                            \
         return cudaGetLastError();                                                                                                 \
     }
@@ -1435,6 +1437,12 @@ static int encode_2d(void* tmap, const void* base, uint64_t inner, uint64_t rows
 
 // Where the uint8 path's sum(x) comes from (TB200_U8_SX, A/B switch): 3 (default) = two extra warps add up the rows of the A tiles,
 // 0 = 16 rows of ones in every B tile (sum(x) is then a 17th..32nd accumulator column; costs image columns and m-tiles per stage).
+bool debug_launch()
+{
+    static const bool on = getenv("TB200_DEBUG_LAUNCH") != nullptr;
+    return on;
+}
+
 int gemm_sx_mode()
 {
     static const int mode = [] { const char* e = getenv("TB200_U8_SX"); return (e && atoi(e) == 0) ? 0 : 3; }();
@@ -1695,6 +1703,7 @@ static cudaError_t launch_gemm_simple(const GemmPlan& p, const EpiParams& e, int
             cudaError_t err = cudaFuncSetAttribute(gemm_simple_kernel<MD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
             if (err != cudaSuccess) return err;                                                                                \
         }                                                                                                                      \
+        if (debug_launch()) fprintf(stderr, "tengine_b200: launch gemm_simple_kernel<MODE=%d>\n", MD);                          \
         gemm_simple_kernel<MD><<<grid, 128, smem, st>>>(ta, tb, g, e);                                                         \
         return cudaGetLastError();                                                                                             \
     }
@@ -1730,7 +1739,7 @@ cudaError_t launch_gemm_i8(const GemmPlan& p, const EpiParams& e, const int32_t*
                         (size_t)EPI_WARPS * 2 * 512 * (p.cs == 8 ? 4 : p.cs) + sizeof(GemmSmemCtl) +
                         (size_t)(g.par_all ? par_ch : p.block_n) * 8 + 16 + 128 * (size_t)acc_pitch(p.mt * g.tcols) + 1024;
     static const bool trace_on = getenv("TB200_GEMM_TRACE") != nullptr;
-    static const bool launch_dbg = getenv("TB200_DEBUG_LAUNCH") != nullptr;
+    const bool launch_dbg = debug_launch();
     static unsigned long long* trace_buf = nullptr;
     g.trace = nullptr;
     if (trace_on)
@@ -1759,6 +1768,9 @@ cudaError_t launch_gemm_i8(const GemmPlan& p, const EpiParams& e, const int32_t*
             if (launch_dbg) gemm_launch_debug((const void*)gemm_i8_tcgen05_kernel<U, MD, C, B>, "set attribute", err, grid, smem, st);    \
             if (err != cudaSuccess) return err;                                                                                \
         }                                                                                                                      \
+        if (launch_dbg)                                                                                                        \
+            fprintf(stderr, "tengine_b200: launch gemm_i8_tcgen05_kernel<U8=%d,MODE=%d,CS=%d,BORDER=%d> out_mode=%d conv=%d n_tiles=%d b_res=%d fixq=%d\n", \
+                    (int)U, MD, C, (int)B, p.out_mode, p.conv, p.n_tiles, p.b_res, p.fixq != nullptr);                      \
         gemm_i8_tcgen05_kernel<U, MD, C, B><<<grid, U ? GEMM_THREADS_U8 : GEMM_THREADS, smem, st>>>(ta, tb, to, tt, g, e);                           \
         if (trace_on) gemm_trace_report(p, g, grid, st);                                                                       \
         err = cudaGetLastError();                                                                                              \

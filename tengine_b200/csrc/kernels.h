@@ -142,6 +142,9 @@ static inline int current_device()
 }
 int gemm_block_n(int ocp, int u8);
 int gemm_sx_mode();                  // TB200_U8_SX: where the uint8 path's sum(x) comes from (gemm_tcgen05.cu)
+// TB200_DEBUG_LAUNCH (read once per process): the templated launchers print one stderr line per launch naming the instantiation,
+// "tengine_b200: launch <kernel><ARG=value,...>"; diagnostic only, changes nothing else
+bool debug_launch();
 int gemm_tile_rows(int ocp, int u8); // rows of one packed B tile (u8 = 1 + weight zero point, 0 for int8)
 int gemm_plan_create(GemmPlan* plan, const void* a, long long lda, const void* b, void* out, long long m, int k, int oc, int ocp, int ldo,
                      int variant, int u8);

@@ -598,7 +598,7 @@ __global__ void __launch_bounds__(256) pointwise_fast_kernel(const uint4* __rest
 }
 
 // concat along channels with per-input requantisation (concat_kernel_ref_int8.c:70-80 roundf(q*s_in/s_out),
-// concat_kernel_ref_uint8.c dequant/requant), and nearest upsample (upsample_ref.c:74); one byte per thread
+// concat_kernel_ref_uint8.c:82 roundf((q-zp)*s_in/s_out + zp_out)), and nearest upsample (upsample_ref.c:74); one byte per thread
 // (channel counts such as 255 / 384 need not be multiples of 4 at the seams).
 template <bool U8>
 __global__ void __launch_bounds__(256) concat_kernel(const uint8_t* __restrict__ in, uint8_t* __restrict__ out,
@@ -619,8 +619,9 @@ __global__ void __launch_bounds__(256) concat_kernel(const uint8_t* __restrict__
     int q;
     if (U8)
     {
-        const float f = __fmul_rn((float)v - (float)z_in, s_in);
-        q = clamp_u8((int)roundf(__fdiv_rn(f, s_out)) + z_out);
+        // concat_kernel_ref_uint8.c:82: roundf((q - zp_in) * (s_in / s_out) + zp_out), the zero point inside the rounding
+        const float f = __fmul_rn((float)((int)v - z_in), __fdiv_rn(s_in, s_out));
+        q = clamp_u8((int)roundf(__fadd_rn(f, (float)z_out)));
     }
     else
     {

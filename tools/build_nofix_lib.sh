@@ -1,7 +1,9 @@
 #!/bin/bash
 # Timing experiment only: the library with the tie guard disabled (TB200_TIE_EPS = -1: no element ever takes the literal rare path,
 # so ~2.4e-4 of the bytes may be off by one).  Used through TB200_LIB to measure what the rare path costs the epilogue warps
-# (an epilogue warp inside it holds up its accumulator stage).  Never shipped, never used by tests or bench defaults.
+# (an epilogue warp inside it holds up its accumulator stage).  Also the mutation check of the tie tests:
+#   TB200_LIB=build/nofix/libtengine_b200_nofix.so python -m pytest tests/test_gpu_requant_ties.py -m gpu
+# must fail every tie-dense case of a fast epilogue (exact-epilogue, LUT and tb200k_* cases still pass).  Never shipped.
 set -e
 cd "$(dirname "$0")/../tengine_b200/csrc"
 mkdir -p ../../build/nofix
