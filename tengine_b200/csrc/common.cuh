@@ -371,78 +371,6 @@ __device__ __forceinline__ uint32_t requant_fix_byte(uint32_t word, int j, int32
     return (word & ~(0xffu << (8 * j))) | (q << (8 * j));
 }
 
-// uint8 flavour of requant_fast8_i8: the reference's chain is f = fl(fl(acc*S) + bias_term), activation clip, q = round(f / s_out)
-// + zero point, saturate.  f is formed with the reference's own two roundings (packed FMUL2 + FADD2); only the division is
-// replaced by a multiplication with fl(1/s_out) (|t - t_ref| <= 3*2^-24*|t|); clip, zero point and saturation are one DPX
-// instruction per channel pair after the rounding (q_add2 carries the zero point).  `a` are TRUE accumulators
-// sum (x-zx)(w-zw); bt = the per-channel bias terms.
-__device__ __forceinline__ void requant_fast8_u8(const int32_t (&a)[8], const float (&bt)[8], const EpiParams& e, uint32_t& w0, uint32_t& w1,
-                                                 float& g0, float& g1)
-{
-    const uint64_t mg = f2_pack(TB200_MAGIC, TB200_MAGIC);
-    const uint64_t S2 = f2_pack(e.in_w_scale, e.in_w_scale), R2 = f2_pack(e.fast_r, e.fast_r);
-    uint64_t f[4], t[4], r[4], s[4], d[4];
-#pragma unroll
-    for (int k = 0; k < 4; k++) f[k] = f2_mul(f2_pack((float)a[2 * k], (float)a[2 * k + 1]), S2);
-#pragma unroll
-    for (int k = 0; k < 4; k++) f[k] = f2_add(f[k], f2_pack(bt[2 * k], bt[2 * k + 1]));
-#pragma unroll
-    for (int k = 0; k < 4; k++) t[k] = f2_mul(f[k], R2);
-#pragma unroll
-    for (int k = 0; k < 4; k++) r[k] = f2_add(t[k], mg);
-#pragma unroll
-    for (int k = 0; k < 4; k++) s[k] = f2_sub(r[k], mg);
-#pragma unroll
-    for (int k = 0; k < 4; k++) d[k] = f2_sub(t[k], s[k]);
-    float dl[4], dh[4];
-    uint32_t rl[4], rh[4];
-#pragma unroll
-    for (int k = 0; k < 4; k++) f2_unpack(d[k], dl[k], dh[k]), f2_unpack_bits(r[k], rl[k], rh[k]);
-    g0 = fmaxf(fmaxf(fabsf(dl[0]), fabsf(dh[0])), fmaxf(fabsf(dl[1]), fabsf(dh[1])));
-    g1 = fmaxf(fmaxf(fabsf(dl[2]), fabsf(dh[2])), fmaxf(fabsf(dl[3]), fabsf(dh[3])));
-    uint32_t q[4];
-#pragma unroll
-    for (int k = 0; k < 4; k++) q[k] = __viaddmin_s16x2_relu(__byte_perm(rl[k], rh[k], 0x5410), e.q_add2, e.q_max2);
-    w0 = __byte_perm(q[0], q[1], 0x6420), w1 = __byte_perm(q[2], q[3], 0x6420);
-}
-
-// 16 channels of one uint8 output row: acc = TRUE accumulators, par = (bias term, -) per channel as loaded from the arena layout
-// float2[OCp].  Returns the four packed words; pad lanes (oc0 + k >= oc_limit) come out 0.
-__device__ __forceinline__ void requant_unit16_u8(const int32_t (&acc)[16], const float (&bt)[16], int oc0, int oc_limit, const EpiParams& e,
-                                                  uint32_t (&w)[4])
-{
-    float gw[4];
-#pragma unroll
-    for (int h = 0; h < 2; h++)
-    {
-        const int32_t a8[8] = {acc[h * 8], acc[h * 8 + 1], acc[h * 8 + 2], acc[h * 8 + 3], acc[h * 8 + 4], acc[h * 8 + 5], acc[h * 8 + 6], acc[h * 8 + 7]};
-        const float b8[8] = {bt[h * 8], bt[h * 8 + 1], bt[h * 8 + 2], bt[h * 8 + 3], bt[h * 8 + 4], bt[h * 8 + 5], bt[h * 8 + 6], bt[h * 8 + 7]};
-        requant_fast8_u8(a8, b8, e, w[2 * h], w[2 * h + 1], gw[2 * h], gw[2 * h + 1]);
-    }
-    if (e.q_byte_add)
-    {
-#pragma unroll
-        for (int j = 0; j < 4; j++) w[j] = requant_byte_fix(w[j], e);
-    }
-    if (fmaxf(fmaxf(gw[0], gw[1]), fmaxf(gw[2], gw[3])) > 0.5f - TB200_TIE_EPS)
-    {
-#pragma unroll
-        for (int j = 0; j < 4; j++)
-            if (gw[j] > 0.5f - TB200_TIE_EPS)
-            {
-#pragma unroll
-                for (int t = 0; t < 4; t++) w[j] = requant_fix_byte(w[j], t, acc[j * 4 + t], oc0 + j * 4 + t, e);
-            }
-    }
-    if (oc0 + 16 > oc_limit)
-    {
-        // pad lanes of uint8 tensors hold 0, not the zero point
-#pragma unroll
-        for (int k = 0; k < 16; k++)
-            if (oc0 + k >= oc_limit) w[k >> 2] &= ~(0xffu << (8 * (k & 3)));
-    }
-}
-
 // Generic entry for kernels that handle one word (4 channels oc0..oc0+3) at a time with constants in global memory.
 // Pad channels (>= oc_limit) have m = 0, y = 0 in fast_par and therefore produce 0.
 template <bool U8>

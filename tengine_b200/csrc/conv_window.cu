@@ -1,10 +1,11 @@
-// conv_window.cu -- small-Cin convolutions on the tensor cores with a TMA-staged input window.
+// conv_window.cu -- small-Cin convolutions on the tensor cores: the window kernel (TMA-staged input window) and the gather
+// kernel (taps gathered from global memory) it falls back to.
 //
 // The layers an implicit GEMM over 4-D TMA boxes serves badly: the NCHW network input (C <= 3; 3x3 and 7x7 stems, int8 and
 // uint8) and 3x3 convolutions over NHWC tensors with 16 or 32 channels (YOLOv3-tiny's second and third layer).  Their K rows
 // are 16-32 bytes per tap, and the TMA unit's cost is per row, not per byte: feeding nine shifted
 // 128-row boxes per tile through it left the tensor pipe idle 90% of the time, and gathering every tap from global memory
-// with bounds predicates (round 1's conv_gather_tc_kernel) cost more instructions than the whole epilogue.
+// with bounds predicates (conv_gather_tc_kernel below) costs more instructions than the whole epilogue.
 //
 // Here a CTA (128 threads = 16 x 8 output pixels) receives the input window of its tile ONCE -- one 4-D cp.async.bulk.tensor
 // load, double-buffered, out-of-image coordinates zero-filled by the TMA unit = the convolution's padding -- and every thread
@@ -39,6 +40,21 @@ struct WindowArgs
     int box_w, box_h, xoff, in_bytes, ks;
     uint32_t fill; // uint8: the input zero point replicated x4 (0 for int8: the TMA zero fill already is the padding)
 };
+
+// The B tiles (weights [OCp][ks*32] -> one SW32 K-major tile of OCp rows per k-step) and the epilogue constants into shared
+// memory: identical for every CTA, L2 resident.  Int8 MODE 2 reads no constants.
+template <int MODE, bool U8>
+__device__ __forceinline__ void stage_b_and_constants(const uint8_t* w, int ks, int ocp, uint32_t sB, uint32_t sPar, const EpiParams& e)
+{
+    const uint32_t b_tile = (uint32_t)ocp * 32u;
+    for (int i = threadIdx.x; i < ks * ocp * 2; i += 128)
+    {
+        const int kb = i / (ocp * 2), j = i - kb * (ocp * 2), r = j >> 1, c16 = j & 1;
+        const uint4 v = __ldg(reinterpret_cast<const uint4*>(w + ((size_t)r * ks + kb) * 32) + c16);
+        sts_u4(sB + (uint32_t)kb * b_tile + sw32_offset(r, c16), v.x, v.y, v.z, v.w);
+    }
+    for (int c = threadIdx.x; c < ocp; c += 128) sts_f2(sPar + c * 8, (MODE != 2 || U8) ? __ldg(e.fast_par + c) : make_float2(0.f, 0.f));
+}
 
 // LAYOUT: 0 NCHW 3x3, 1 NCHW 7x7, 2 NHWC 16 bytes per pixel (3x3), 3 NHWC 32 bytes per pixel (3x3)
 template <int MODE, bool U8, int LAYOUT> // MODE: 0 fast, 1 fast + fused bias (int8), 2 exact
@@ -86,14 +102,7 @@ __global__ void __launch_bounds__(128) conv_window_tc_kernel(const __grid_consta
                         oh0_ * a.stride - a.ph, n_);                                                                                    \
     } while (0)
     if (tid == 0 && blockIdx.x < a.ntiles) TB200_WIN_LOAD_TILE(blockIdx.x, 0);
-    // ---- B tiles (one per k-step) and the epilogue constants: identical for every CTA, L2 resident ----
-    for (int i = tid; i < a.ks * a.ocp * 2; i += 128)
-    {
-        const int kb = i / (a.ocp * 2), j = i - kb * (a.ocp * 2), r = j >> 1, c16 = j & 1;
-        const uint4 v = __ldg(reinterpret_cast<const uint4*>(a.w + ((size_t)r * a.ks + kb) * 32) + c16);
-        sts_u4(sB + (uint32_t)kb * b_tile + sw32_offset(r, c16), v.x, v.y, v.z, v.w);
-    }
-    for (int c = tid; c < a.ocp; c += 128) sts_f2(sPar + c * 8, (MODE != 2 || U8) ? __ldg(e.fast_par + c) : make_float2(0.f, 0.f));
+    stage_b_and_constants<MODE, U8>(a.w, a.ks, a.ocp, sB, sPar, e);
     if (LAYOUT == 2) sts_u4(sA + 4u * 4096u + sw32_offset(tid, 1), 0u, 0u, 0u, 0u); // K = 144 of 160: the last half k-step stays 0
 
     uint32_t it = 0;
@@ -212,81 +221,9 @@ __global__ void __launch_bounds__(128) conv_window_tc_kernel(const __grid_consta
         const int32_t rowc = U8 ? -e.w_zero * sx : 0;
         for (int c = 0; c < a.ocp; c += 16)
         {
-            uint32_t v[16];
+            uint32_t v[16], w[4];
             acc_ld16(tb + 4u * c, v);
-            uint32_t w[4];
-            if (U8)
-            {
-                // the int8 form (engine.cu: constants { M, M, y, y } with y = corr[oc] + bias[oc]): a' = v - zw*sum(x) + y, t = fl(a' * M)
-                if (MODE == 2)
-                {
-#pragma unroll
-                    for (int k = 0; k < 16; k++)
-                    {
-                        if ((k & 3) == 0) w[k >> 2] = 0;
-                        if (c + k < a.oc)
-                        {
-                            const float4 pp = lds_f4(sPar + c * 8 + (k >> 1) * 16);
-                            const int32_t acc = (int32_t)v[k] + rowc + __float_as_int((k & 1) ? pp.w : pp.z) - (e.has_bias ? __ldg(e.bias + c + k) : 0);
-                            w[k >> 2] |= ((uint32_t)requant(acc, c + k, e) & 0xffu) << (8 * (k & 3));
-                        }
-                    }
-                }
-                else
-                {
-                    float gw[4];
-#pragma unroll
-                    for (int h = 0; h < 2; h++)
-                    {
-                        float4 p[4];
-#pragma unroll
-                        for (int k = 0; k < 4; k++) p[k] = lds_f4(sPar + c * 8 + h * 64 + k * 16);
-                        int32_t a8[8];
-#pragma unroll
-                        for (int k = 0; k < 8; k++) a8[k] = (int32_t)v[h * 8 + k] + rowc;
-                        requant_fast8_i8<false>(a8, p, e, w[2 * h], w[2 * h + 1], gw[2 * h], gw[2 * h + 1]);
-                    }
-                    if (e.q_byte_add)
-                    {
-#pragma unroll
-                        for (int j = 0; j < 4; j++) w[j] = requant_byte_fix(w[j], e);
-                    }
-                    if (fmaxf(fmaxf(gw[0], gw[1]), fmaxf(gw[2], gw[3])) > 0.5f - TB200_TIE_EPS)
-                    {
-#pragma unroll
-                        for (int j = 0; j < 4; j++)
-                            if (gw[j] > 0.5f - TB200_TIE_EPS)
-                            {
-                                int32_t at[4]; // accumulator + y of the word's four channels (what the fast path multiplied by M)
-#pragma unroll
-                                for (int t = 0; t < 4; t++)
-                                {
-                                    const float4 pp = lds_f4(sPar + c * 8 + ((j * 4 + t) >> 1) * 16);
-                                    at[t] = (int32_t)v[j * 4 + t] + rowc + __float_as_int((t & 1) ? pp.w : pp.z);
-                                }
-                                w[j] = requant_fix_word_u8(w[j], at[0], at[1], at[2], at[3], c + j * 4, a.oc, e);
-                            }
-                    }
-                    if (c + 16 > a.oc)
-                    {
-                        // pad lanes of uint8 tensors hold 0, not the zero point
-#pragma unroll
-                        for (int k = 0; k < 16; k++)
-                            if (c + k >= a.oc) w[k >> 2] &= ~(0xffu << (8 * (k & 3)));
-                    }
-                }
-            }
-            else if (MODE == 2)
-            {
-#pragma unroll
-                for (int k = 0; k < 16; k++)
-                {
-                    if ((k & 3) == 0) w[k >> 2] = 0;
-                    if (c + k < a.oc) w[k >> 2] |= ((uint32_t)requant((int32_t)v[k], c + k, e) & 0xffu) << (8 * (k & 3));
-                }
-            }
-            else
-                stem_unit_fast<MODE == 1>(v, sPar + c * 8, c, e, w);
+            tc_unit16<MODE, U8>(v, rowc, sPar + c * 8, c, a.oc, e, w);
             if (valid) *reinterpret_cast<uint4*>(op + c) = make_uint4(w[0], w[1], w[2], w[3]);
         }
         // the next tile's MMAs overwrite the accumulator image and its gather overwrites the A tiles
@@ -350,7 +287,7 @@ int window_plan_create(WindowPlan* p, const void* in, const ConvShape& s, int nh
     return 0;
 }
 
-cudaError_t launch_conv_window(const WindowPlan& p, const void* w, void* out, const ConvShape& s, const EpiParams& e, cudaStream_t st)
+cudaError_t launch_conv_window(const WindowPlan& p, const void* w, void* out, const ConvShape& s, const EpiParams& e, int num_sms, cudaStream_t st)
 {
     if (!p.valid) return cudaErrorInvalidValue;
     if ((long long)s.n * s.oh * s.ow >= (1ll << 31)) return cudaErrorInvalidValue; // 32-bit pixel index
@@ -365,30 +302,21 @@ cudaError_t launch_conv_window(const WindowPlan& p, const void* w, void* out, co
     a.th_magic = a.tiles_h == 1 ? 0u : (uint32_t)((1ull << 32) / (unsigned)a.tiles_h) + 1u;
     a.box_w = p.box_w, a.box_h = p.box_h, a.xoff = p.xoff, a.in_bytes = p.in_bytes, a.ks = p.ks;
     a.fill = e.is_uint8 ? ((uint32_t)(e.in_zero & 0xff) * 0x01010101u) : 0u;
-    static int sms = 0;
-    if (!sms)
-    {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    }
-    // several resident CTAs per SM overlap gather / MMA / epilogue of different tiles; each loops over its share
-    int per_sm = (220 * 1024) / p.smem_bytes;
-    if (per_sm > 8) per_sm = 8;
-    if (per_sm < 1) per_sm = 1;
-    const unsigned cap = (unsigned)(sms * per_sm);
-    const unsigned grid = a.ntiles < cap ? a.ntiles : cap;
     const int mode = !e.fast_ok ? 2 : ((!e.is_uint8 && e.fuse_bias) ? 1 : 0);
     CUtensorMap tm;
     memcpy(&tm, p.tmap_in, sizeof tm);
+    // Several resident CTAs per SM overlap gather / MMA / epilogue of different tiles; each loops over its share.  The grid is
+    // exactly the CTAs that can be resident at once (registers and shared memory): a larger one leaves a tail of late CTAs.
 #define TB200_WIN_CASE(MD, U, LY)                                                                                                           \
     if (mode == MD && (e.is_uint8 != 0) == U && p.layout == LY)                                                                             \
     {                                                                                                                                       \
         /* the opt-in is per device AND per context: set it before every launch (launches happen at graph capture only) */ \
-        {                                                                                                                                   \
-            cudaError_t err = cudaFuncSetAttribute(conv_window_tc_kernel<MD, U, LY>, cudaFuncAttributeMaxDynamicSharedMemorySize, WINDOW_SMEM_MAX); \
-            if (err != cudaSuccess) return err;                                                                                             \
-        }                                                                                                                                   \
+        cudaError_t err = cudaFuncSetAttribute(conv_window_tc_kernel<MD, U, LY>, cudaFuncAttributeMaxDynamicSharedMemorySize, WINDOW_SMEM_MAX); \
+        if (err != cudaSuccess) return err;                                                                                                 \
+        int per_sm = 0;                                                                                                                     \
+        err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, conv_window_tc_kernel<MD, U, LY>, 128, (size_t)p.smem_bytes);          \
+        if (err != cudaSuccess) return err;                                                                                                 \
+        const unsigned cap = (unsigned)num_sms * (unsigned)(per_sm > 1 ? per_sm : 1), grid = a.ntiles < cap ? a.ntiles : cap;             \
         if (debug_launch()) fprintf(stderr, "tengine_b200: launch conv_window_tc_kernel<MODE=%d,U8=%d,LAYOUT=%d>\n", MD, (int)U, LY);     \
         conv_window_tc_kernel<MD, U, LY><<<grid, 128, (size_t)p.smem_bytes, st>>>(tm, a, e);                                                \
         return cudaGetLastError();                                                                                                          \
@@ -397,6 +325,167 @@ cudaError_t launch_conv_window(const WindowPlan& p, const void* w, void* out, co
     TB200_WIN_LAYOUTS(0, false) TB200_WIN_LAYOUTS(1, false) TB200_WIN_LAYOUTS(2, false) TB200_WIN_LAYOUTS(0, true) TB200_WIN_LAYOUTS(2, true)
 #undef TB200_WIN_LAYOUTS
 #undef TB200_WIN_CASE
+    return cudaErrorInvalidValue;
+}
+
+// ---- gather convolution on the tensor cores (NCHW stems, 3x3 convolutions over 16-channel NHWC tensors) ----------------
+// The window kernel's layers when it has no plan: NCHW inputs whose width is not a multiple of 16 (a tensor map's global
+// strides must be), windows too large for shared memory, TB200_NO_WINDOW_CONV.  Same skeleton, without the staged window:
+// every thread gathers the K bytes of its output pixel itself -- NCHW: 27 / 147 byte loads; NHWC16: nine 16-byte loads, one
+// per tap -- and writes them as one row of `ks` SW32 K-major k-block tiles; `ks`
+// k-steps (K = 32 each) accumulate.  uint8: taps outside the image are filled with the input zero point (they then contribute
+// (zx-zx)(w-zw) = 0, exactly like the reference, which skips them), padding K positions hold 0 in A and B, and the thread
+// sums its own row (dp4a) so that  sum (x-zx)(w-zw) = acc - zw*sum(x) + corr[oc]  needs no ones-row and no border table.
+// Takes the role of im2col + sgemm of conv_hcl_run for these shapes (conv_kernel_x86.c:187-242, 1008-1631).
+struct GatherArgs
+{
+    const uint8_t* in;
+    const uint8_t* w; // [OCp][ks*32]; NCHW: k = (c*3 + kh)*3 + kw ; NHWC16: k = (kh*3 + kw)*16 + c ; zero padded
+    uint8_t* out;
+    int n, c, h, w_in, oh, ow, ocp, oc, stride, ph, pw;
+    unsigned npix, ntiles;
+    int ks, nhwc16;
+    uint32_t fill; // byte for taps outside the image, replicated x4 (uint8: the input zero point; int8: 0)
+    uint32_t fill16[4]; // NHWC16: the same for a whole 16-channel tap; pad channels (c >= C) stay 0 like in the tensor itself
+};
+
+template <int MODE, bool U8, int KHW> // MODE: 0 fast, 1 fast + fused bias (int8), 2 exact; KHW: 3 or 7 (NCHW stems; NHWC16 is 3x3)
+__global__ void __launch_bounds__(128) conv_gather_tc_kernel(const GatherArgs a, const __grid_constant__ EpiParams e)
+{
+    extern __shared__ __align__(1024) uint8_t gat_smem[];
+    uint8_t* sm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(gat_smem) + 1023) & ~(uintptr_t)1023);
+    const uint32_t sA = smem_u32(sm), sB = sA + (uint32_t)a.ks * 4096u, b_tile = (uint32_t)a.ocp * 32u, sPar = sB + (uint32_t)a.ks * b_tile;
+    const uint32_t pitch = acc_pitch(a.ocp), sImg = (sPar + (uint32_t)a.ocp * 8u + 15u) & ~15u; // accumulator image [128][pitch]
+    const int tid = threadIdx.x;
+    stage_b_and_constants<MODE, U8>(a.w, a.ks, a.ocp, sB, sPar, e);
+
+    for (unsigned tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x)
+    {
+        const unsigned pix = tile * 128u + (unsigned)tid;
+        const bool valid = pix < a.npix;
+        int32_t sx = 0;
+        int n = 0, oh = 0, ow = 0;
+        if (valid)
+        {
+            const unsigned prow = pix / (unsigned)a.ow;
+            ow = (int)(pix - prow * a.ow);
+            n = (int)(prow / (unsigned)a.oh);
+            oh = (int)(prow - (unsigned)n * a.oh);
+        }
+        const int iy0 = oh * a.stride - a.ph, ix0 = ow * a.stride - a.pw;
+        if (a.nhwc16)
+        {
+            // nine 16-byte taps + one half-row of padding = 160 bytes = five k-steps
+            const uint8_t* img = a.in + (size_t)n * a.h * a.w_in * 16;
+#pragma unroll
+            for (int t = 0; t < 10; t++)
+            {
+                uint4 v = make_uint4(0, 0, 0, 0);
+                if (t < 9)
+                {
+                    const int iy = iy0 + t / 3, ix = ix0 + t % 3;
+                    v = make_uint4(a.fill16[0], a.fill16[1], a.fill16[2], a.fill16[3]);
+                    if (valid && iy >= 0 && iy < a.h && ix >= 0 && ix < a.w_in) v = __ldg(reinterpret_cast<const uint4*>(img + ((size_t)iy * a.w_in + ix) * 16));
+                    if (U8) sx = (int32_t)__dp4a(v.w, 0x01010101u, __dp4a(v.z, 0x01010101u, __dp4a(v.y, 0x01010101u, __dp4a(v.x, 0x01010101u, (unsigned)sx))));
+                }
+                sts_u4(sA + (uint32_t)(t >> 1) * 4096u + sw32_offset(tid, t & 1), v.x, v.y, v.z, v.w);
+            }
+        }
+        else
+        {
+            // NCHW stem: C*KHW*KHW bytes (27 for 3x3, 147 for ResNet's 7x7), k = (c*KHW + kh)*KHW + kw, in NW words = NW/8 k-steps
+            constexpr int NW = KHW == 3 ? 8 : 40;
+            uint32_t row[NW];
+#pragma unroll
+            for (int j = 0; j < NW; j++) row[j] = 0;
+            const size_t plane = (size_t)a.h * a.w_in;
+            const uint8_t* img = a.in + (size_t)n * a.c * plane;
+            const uint32_t fb = a.fill & 0xffu;
+#pragma unroll
+            for (int c = 0; c < 3; c++)
+            {
+                if (c < a.c)
+                {
+#pragma unroll
+                    for (int kh = 0; kh < KHW; kh++)
+                    {
+                        const int iy = iy0 + kh;
+                        const bool rok = valid && iy >= 0 && iy < a.h;
+                        const uint8_t* rp = img + (size_t)c * plane + (size_t)(rok ? iy : 0) * a.w_in;
+#pragma unroll
+                        for (int kw = 0; kw < KHW; kw++)
+                        {
+                            const int ix = ix0 + kw;
+                            const uint32_t b = (rok && ix >= 0 && ix < a.w_in) ? (uint32_t)__ldg(rp + ix) : fb;
+                            const int k = (c * KHW + kh) * KHW + kw; // compile-time after unrolling
+                            row[k >> 2] |= b << (8 * (k & 3));
+                        }
+                    }
+                }
+            }
+            if (U8)
+            {
+#pragma unroll
+                for (int j = 0; j < NW; j++) sx = (int32_t)__dp4a(row[j], 0x01010101u, (unsigned)sx);
+            }
+#pragma unroll
+            for (int j = 0; j < NW / 4; j++)
+                sts_u4(sA + (uint32_t)(j >> 1) * 4096u + sw32_offset(tid, j & 1), row[4 * j], row[4 * j + 1], row[4 * j + 2], row[4 * j + 3]);
+        }
+        fence_proxy_async_smem(); // the MMAs read these generic-proxy writes through the async proxy
+        __syncthreads();          // (first iteration: also publishes the B tiles and the constants)
+        wg_mma_to_image<U8, U8>(sA, 4096u, sB, b_tile, a.ks, 32, a.ocp, sImg, pitch);
+        __syncthreads();
+
+        uint8_t* op = a.out + (size_t)pix * a.ocp;
+        const uint32_t tb = sImg + (uint32_t)tid * pitch;
+        const int32_t rowc = U8 ? -e.w_zero * sx : 0;
+        for (int c = 0; c < a.ocp; c += 16)
+        {
+            uint32_t v[16], w[4];
+            acc_ld16(tb + 4u * c, v);
+            tc_unit16<MODE, U8>(v, rowc, sPar + c * 8, c, a.oc, e, w);
+            if (valid) *reinterpret_cast<uint4*>(op + c) = make_uint4(w[0], w[1], w[2], w[3]);
+        }
+        __syncthreads(); // the next tile's gather overwrites the A tiles, its MMAs the accumulator image
+    }
+}
+
+cudaError_t launch_conv_gather_tc(const void* in, const void* w, void* out, const ConvShape& s, const EpiParams& e, int nhwc16, int num_sms, cudaStream_t st)
+{
+    const int khw = nhwc16 ? 3 : s.kh;
+    GatherArgs a;
+    a.in = (const uint8_t*)in, a.w = (const uint8_t*)w, a.out = (uint8_t*)out;
+    a.n = s.n, a.c = s.c, a.h = s.h, a.w_in = s.w, a.oh = s.oh, a.ow = s.ow, a.ocp = s.ocp, a.oc = s.oc, a.stride = s.sh, a.ph = s.ph0, a.pw = s.pw0;
+    a.npix = (unsigned)((long long)s.n * s.oh * s.ow);
+    a.ntiles = (a.npix + 127u) / 128u;
+    a.ks = nhwc16 ? 5 : (s.c * s.kh * s.kw + 31) / 32, a.nhwc16 = nhwc16;
+    a.fill = e.is_uint8 ? ((uint32_t)(e.in_zero & 0xff) * 0x01010101u) : 0u;
+    for (int j = 0; j < 4; j++)
+    {
+        a.fill16[j] = 0;
+        for (int t = 0; t < 4; t++)
+            if (j * 4 + t < s.c) a.fill16[j] |= (a.fill & 0xffu) << (8 * t);
+    }
+    const size_t smem = (size_t)a.ks * 4096 + (size_t)a.ks * s.ocp * 32 + (size_t)s.ocp * 8 + 16 + 128 * (size_t)acc_pitch(s.ocp) + 1024;
+    const unsigned cap = (unsigned)num_sms * 6u;
+    const unsigned grid = a.ntiles < cap ? a.ntiles : cap;
+    const int mode = !e.fast_ok ? 2 : ((!e.is_uint8 && e.fuse_bias) ? 1 : 0);
+#define TB200_GAT_CASE(MD, U, K)                                                                                                   \
+    if (mode == MD && (e.is_uint8 != 0) == U && khw == K)                                                                          \
+    {                                                                                                                              \
+        /* the opt-in is per device AND per context: set it before every launch (launches happen at graph capture only) */ \
+        {                                                                                                                          \
+            cudaError_t err = cudaFuncSetAttribute(conv_gather_tc_kernel<MD, U, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
+            if (err != cudaSuccess) return err;                                                                                    \
+        }                                                                                                                          \
+        if (debug_launch()) fprintf(stderr, "tengine_b200: launch conv_gather_tc_kernel<MODE=%d,U8=%d,KHW=%d>\n", MD, (int)U, K);  \
+        conv_gather_tc_kernel<MD, U, K><<<grid, 128, smem, st>>>(a, e);                                                            \
+        return cudaGetLastError();                                                                                                 \
+    }
+    TB200_GAT_CASE(0, false, 3) TB200_GAT_CASE(1, false, 3) TB200_GAT_CASE(2, false, 3) TB200_GAT_CASE(0, true, 3) TB200_GAT_CASE(2, true, 3)
+    TB200_GAT_CASE(0, false, 7) TB200_GAT_CASE(1, false, 7) TB200_GAT_CASE(2, false, 7) TB200_GAT_CASE(0, true, 7) TB200_GAT_CASE(2, true, 7)
+#undef TB200_GAT_CASE
     return cudaErrorInvalidValue;
 }
 

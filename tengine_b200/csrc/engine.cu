@@ -130,7 +130,6 @@ enum StepKind
     K_NCHW2NHWC,
     K_NHWC2NCHW,
     K_CONV_STEM,
-    K_STEM_TC,
     K_GATHER_TC,
     K_CONV_DW,
     K_CONV_DIRECT,
@@ -146,7 +145,7 @@ enum StepKind
     K_RESHAPE,
     K_NONE // a node folded into its producer
 };
-static const char* kStepName[] = {"nchw_to_nhwc", "nhwc_to_nchw", "conv_stem_nchw_dp4a", "conv_stem_nchw_tcgen05", "conv_gather_tcgen05", "conv_dw_direct", "conv_direct_dp4a",
+static const char* kStepName[] = {"nchw_to_nhwc", "nhwc_to_nchw", "conv_stem_nchw_dp4a", "conv_gather_tcgen05", "conv_dw_direct", "conv_direct_dp4a",
                                   "gemm_i8_tcgen05", "conv_igemm_i8_tcgen05", "pool", "pointwise", "concat_requant", "upsample_nearest", "copy",
                                   "byte_lut", "softmax", "reshape_nchw_order", "fused_into_producer"};
 
@@ -432,8 +431,9 @@ static EpiParams make_epi(const tb200_layer_desc& L, const tb200_tensor_desc& ti
     {
         e.fast_lo = (float)(0 - tout.zero_point), e.fast_hi = (float)(255 - tout.zero_point);
         e.fast_r = 1.0f / so;
-        // integer-domain clip + zero point + saturation (common.cuh requant_fast8_u8): the activation bounds become the integers
-        // the reference's own division and round() give for them; q' = max(min(q + zp - L, H - L), 0), byte = q' + L
+        // integer-domain clip + zero point + saturation (common.cuh requant_fast8_i8, the int8 form the uint8 tensor-core epilogues
+        // use): the activation bounds become the integers the reference's own division and round() give for them;
+        // q' = max(min(q + zp - L, H - L), 0), byte = q' + L
         int q_lo = -30000, q_hi = 30000;
         if (flo > -inf) q_lo = (int)roundf(flo / so);
         if (fhi < inf) q_hi = (int)roundf(fhi / so);
@@ -480,9 +480,9 @@ static int run_step(tb200_graph* g, const Step& s, cudaStream_t st)
     case K_NCHW2NHWC: err = launch_nchw_to_nhwc(s.in, s.out, s.n, s.c, s.h, s.w_, st); break;
     case K_NHWC2NCHW: err = launch_nhwc_to_nchw(s.in, s.out, s.n, s.c, s.h, s.w_, st); break;
     case K_CONV_STEM: err = launch_conv_stem(s.in, s.w, s.out, s.cs, s.epi, st); break;
-    case K_STEM_TC: err = launch_stem_tc(s.dwp, s.in, s.w, s.out, s.cs, s.epi, st); break;
     case K_GATHER_TC:
-        err = s.wp.valid ? launch_conv_window(s.wp, s.w, s.out, s.cs, s.epi, st) : launch_conv_gather_tc(s.in, s.w, s.out, s.cs, s.epi, s.nhwc16, st);
+        err = s.wp.valid ? launch_conv_window(s.wp, s.w, s.out, s.cs, s.epi, g->ctx->num_sms, st)
+                         : launch_conv_gather_tc(s.in, s.w, s.out, s.cs, s.epi, s.nhwc16, g->ctx->num_sms, st);
         break;
     case K_CONV_DW:
         err = s.dwp.valid ? launch_conv_dw_tma(s.dwp, s.w, s.out, s.cs, s.epi, st) : launch_conv_dw(s.in, s.w, s.out, s.cs, s.epi, st);
@@ -771,10 +771,8 @@ static int plan_conv(int li, const tb200_layer_desc& L, const TensorInfo& tin, c
     const bool k3 = L.kernel_h == 3 && L.kernel_w == 3, u8_tc_on = !(u8 && getenv("TB200_NO_U8_TC"));
     const bool gather = tc && plain && tout.cp <= 256 && !getenv("TB200_NO_GATHER_TC");
     size_t& wsize = P.blob.w_size;
-    if (nchw_input && tc && plain && k3 && !u8 && tout.cp <= 256 && !getenv("TB200_NO_STEM_TC"))
-        P.kind = K_STEM_TC, P.reads_nchw = true, wsize = (size_t)tout.cp * 32; // one 32-byte wgmma k-step per output channel
-    else if (nchw_input && gather && L.kernel_h == L.kernel_w && (L.kernel_h == 7 || (u8 && L.kernel_h == 3)))
-        // uint8 3x3 stems and 7x7 stems (ResNet): threads gather, taps outside the image = zero point; K padded to 32*ks
+    if (nchw_input && gather && L.kernel_h == L.kernel_w && (L.kernel_h == 3 || L.kernel_h == 7))
+        // 3x3 and 7x7 (ResNet) stems: K = C*KH*KW padded to 32*ks (one k-step for a 3x3 stem); uint8 taps outside the image = zero point
         P.kind = K_GATHER_TC, P.reads_nchw = true, wsize = (size_t)tout.cp * 32 * ((C * L.kernel_h * L.kernel_w + 31) / 32);
     else if (tin.input_index >= 0 && C <= 4 && L.group == 1)
         P.kind = K_CONV_STEM, P.reads_nchw = true, wsize = (size_t)tout.cp * L.kernel_h * L.kernel_w * 4;
@@ -1129,7 +1127,7 @@ static void pack_conv_weights(const tb200_layer_desc& L, const LayerPlan& P, con
                 for (int t = 0; t < 9; t++) dst[(size_t)o * rowb + t * tin.cp + c] = src[((size_t)o * C + c) * 9 + t];
         return;
     }
-    if (P.kind == K_STEM_TC || P.kind == K_GATHER_TC)
+    if (P.kind == K_GATHER_TC)
     {
         // [OC][C][KH][KW] is already k = (c*KH + kh)*KW + kw order: one zero-padded row of 32*ks bytes per channel
         const size_t kp = ((P.k + 31) / 32) * 32;
@@ -1480,7 +1478,6 @@ static int fill_conv_step(tb200_graph* g, int li, const LayerPlan& P, const Slic
     }
     if (P.reads_nchw) s.in = g->in_nchw_dev[tin.input_index] + sl.off(tin.nchw_bytes);
     s.nhwc16 = P.nhwc16;
-    if (s.kind == K_STEM_TC) stem_plan_create(&s.dwp, s.in, s.cs); // falls back to the global-memory gather
     if (s.kind == K_GATHER_TC)
     {
         window_plan_create(&s.wp, s.in, s.cs, s.nhwc16); // falls back to the global-memory gather (16 channels / NCHW only)

@@ -725,502 +725,13 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
     }
 }
 
-// ---- stem on the tensor cores ------------------------------------------------------------------------------
-// First convolution of a network: NCHW int8 input with C <= 3 channels (as the application hands it over), 3x3 filter,
-// any stride / padding -> NHWC output.  K = C*9 <= 27 is padded to ONE 32-byte wgmma k-step: the 128 threads of a CTA
-// each gather the 27 input bytes of one output pixel, write them as one row of a SW32 K-major A tile, the warpgroup
-// multiplies it (128 x OCp x 32) into the shared-memory accumulator image, and every thread requantises its own row and
-// writes OCp contiguous bytes.
-// Replaces ~290 dp4a per pixel of the CUDA-core stem kernel (kernels_direct.cu) by one MMA; the work left is the gather
-// (~80 instructions) and the epilogue.  Several CTAs per SM overlap each other.
-// Takes the role of the first im2col + sgemm of conv_hcl_run (conv_kernel_x86.c:187-242).
-struct StemArgs
-{
-    const uint8_t* in;  // NCHW
-    const uint8_t* w;   // [OCp][32]: k = (c*3 + kh)*3 + kw, zero padded
-    uint8_t* out;       // NHWC, OCp bytes per pixel
-    int n, c, h, w_in, oh, ow, ocp, oc, stride, ph, pw;
-    unsigned npix, ntiles;
-    int tiles_w, tiles_h, box_w, box_h, in_bytes; // TMA-staged input window (16 x 8 output pixels per tile)
-    int xoff; // the window starts xoff bytes left of the first tap: the innermost TMA coordinate must be 16-byte aligned
-};
-
-// TMA_IN: the input window of the tile (3 channel planes x box_h rows x box_w bytes, zero-filled outside the image) is
-// staged in shared memory by one 4-D TMA load, double-buffered; the gather is then 27 unpredicated LDS.U8 + IMAD per
-// pixel.  Without it (image width not a multiple of 16) every thread gathers from global memory with bounds predicates,
-// which costs more instructions than the whole epilogue.
-template <int MODE, bool TMA_IN> // MODE: 0 fast, 1 fast + fused bias, 2 exact
-__global__ void __launch_bounds__(128) stem_tc_kernel(const __grid_constant__ CUtensorMap tmap_in, const StemArgs a, const __grid_constant__ EpiParams e)
-{
-    extern __shared__ __align__(1024) uint8_t stem_smem[];
-    uint8_t* sm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(stem_smem) + 1023) & ~(uintptr_t)1023);
-    const uint32_t sA = smem_u32(sm), sB = sA + 4096, sPar = sB + (uint32_t)a.ocp * 32u;
-    const uint32_t in_stride = ((uint32_t)a.in_bytes + 127u) & ~127u;
-    const uint32_t sIn = (sPar + (uint32_t)a.ocp * 8u + 127u) & ~127u;
-    const uint32_t pitch = acc_pitch(a.ocp), sImg = sIn + 2u * in_stride; // accumulator image [128][pitch]
-    __shared__ __align__(8) uint64_t in_full[2];
-    const int tid = threadIdx.x;
-    const int tw = tid & 15, th = tid >> 4; // TMA_IN: the tile is 16 x 8 output pixels
-
-    if (tid == 0)
-    {
-        mbar_init(&in_full[0], 1), mbar_init(&in_full[1], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    auto tile_coords = [&](unsigned tile, int& n, int& oh0, int& ow0)
-    {
-        const unsigned r = tile / (unsigned)a.tiles_w;
-        ow0 = (int)(tile - r * a.tiles_w) * 16;
-        n = (int)(r / (unsigned)a.tiles_h);
-        oh0 = (int)(r - (unsigned)n * a.tiles_h) * 8;
-    };
-    // (kept in the kernel body: the tensor map must be addressed as the kernel parameter itself, which a lambda that is
-    //  not inlined does not guarantee -- compute-sanitizer: illegal instruction at the cp.async.bulk.tensor)
-#define TB200_STEM_LOAD_TILE(TILE, BUF)                                                                                               \
-    do                                                                                                                                \
-    {                                                                                                                                 \
-        int n_, oh0_, ow0_;                                                                                                           \
-        tile_coords((TILE), n_, oh0_, ow0_);                                                                                          \
-        mbar_expect_tx(&in_full[(BUF)], (uint32_t)a.in_bytes);                                                                        \
-        tma_load_4d(&tmap_in, &in_full[(BUF)], sm + (sIn - sA) + (size_t)(BUF) * in_stride, ow0_ * a.stride - a.pw - a.xoff, oh0_ * a.stride - a.ph, \
-                    0, n_);                                                                                                           \
-    } while (0)
-    if (TMA_IN && tid == 0 && blockIdx.x < a.ntiles) TB200_STEM_LOAD_TILE(blockIdx.x, 0);
-    // ---- B tile and the epilogue constants (identical for every CTA; L2 / L1 resident) ----
-    for (int i = tid; i < a.ocp * 2; i += 128)
-    {
-        const uint4 v = __ldg(reinterpret_cast<const uint4*>(a.w) + i);
-        sts_u4(sB + sw32_offset(i >> 1, i & 1), v.x, v.y, v.z, v.w);
-    }
-    for (int c = tid; c < a.ocp; c += 128) sts_f2(sPar + c * 8, (MODE != 2) ? __ldg(e.fast_par + c) : make_float2(0.f, 0.f));
-
-    uint32_t it = 0;
-    for (unsigned tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x, it++)
-    {
-        uint32_t row[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-        unsigned pix;
-        bool valid;
-        if (TMA_IN)
-        {
-            int n, oh0, ow0;
-            tile_coords(tile, n, oh0, ow0);
-            const int oh = oh0 + th, ow = ow0 + tw;
-            valid = oh < a.oh && ow < a.ow;
-            pix = ((unsigned)n * a.oh + oh) * a.ow + ow;
-            const int buf = it & 1;
-            mbar_wait(&in_full[buf], (it >> 1) & 1);
-            const uint32_t base = sIn + (uint32_t)buf * in_stride + (uint32_t)((th * a.stride) * a.box_w + tw * a.stride + a.xoff);
-#pragma unroll
-            for (int c = 0; c < 3; c++)
-            {
-                if (c < a.c)
-                {
-#pragma unroll
-                    for (int kh = 0; kh < 3; kh++)
-#pragma unroll
-                        for (int kw = 0; kw < 3; kw++)
-                        {
-                            uint32_t b;
-                            asm volatile("ld.shared.u8 %0, [%1];" : "=r"(b) : "r"(base + (uint32_t)((c * a.box_h + kh) * a.box_w + kw)));
-                            const int k = (c * 3 + kh) * 3 + kw; // compile-time after unrolling
-                            row[k >> 2] += b << (8 * (k & 3)); // disjoint bytes: add == or (IMAD, off the ALU pipe)
-                        }
-                }
-            }
-        }
-        else
-        {
-            // ---- gather the 3x3 x C window from the NCHW planes in global memory ----
-            pix = tile * 128u + (unsigned)tid;
-            valid = pix < a.npix;
-            if (valid)
-            {
-                const unsigned prow = pix / (unsigned)a.ow;
-                const int ow = (int)(pix - prow * a.ow);
-                const int n = (int)(prow / (unsigned)a.oh);
-                const int oh = (int)(prow - (unsigned)n * a.oh);
-                const int iy0 = oh * a.stride - a.ph, ix0 = ow * a.stride - a.pw;
-                const size_t plane = (size_t)a.h * a.w_in;
-                const uint8_t* img = a.in + (size_t)n * a.c * plane;
-#pragma unroll
-                for (int c = 0; c < 3; c++)
-                {
-                    if (c < a.c)
-                    {
-#pragma unroll
-                        for (int kh = 0; kh < 3; kh++)
-                        {
-                            const int iy = iy0 + kh;
-                            const bool rok = iy >= 0 && iy < a.h;
-                            const uint8_t* rp = img + (size_t)c * plane + (size_t)(rok ? iy : 0) * a.w_in;
-#pragma unroll
-                            for (int kw = 0; kw < 3; kw++)
-                            {
-                                const int ix = ix0 + kw;
-                                const uint32_t b = (rok && ix >= 0 && ix < a.w_in) ? (uint32_t)__ldg(rp + ix) : 0u;
-                                const int k = (c * 3 + kh) * 3 + kw;
-                                row[k >> 2] |= b << (8 * (k & 3));
-                            }
-                        }
-                    }
-                }
-            }
-        }
-        sts_u4(sA + sw32_offset(tid, 0), row[0], row[1], row[2], row[3]);
-        sts_u4(sA + sw32_offset(tid, 1), row[4], row[5], row[6], row[7]);
-        fence_proxy_async_smem(); // the MMA reads these generic-proxy writes through the async proxy
-        __syncthreads();          // (first iteration: also publishes the B tile and the constants)
-        // everybody has read this tile's window: prefetch the next one into the other buffer
-        if (TMA_IN && tid == 0 && tile + gridDim.x < a.ntiles) TB200_STEM_LOAD_TILE(tile + gridDim.x, (it + 1) & 1);
-        wg_mma_to_image<false, false>(sA, 0u, sB, 0u, 1, 32, a.ocp, sImg, pitch);
-        __syncthreads();
-
-        // ---- epilogue: thread = pixel = accumulator row, 16 channels per load, OCp contiguous output bytes per pixel ----
-        uint8_t* op = a.out + (size_t)pix * a.ocp;
-        const uint32_t tb = sImg + (uint32_t)tid * pitch;
-        for (int c = 0; c < a.ocp; c += 16)
-        {
-            uint32_t v[16];
-            acc_ld16(tb + 4u * c, v);
-            uint32_t w[4];
-            if (MODE == 2)
-            {
-#pragma unroll
-                for (int k = 0; k < 16; k++)
-                {
-                    if ((k & 3) == 0) w[k >> 2] = 0;
-                    if (c + k < a.oc) w[k >> 2] |= ((uint32_t)requant((int32_t)v[k], c + k, e) & 0xffu) << (8 * (k & 3));
-                }
-            }
-            else
-                stem_unit_fast<MODE == 1>(v, sPar + c * 8, c, e, w);
-            if (valid) *reinterpret_cast<uint4*>(op + c) = make_uint4(w[0], w[1], w[2], w[3]);
-        }
-        // the next tile's MMA overwrites the accumulator image and its gather overwrites the A tile
-        __syncthreads();
-    }
-}
-
-#undef TB200_STEM_LOAD_TILE
-
-bool stem_tc_supported(const ConvShape& s, const EpiParams& e)
-{
-    return !e.is_uint8 && s.kh == 3 && s.kw == 3 && s.c <= 3 && s.group == 1 && s.dh == 1 && s.dw == 1 && s.sh == s.sw && s.ocp <= 256 &&
-           (long long)s.n * s.oh * s.ow < (1ll << 31);
-}
-
-// Tensor map over the NCHW network input for the TMA-staged variant: dims (W, H, C, N), box (box_w, box_h, C, 1).
-int stem_plan_create(DwPlan* p, const void* in, const ConvShape& s)
-{
-    p->valid = 0;
-    if (s.w % 16 || getenv("TB200_STEM_NO_TMA")) return -1; // global strides of a tensor map are multiples of 16 bytes
-    // innermost coordinate = ow0*S - pw - xoff must be a multiple of 16 (ow0*S is a multiple of 16*S)
-    const int xoff = (16 - (((-s.pw0) % 16) + 16) % 16) % 16 == 0 ? 0 : ((((-s.pw0) % 16) + 16) % 16);
-    const int box_w = (xoff + (16 - 1) * s.sw + 3 + 15) & ~15, box_h = (8 - 1) * s.sh + 3;
-    if (box_w > 256 || box_h > 256) return -1;
-    const uint64_t dims[4] = {(uint64_t)s.w, (uint64_t)s.h, (uint64_t)s.c, (uint64_t)s.n};
-    const uint64_t strides[3] = {(uint64_t)s.w, (uint64_t)s.w * s.h, (uint64_t)s.w * s.h * s.c};
-    const uint32_t box[4] = {(uint32_t)box_w, (uint32_t)box_h, (uint32_t)s.c, 1u};
-    if (tmap_encode(p->tmap_in, in, 4, dims, strides, box, nullptr, 0)) return -1;
-    p->tile_cols = box_w, p->tile_rows = box_h, p->gpr = xoff;
-    p->valid = 1;
-    return 0;
-}
-
-cudaError_t launch_stem_tc(const DwPlan& plan, const void* in, const void* w, void* out, const ConvShape& s, const EpiParams& e, cudaStream_t st)
-{
-    StemArgs a;
-    a.in = (const uint8_t*)in, a.w = (const uint8_t*)w, a.out = (uint8_t*)out;
-    a.n = s.n, a.c = s.c, a.h = s.h, a.w_in = s.w, a.oh = s.oh, a.ow = s.ow, a.ocp = s.ocp, a.oc = s.oc, a.stride = s.sh, a.ph = s.ph0, a.pw = s.pw0;
-    a.npix = (unsigned)((long long)s.n * s.oh * s.ow);
-    const bool tma = plan.valid != 0;
-    a.tiles_w = (s.ow + 15) / 16, a.tiles_h = (s.oh + 7) / 8;
-    a.box_w = plan.tile_cols, a.box_h = plan.tile_rows, a.in_bytes = tma ? plan.tile_cols * plan.tile_rows * s.c : 0, a.xoff = plan.gpr;
-    a.ntiles = tma ? (unsigned)a.tiles_w * a.tiles_h * s.n : (a.npix + 127u) / 128u;
-    const size_t smem = 4096 + (size_t)s.ocp * 32 + (size_t)s.ocp * 8 + 128 + 2 * (size_t)((a.in_bytes + 127) & ~127) + 128 * (size_t)acc_pitch(s.ocp) + 1024;
-    static int sms = 0;
-    if (!sms)
-    {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    }
-    // several resident CTAs per SM overlap gather / MMA / epilogue of different tiles; each loops over its share
-    const unsigned cap = (unsigned)sms * 8u;
-    const unsigned grid = a.ntiles < cap ? a.ntiles : cap;
-    const int mode = !e.fast_ok ? 2 : (e.fuse_bias ? 1 : 0);
-    CUtensorMap tm;
-    memcpy(&tm, plan.tmap_in, sizeof tm);
-#define TB200_STEM_CASE(MD, T)                                                                                                 \
-    if (mode == MD && tma == T)                                                                                                \
-    {                                                                                                                          \
-        cudaError_t err = cudaFuncSetAttribute(stem_tc_kernel<MD, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-        if (err != cudaSuccess) return err;                                                                                    \
-        if (debug_launch()) fprintf(stderr, "tengine_b200: launch stem_tc_kernel<MODE=%d,TMA_IN=%d>\n", MD, (int)T);         \
-        stem_tc_kernel<MD, T><<<grid, 128, smem, st>>>(tm, a, e);                                                              \
-        return cudaGetLastError();                                                                                             \
-    }
-    TB200_STEM_CASE(0, true) TB200_STEM_CASE(1, true) TB200_STEM_CASE(2, true)
-    TB200_STEM_CASE(0, false) TB200_STEM_CASE(1, false) TB200_STEM_CASE(2, false)
-#undef TB200_STEM_CASE
-    return cudaErrorInvalidValue;
-}
-
-// ---- gather convolution on the tensor cores (uint8 stems, 3x3 convolutions over 16-channel NHWC tensors) ---------------
-// Same skeleton as the stem above, for the two YOLOv3-tiny layers the implicit GEMM cannot take: the uint8 NCHW stem
-// (3 -> 16 channels at 416x416) and the 3x3 convolution whose input has only 16 channels (a 32-byte wgmma k-step would
-// straddle two filter taps of a 4-D TMA box).  Every thread gathers the K bytes of its output pixel itself -- NCHW: 27 byte
-// loads; NHWC16: nine 16-byte loads, one per tap -- and writes them as one row of `ks` SW32 K-major k-block tiles; `ks`
-// k-steps (K = 32 each) accumulate.  uint8: taps outside the image are filled with the input zero point (they then contribute
-// (zx-zx)(w-zw) = 0, exactly like the reference, which skips them), padding K positions hold 0 in A and B, and the thread
-// sums its own row (dp4a) so that  sum (x-zx)(w-zw) = acc - zw*sum(x) + corr[oc]  needs no ones-row and no border table.
-// Takes the role of im2col + sgemm of conv_hcl_run for these shapes (conv_kernel_x86.c:187-242, 1008-1631).
-struct GatherArgs
-{
-    const uint8_t* in;
-    const uint8_t* w; // [OCp][ks*32]; NCHW: k = (c*3 + kh)*3 + kw ; NHWC16: k = (kh*3 + kw)*16 + c ; zero padded
-    uint8_t* out;
-    int n, c, h, w_in, oh, ow, ocp, oc, stride, ph, pw;
-    unsigned npix, ntiles;
-    int ks, nhwc16;
-    uint32_t fill; // byte for taps outside the image, replicated x4 (uint8: the input zero point; int8: 0)
-    uint32_t fill16[4]; // NHWC16: the same for a whole 16-channel tap; pad channels (c >= C) stay 0 like in the tensor itself
-};
-
-template <int MODE, bool U8, int KHW> // MODE: 0 fast, 1 fast + fused bias (int8), 2 exact; KHW: 3 or 7 (NCHW stems; NHWC16 is 3x3)
-__global__ void __launch_bounds__(128) conv_gather_tc_kernel(const GatherArgs a, const __grid_constant__ EpiParams e)
-{
-    extern __shared__ __align__(1024) uint8_t gat_smem[];
-    uint8_t* sm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(gat_smem) + 1023) & ~(uintptr_t)1023);
-    const uint32_t sA = smem_u32(sm), sB = sA + (uint32_t)a.ks * 4096u, b_tile = (uint32_t)a.ocp * 32u, sPar = sB + (uint32_t)a.ks * b_tile;
-    const uint32_t pitch = acc_pitch(a.ocp), sImg = (sPar + (uint32_t)a.ocp * 8u + 15u) & ~15u; // accumulator image [128][pitch]
-    const int tid = threadIdx.x;
-    // B tiles (one per k-step) and the epilogue constants: identical for every CTA, L2 resident
-    for (int i = tid; i < a.ks * a.ocp * 2; i += 128)
-    {
-        const int kb = i / (a.ocp * 2), j = i - kb * (a.ocp * 2), r = j >> 1, c16 = j & 1;
-        const uint4 v = __ldg(reinterpret_cast<const uint4*>(a.w + ((size_t)r * a.ks + kb) * 32) + c16);
-        sts_u4(sB + (uint32_t)kb * b_tile + sw32_offset(r, c16), v.x, v.y, v.z, v.w);
-    }
-    for (int c = tid; c < a.ocp; c += 128) sts_f2(sPar + c * 8, (MODE != 2 || U8) ? __ldg(e.fast_par + c) : make_float2(0.f, 0.f));
-
-    for (unsigned tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x)
-    {
-        const unsigned pix = tile * 128u + (unsigned)tid;
-        const bool valid = pix < a.npix;
-        int32_t sx = 0;
-        int n = 0, oh = 0, ow = 0;
-        if (valid)
-        {
-            const unsigned prow = pix / (unsigned)a.ow;
-            ow = (int)(pix - prow * a.ow);
-            n = (int)(prow / (unsigned)a.oh);
-            oh = (int)(prow - (unsigned)n * a.oh);
-        }
-        const int iy0 = oh * a.stride - a.ph, ix0 = ow * a.stride - a.pw;
-        if (a.nhwc16)
-        {
-            // nine 16-byte taps + one half-row of padding = 160 bytes = five k-steps
-            const uint8_t* img = a.in + (size_t)n * a.h * a.w_in * 16;
-#pragma unroll
-            for (int t = 0; t < 10; t++)
-            {
-                uint4 v = make_uint4(0, 0, 0, 0);
-                if (t < 9)
-                {
-                    const int iy = iy0 + t / 3, ix = ix0 + t % 3;
-                    v = make_uint4(a.fill16[0], a.fill16[1], a.fill16[2], a.fill16[3]);
-                    if (valid && iy >= 0 && iy < a.h && ix >= 0 && ix < a.w_in) v = __ldg(reinterpret_cast<const uint4*>(img + ((size_t)iy * a.w_in + ix) * 16));
-                    if (U8) sx = (int32_t)__dp4a(v.w, 0x01010101u, __dp4a(v.z, 0x01010101u, __dp4a(v.y, 0x01010101u, __dp4a(v.x, 0x01010101u, (unsigned)sx))));
-                }
-                sts_u4(sA + (uint32_t)(t >> 1) * 4096u + sw32_offset(tid, t & 1), v.x, v.y, v.z, v.w);
-            }
-        }
-        else
-        {
-            // NCHW stem: C*KHW*KHW bytes (27 for 3x3, 147 for ResNet's 7x7), k = (c*KHW + kh)*KHW + kw, in NW words = NW/8 k-steps
-            constexpr int NW = KHW == 3 ? 8 : 40;
-            uint32_t row[NW];
-#pragma unroll
-            for (int j = 0; j < NW; j++) row[j] = 0;
-            const size_t plane = (size_t)a.h * a.w_in;
-            const uint8_t* img = a.in + (size_t)n * a.c * plane;
-            const uint32_t fb = a.fill & 0xffu;
-#pragma unroll
-            for (int c = 0; c < 3; c++)
-            {
-                if (c < a.c)
-                {
-#pragma unroll
-                    for (int kh = 0; kh < KHW; kh++)
-                    {
-                        const int iy = iy0 + kh;
-                        const bool rok = valid && iy >= 0 && iy < a.h;
-                        const uint8_t* rp = img + (size_t)c * plane + (size_t)(rok ? iy : 0) * a.w_in;
-#pragma unroll
-                        for (int kw = 0; kw < KHW; kw++)
-                        {
-                            const int ix = ix0 + kw;
-                            const uint32_t b = (rok && ix >= 0 && ix < a.w_in) ? (uint32_t)__ldg(rp + ix) : fb;
-                            const int k = (c * KHW + kh) * KHW + kw; // compile-time after unrolling
-                            row[k >> 2] |= b << (8 * (k & 3));
-                        }
-                    }
-                }
-            }
-            if (U8)
-            {
-#pragma unroll
-                for (int j = 0; j < NW; j++) sx = (int32_t)__dp4a(row[j], 0x01010101u, (unsigned)sx);
-            }
-#pragma unroll
-            for (int j = 0; j < NW / 4; j++)
-                sts_u4(sA + (uint32_t)(j >> 1) * 4096u + sw32_offset(tid, j & 1), row[4 * j], row[4 * j + 1], row[4 * j + 2], row[4 * j + 3]);
-        }
-        fence_proxy_async_smem(); // the MMAs read these generic-proxy writes through the async proxy
-        __syncthreads();          // (first iteration: also publishes the B tiles and the constants)
-        wg_mma_to_image<U8, U8>(sA, 4096u, sB, b_tile, a.ks, 32, a.ocp, sImg, pitch);
-        __syncthreads();
-
-        uint8_t* op = a.out + (size_t)pix * a.ocp;
-        const uint32_t tb = sImg + (uint32_t)tid * pitch;
-        const int32_t rowc = U8 ? -e.w_zero * sx : 0;
-        for (int c = 0; c < a.ocp; c += 16)
-        {
-            uint32_t v[16];
-            acc_ld16(tb + 4u * c, v);
-            uint32_t w[4];
-            if (U8)
-            {
-                // the int8 form (engine.cu: constants { M, M, y, y } with y = corr[oc] + bias[oc]): a' = v - zw*sum(x) + y, t = fl(a' * M)
-                if (MODE == 2)
-                {
-#pragma unroll
-                    for (int k = 0; k < 16; k++)
-                    {
-                        if ((k & 3) == 0) w[k >> 2] = 0;
-                        if (c + k < a.oc)
-                        {
-                            const float4 pp = lds_f4(sPar + c * 8 + (k >> 1) * 16);
-                            const int32_t acc = (int32_t)v[k] + rowc + __float_as_int((k & 1) ? pp.w : pp.z) - (e.has_bias ? __ldg(e.bias + c + k) : 0);
-                            w[k >> 2] |= ((uint32_t)requant(acc, c + k, e) & 0xffu) << (8 * (k & 3));
-                        }
-                    }
-                }
-                else
-                {
-                    float gw[4];
-#pragma unroll
-                    for (int h = 0; h < 2; h++)
-                    {
-                        float4 p[4];
-#pragma unroll
-                        for (int k = 0; k < 4; k++) p[k] = lds_f4(sPar + c * 8 + h * 64 + k * 16);
-                        int32_t a8[8];
-#pragma unroll
-                        for (int k = 0; k < 8; k++) a8[k] = (int32_t)v[h * 8 + k] + rowc;
-                        requant_fast8_i8<false>(a8, p, e, w[2 * h], w[2 * h + 1], gw[2 * h], gw[2 * h + 1]);
-                    }
-                    if (e.q_byte_add)
-                    {
-#pragma unroll
-                        for (int j = 0; j < 4; j++) w[j] = requant_byte_fix(w[j], e);
-                    }
-                    if (fmaxf(fmaxf(gw[0], gw[1]), fmaxf(gw[2], gw[3])) > 0.5f - TB200_TIE_EPS)
-                    {
-#pragma unroll
-                        for (int j = 0; j < 4; j++)
-                            if (gw[j] > 0.5f - TB200_TIE_EPS)
-                            {
-                                int32_t at[4]; // accumulator + y of the word's four channels (what the fast path multiplied by M)
-#pragma unroll
-                                for (int t = 0; t < 4; t++)
-                                {
-                                    const float4 pp = lds_f4(sPar + c * 8 + ((j * 4 + t) >> 1) * 16);
-                                    at[t] = (int32_t)v[j * 4 + t] + rowc + __float_as_int((t & 1) ? pp.w : pp.z);
-                                }
-                                w[j] = requant_fix_word_u8(w[j], at[0], at[1], at[2], at[3], c + j * 4, a.oc, e);
-                            }
-                    }
-                    if (c + 16 > a.oc)
-                    {
-                        // pad lanes of uint8 tensors hold 0, not the zero point
-#pragma unroll
-                        for (int k = 0; k < 16; k++)
-                            if (c + k >= a.oc) w[k >> 2] &= ~(0xffu << (8 * (k & 3)));
-                    }
-                }
-            }
-            else if (MODE == 2)
-            {
-#pragma unroll
-                for (int k = 0; k < 16; k++)
-                {
-                    if ((k & 3) == 0) w[k >> 2] = 0;
-                    if (c + k < a.oc) w[k >> 2] |= ((uint32_t)requant((int32_t)v[k], c + k, e) & 0xffu) << (8 * (k & 3));
-                }
-            }
-            else
-                stem_unit_fast<MODE == 1>(v, sPar + c * 8, c, e, w);
-            if (valid) *reinterpret_cast<uint4*>(op + c) = make_uint4(w[0], w[1], w[2], w[3]);
-        }
-        __syncthreads(); // the next tile's gather overwrites the A tiles, its MMAs the accumulator image
-    }
-}
-
-cudaError_t launch_conv_gather_tc(const void* in, const void* w, void* out, const ConvShape& s, const EpiParams& e, int nhwc16, cudaStream_t st)
-{
-    const int khw = nhwc16 ? 3 : s.kh;
-    GatherArgs a;
-    a.in = (const uint8_t*)in, a.w = (const uint8_t*)w, a.out = (uint8_t*)out;
-    a.n = s.n, a.c = s.c, a.h = s.h, a.w_in = s.w, a.oh = s.oh, a.ow = s.ow, a.ocp = s.ocp, a.oc = s.oc, a.stride = s.sh, a.ph = s.ph0, a.pw = s.pw0;
-    a.npix = (unsigned)((long long)s.n * s.oh * s.ow);
-    a.ntiles = (a.npix + 127u) / 128u;
-    a.ks = nhwc16 ? 5 : (s.c * s.kh * s.kw + 31) / 32, a.nhwc16 = nhwc16;
-    a.fill = e.is_uint8 ? ((uint32_t)(e.in_zero & 0xff) * 0x01010101u) : 0u;
-    for (int j = 0; j < 4; j++)
-    {
-        a.fill16[j] = 0;
-        for (int t = 0; t < 4; t++)
-            if (j * 4 + t < s.c) a.fill16[j] |= (a.fill & 0xffu) << (8 * t);
-    }
-    const size_t smem = (size_t)a.ks * 4096 + (size_t)a.ks * s.ocp * 32 + (size_t)s.ocp * 8 + 16 + 128 * (size_t)acc_pitch(s.ocp) + 1024;
-    static int sms = 0;
-    if (!sms)
-    {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    }
-    const unsigned cap = (unsigned)sms * 6u;
-    const unsigned grid = a.ntiles < cap ? a.ntiles : cap;
-    const int mode = !e.fast_ok ? 2 : ((!e.is_uint8 && e.fuse_bias) ? 1 : 0);
-#define TB200_GAT_CASE(MD, U, K)                                                                                                   \
-    if (mode == MD && (e.is_uint8 != 0) == U && khw == K)                                                                          \
-    {                                                                                                                              \
-        /* the opt-in is per device AND per context: set it before every launch (launches happen at graph capture only) */ \
-        {                                                                                                                          \
-            cudaError_t err = cudaFuncSetAttribute(conv_gather_tc_kernel<MD, U, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-            if (err != cudaSuccess) return err;                                                                                    \
-        }                                                                                                                          \
-        if (debug_launch()) fprintf(stderr, "tengine_b200: launch conv_gather_tc_kernel<MODE=%d,U8=%d,KHW=%d>\n", MD, (int)U, K);  \
-        conv_gather_tc_kernel<MD, U, K><<<grid, 128, smem, st>>>(a, e);                                                            \
-        return cudaGetLastError();                                                                                                 \
-    }
-    TB200_GAT_CASE(0, false, 3) TB200_GAT_CASE(1, false, 3) TB200_GAT_CASE(2, false, 3) TB200_GAT_CASE(0, true, 3) TB200_GAT_CASE(2, true, 3)
-    TB200_GAT_CASE(0, false, 7) TB200_GAT_CASE(1, false, 7) TB200_GAT_CASE(2, false, 7) TB200_GAT_CASE(0, true, 7) TB200_GAT_CASE(2, true, 7)
-#undef TB200_GAT_CASE
-    return cudaErrorInvalidValue;
-}
-
 // ---- small-K pointwise GEMM: many small CTAs instead of one warp-specialised persistent CTA ---------------------------
 // For K <= 256 (the first pointwise layers: K = 32..128, one or two k-blocks) the persistent kernel above spends more
 // time in hand-overs between its roles than in work (timeline: the epilogue warps idle ~50% of the time).  Here a CTA is
 // one warpgroup; it keeps the N tile's weights in shared memory, double-buffers the A tile (TMA), and per m-tile does:
 // wait A -> the warpgroup's MMAs into the accumulator image -> everybody requantises its own accumulator row and writes its
 // bn contiguous output bytes straight to global memory.  There is no pipelining inside a CTA beyond the A prefetch; several
-// CTAs are resident per SM (bounded by shared memory) and overlap each other, the way the tensor-core stem above does.
+// CTAs are resident per SM (bounded by shared memory) and overlap each other, as in the window kernel (conv_window.cu).
 struct SimpleArgs
 {
     uint8_t* out;
@@ -1293,34 +804,14 @@ __global__ void __launch_bounds__(128) gemm_simple_kernel(const __grid_constant_
             if (c + 1 < nch) acc_ld16(tb + (c + 1) * 64, v1);
             {
                 uint32_t w[4];
-                if (MODE == 2)
-                {
-#pragma unroll
-                    for (int k = 0; k < 16; k++)
-                    {
-                        if ((k & 3) == 0) w[k >> 2] = 0;
-                        if (n0 + c * 16 + k < g.oc) w[k >> 2] |= ((uint32_t)requant((int32_t)v0[k], n0 + c * 16 + k, e) & 0xffu) << (8 * (k & 3));
-                    }
-                }
-                else
-                    stem_unit_fast<MODE == 1>(v0, sPar + c * 128, n0 + c * 16, e, w);
+                tc_unit16<MODE, false>(v0, 0, sPar + c * 128, n0 + c * 16, g.oc, e, w);
                 if (row < g.m && n0 + c * 16 < g.ocp) *reinterpret_cast<uint4*>(op + c * 16) = make_uint4(w[0], w[1], w[2], w[3]);
             }
             if (c + 1 >= nch) break;
             if (c + 2 < nch) acc_ld16(tb + (c + 2) * 64, v0);
             {
                 uint32_t w[4];
-                if (MODE == 2)
-                {
-#pragma unroll
-                    for (int k = 0; k < 16; k++)
-                    {
-                        if ((k & 3) == 0) w[k >> 2] = 0;
-                        if (n0 + (c + 1) * 16 + k < g.oc) w[k >> 2] |= ((uint32_t)requant((int32_t)v1[k], n0 + (c + 1) * 16 + k, e) & 0xffu) << (8 * (k & 3));
-                    }
-                }
-                else
-                    stem_unit_fast<MODE == 1>(v1, sPar + (c + 1) * 128, n0 + (c + 1) * 16, e, w);
+                tc_unit16<MODE, false>(v1, 0, sPar + (c + 1) * 128, n0 + (c + 1) * 16, g.oc, e, w);
                 if (row < g.m && n0 + (c + 1) * 16 < g.ocp) *reinterpret_cast<uint4*>(op + (c + 1) * 16) = make_uint4(w[0], w[1], w[2], w[3]);
             }
         }

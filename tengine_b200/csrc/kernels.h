@@ -98,7 +98,10 @@ struct WindowPlan
 };
 int window_plan_create(WindowPlan* plan, const void* in, const ConvShape& s, int nhwc); // < 0: not applicable
 bool window_nhwc_fits(int cp, int ocp, int stride); // a 3x3 conv over an NHWC input of cp bytes per pixel fits the kernel's shared memory
-cudaError_t launch_conv_window(const WindowPlan& plan, const void* w, void* out, const ConvShape& s, const EpiParams& e, cudaStream_t st);
+cudaError_t launch_conv_window(const WindowPlan& plan, const void* w, void* out, const ConvShape& s, const EpiParams& e, int num_sms, cudaStream_t st);
+// the same layers without a window plan: every thread gathers its pixel's taps from global memory (NCHW stems, 16-channel NHWC inputs)
+cudaError_t launch_conv_gather_tc(const void* in, const void* w, void* out, const ConvShape& s, const EpiParams& e, int nhwc16, int num_sms,
+                                  cudaStream_t st);
 
 // ---- wgmma GEMM (gemm_tcgen05.cu) --------------------------------------------------------------------
 // out[M][ldo] (bytes) = requant( A[M][K] (row pitch lda bytes) . B[OCp][K]^T )
@@ -149,12 +152,6 @@ int gemm_tile_rows(int ocp, int u8); // rows of one packed B tile (u8 = 1 + weig
 int gemm_plan_create(GemmPlan* plan, const void* a, long long lda, const void* b, void* out, long long m, int k, int oc, int ocp, int ldo,
                      int variant, int u8);
 int gemm_plan_create_conv(GemmPlan* plan, const void* in, const void* w, void* out, const ConvShape& s, int u8);
-// int8 3x3 stem with C <= 3 on the tensor cores (gemm_tcgen05.cu); weights [OCp][32], k = (c*3 + kh)*3 + kw
-bool stem_tc_supported(const ConvShape& s, const EpiParams& e);
-int stem_plan_create(DwPlan* plan, const void* in, const ConvShape& s); // TMA-staged input window; <0: gather from global memory
-cudaError_t launch_stem_tc(const DwPlan& plan, const void* in, const void* w, void* out, const ConvShape& s, const EpiParams& e, cudaStream_t st);
-// 3x3 convolutions whose K the threads gather themselves (uint8 NCHW stems, 16-channel NHWC inputs), gemm_tcgen05.cu
-cudaError_t launch_conv_gather_tc(const void* in, const void* w, void* out, const ConvShape& s, const EpiParams& e, int nhwc16, cudaStream_t st);
 cudaError_t launch_gemm_i8(const GemmPlan& plan, const EpiParams& e, const int32_t* btab, int num_sms, cudaStream_t st);
 // measured peak of wgmma m64n128k32 s8 (two warpgroups per SM) on this GPU, in TOP/s: the tensor roofline's denominator
 cudaError_t probe_int8_mma_peak(int num_sms, double* tops, cudaStream_t st);

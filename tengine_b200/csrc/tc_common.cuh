@@ -1,5 +1,5 @@
 // tc_common.cuh -- device helpers shared by the tensor-core kernels (gemm_tcgen05.cu, conv_window.cu): wgmma shared-memory
-// descriptors, the accumulator image, the SW32 tile addressing of the thread-built A tiles, the per-lane fast epilogue unit.
+// descriptors, the accumulator image, the SW32 tile addressing of the thread-built A tiles, the requantising row unit.
 #pragma once
 #include "common.cuh"
 #include "ptx.cuh"
@@ -62,9 +62,34 @@ __device__ __forceinline__ void wg_mma_to_image(uint32_t sA, uint32_t a_kb, uint
         }
 }
 
-template <bool FUSE>
-__device__ __forceinline__ void stem_unit_fast(const uint32_t (&v)[16], uint32_t par_addr, int oc0, const EpiParams& e, uint32_t (&w)[4])
+// Requantise accumulator columns oc0..oc0+15 of one row (v) into four output words.  par_addr: the 16 channels' epilogue
+// constants in shared memory, 8 bytes each (unused by int8 MODE 2).  oc: real channels; pad channels come out 0.
+// MODE: 0 fast, 1 fast + fused bias (int8), 2 exact.  U8: uint8 layers in the int8 form (engine.cu: constants {M, M, y, y} with
+// y = corr[oc] + bias[oc]): a' = v + rowc + y, t = fl(a' * M), where rowc = -zw * sum(x) of the row; int8 ignores rowc.
+template <int MODE, bool U8>
+__device__ __forceinline__ void tc_unit16(const uint32_t (&v)[16], int32_t rowc, uint32_t par_addr, int oc0, int oc, const EpiParams& e,
+                                          uint32_t (&w)[4])
 {
+    if (MODE == 2)
+    {
+#pragma unroll
+        for (int k = 0; k < 16; k++)
+        {
+            if ((k & 3) == 0) w[k >> 2] = 0;
+            if (oc0 + k < oc)
+            {
+                int32_t acc = (int32_t)v[k];
+                if (U8)
+                {
+                    const float4 pp = lds_f4(par_addr + (k >> 1) * 16);
+                    acc += rowc + __float_as_int((k & 1) ? pp.w : pp.z) - (e.has_bias ? __ldg(e.bias + oc0 + k) : 0);
+                }
+                w[k >> 2] |= ((uint32_t)requant(acc, oc0 + k, e) & 0xffu) << (8 * (k & 3));
+            }
+        }
+        return;
+    }
+    constexpr bool FUSE = !U8 && MODE == 1;
     float gw[4];
 #pragma unroll
     for (int h = 0; h < 2; h++)
@@ -72,8 +97,9 @@ __device__ __forceinline__ void stem_unit_fast(const uint32_t (&v)[16], uint32_t
         float4 p[4];
 #pragma unroll
         for (int k = 0; k < 4; k++) p[k] = lds_f4(par_addr + h * 64 + k * 16);
-        const int32_t a8[8] = {(int32_t)v[h * 8], (int32_t)v[h * 8 + 1], (int32_t)v[h * 8 + 2], (int32_t)v[h * 8 + 3],
-                               (int32_t)v[h * 8 + 4], (int32_t)v[h * 8 + 5], (int32_t)v[h * 8 + 6], (int32_t)v[h * 8 + 7]};
+        int32_t a8[8];
+#pragma unroll
+        for (int k = 0; k < 8; k++) a8[k] = (int32_t)v[h * 8 + k] + (U8 ? rowc : 0);
         requant_fast8_i8<FUSE>(a8, p, e, w[2 * h], w[2 * h + 1], gw[2 * h], gw[2 * h + 1]);
     }
     if (e.q_byte_add)
@@ -86,7 +112,29 @@ __device__ __forceinline__ void stem_unit_fast(const uint32_t (&v)[16], uint32_t
 #pragma unroll
         for (int j = 0; j < 4; j++)
             if (gw[j] > 0.5f - TB200_TIE_EPS)
-                w[j] = requant_fix_word<FUSE>(w[j], (int32_t)v[j * 4], (int32_t)v[j * 4 + 1], (int32_t)v[j * 4 + 2], (int32_t)v[j * 4 + 3], oc0 + j * 4, e);
+            {
+                if (U8)
+                {
+                    int32_t at[4]; // accumulator + y of the word's four channels (what the fast path multiplied by M)
+#pragma unroll
+                    for (int t = 0; t < 4; t++)
+                    {
+                        const float4 pp = lds_f4(par_addr + ((j * 4 + t) >> 1) * 16);
+                        at[t] = (int32_t)v[j * 4 + t] + rowc + __float_as_int((t & 1) ? pp.w : pp.z);
+                    }
+                    w[j] = requant_fix_word_u8(w[j], at[0], at[1], at[2], at[3], oc0 + j * 4, oc, e);
+                }
+                else
+                    w[j] = requant_fix_word<FUSE>(w[j], (int32_t)v[j * 4], (int32_t)v[j * 4 + 1], (int32_t)v[j * 4 + 2], (int32_t)v[j * 4 + 3],
+                                                  oc0 + j * 4, e);
+            }
+    }
+    if (U8 && oc0 + 16 > oc)
+    {
+        // pad lanes of uint8 tensors hold 0, not the zero point
+#pragma unroll
+        for (int k = 0; k < 16; k++)
+            if (oc0 + k >= oc) w[k >> 2] &= ~(0xffu << (8 * (k & 3)));
     }
 }
 

@@ -58,7 +58,7 @@ class FakeGraph:
         pass
 
     def layer_kernels(self):
-        names = ["conv_stem_nchw_tcgen05", "conv_dw3x3_tma_dp4a", "gemm_i8_tcgen05", "pool"]
+        names = ["conv_window_tcgen05", "conv_dw3x3_tma_dp4a", "gemm_i8_tcgen05", "pool"]
         return [names[min(i, 3) if i < 2 else (1 + i % 2 if i < len(self.g.layers) - 2 else 3)] for i in range(len(self.g.layers))]
 
     def num_launches(self):

@@ -76,8 +76,7 @@ for mode in (0, 2):
     _add(f"fc_u8_m{mode}", lambda r, m=mode: ties.uint8_conv(r, 5, 32, 2, 2, 200, fc=True, mode=m))
 # ---- the other tensor-core families ----
 for mode in (0, 1, 2):
-    for tag, env in (("window", {}), ("stemtc_tma", {"TB200_NO_WINDOW_CONV": "1"}),
-                     ("stemtc_notma", {"TB200_NO_WINDOW_CONV": "1", "TB200_STEM_NO_TMA": "1"})):
+    for tag, env in (("window", {}), ("gather", {"TB200_NO_WINDOW_CONV": "1"})):
         _add(f"stem3x3_i8_{tag}_m{mode}", _i8(2, 3, 24, 32, 40, k=3, stride=2, pad=1, mode=mode, activation=0), env)
     _add(f"stem3x3_i8_w30_m{mode}", _i8(2, 3, 22, 30, 40, k=3, stride=1, pad=1, mode=mode), {"TB200_NO_WINDOW_CONV": "1"})
     for tag, env in (("window", {}), ("gather", {"TB200_NO_WINDOW_CONV": "1"})):
@@ -267,8 +266,6 @@ def _expected_instantiations():
                 exp.add(f"conv_window_tc_kernel<MODE={m},U8={u8},LAYOUT={ly}>")
     for m in (0, 1, 2):
         exp.add(f"gemm_simple_kernel<MODE={m}>")
-        for tma in (0, 1):
-            exp.add(f"stem_tc_kernel<MODE={m},TMA_IN={tma}>")
     for k in ("conv_dw3x3_tma_pack3_kernel", "conv_dw3x3_tma_kernel<4,2>"):
         for m in (0, 1, 2):
             exp.add(f"{k} MODE={m}")
@@ -281,8 +278,6 @@ UNREACHABLE = {
     # with the 144-column accumulator image (ACC_COLS_MAX) a 128-column N tile always runs one m-tile per stage
     **{f"gemm_i8_tcgen05_kernel<U8={u},MODE={m},CS=8,BORDER={b}>": "CS 8 needs two m-tiles of a 128-channel N tile per stage"
        for u, ms, bs in ((0, (0, 1, 2), (0,)), (1, (0, 2), (0, 1))) for m in ms for b in bs},
-    # int8 3x3 NCHW stems are planned as K_STEM_TC (stem_tc_kernel); only uint8 3x3 stems reach the window kernel's LAYOUT 0
-    **{f"conv_window_tc_kernel<MODE={m},U8=0,LAYOUT=0>": "int8 3x3 stems run on stem_tc_kernel" for m in (0, 1, 2)},
 }
 
 
