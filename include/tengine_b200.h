@@ -274,6 +274,13 @@ typedef struct tb200_detection
 } tb200_detection;
 /* out: [images][max_per_image]; counts[image] = boxes kept (negative: more than fit -- -needed is returned there) */
 TB200_API int tb200_graph_yolo_detect(tb200_graph* g, const tb200_yolo_params* p, tb200_detection* out, int max_per_image, int32_t* counts);
+/* The same for YOLOv5 heads: restates examples/tm_yolov5s.cpp:140-207,561-576.  Parameters, output layout and the overflow
+ * convention are those of tb200_graph_yolo_detect; only the box formula differs:
+ *   centre = (sigmoid(tx) * 2 - 0.5 + w) * stride, size = sigmoid(tw) * sigmoid(tw) * 4 * anchor_w  (float, in that order).
+ * Quantised heads are dequantised as ((float)q - zero_point) * scale.  Pass the heads in the example's proposal order:
+ * stride 32, 16, 8 (:567-572), with anchors {116,90, 156,198, 373,326}, {30,61, 62,45, 59,119}, {10,13, 16,30, 33,23} (:143).
+ * The example's letterbox back-mapping (:580-626) is left to the caller: boxes are in network-input pixels. */
+TB200_API int tb200_graph_yolov5_detect(tb200_graph* g, const tb200_yolo_params* p, tb200_detection* out, int max_per_image, int32_t* counts);
 
 /* ---- kernel launchers (device pointers; NHWC with channels padded to tb200k_cpad(c)) --------------- */
 typedef struct tb200k_epilogue

@@ -83,7 +83,13 @@ struct YoloDet
     float x, y, w, h, prob;
     int label;
 };
-cudaError_t launch_yolo_decode(const void* tensor, int cp, int h, int w, int n_img, int anchors_n, int classes, const float* sig, const double* ex, float stride,
+// box formula of the region decode: examples/tm_yolov3_tiny_uint8.cpp (V3) or examples/tm_yolov5s.cpp (V5)
+enum class YoloBox
+{
+    V3,
+    V5
+};
+cudaError_t launch_yolo_decode(YoloBox f, const void* tensor, int cp, int h, int w, int n_img, int classes, const float* sig, const double* ex, float stride,
                                const float* anchors6, float thr, YoloCand* cand, int* count, int max_cand, unsigned key_base, bool is_u8, cudaStream_t st);
 cudaError_t launch_yolo_nms(const YoloCand* cand, const int* count, int n_img, int max_cand, float nms_thr, YoloCand* sorted, YoloDet* out, int max_out,
                             int* out_count, cudaStream_t st);

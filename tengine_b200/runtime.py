@@ -269,10 +269,13 @@ class Graph:
         _check(lib().tb200_graph_arena_bytes(self.h, C.byref(a), C.byref(u), C.byref(w)))
         return a.value, u.value, w.value
 
-    def yolo_detect(self, heads, num_classes=80, prob_threshold=0.4, nms_threshold=0.25, max_per_image=256, max_candidates=0):
-        """Region decode + NMS on the device from the graph's output tensors of the last run (tb200_graph_yolo_detect).
+    def yolo_detect(self, heads, num_classes=80, prob_threshold=0.4, nms_threshold=0.25, max_per_image=256, max_candidates=0, version=3):
+        """Region decode + NMS on the device from the graph's output tensors of the last run: tb200_graph_yolo_detect (version=3,
+        the box formula of examples/tm_yolov3_tiny_uint8.cpp) or tb200_graph_yolov5_detect (version=5, examples/tm_yolov5s.cpp).
         heads: [(graph output index, stride, six anchor values)] in proposal order.  Returns per image a list of
         (x, y, w, h, prob, label)."""
+        if version not in (3, 5):
+            raise ValueError(f"version must be 3 or 5, not {version!r}")
         p = abi.YoloParams()
         p.num_heads = len(heads)
         for i, (oi, stride, anchors) in enumerate(heads):
@@ -283,8 +286,9 @@ class Graph:
         n = self.gdef.dims(self.gdef.outputs[0])[0]
         out = (abi.Detection * (n * max_per_image))()
         counts = (C.c_int32 * n)()
-        lib().tb200_graph_yolo_detect.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
-        _check(lib().tb200_graph_yolo_detect(self.h, C.byref(p), out, int(max_per_image), counts))
+        fn = lib().tb200_graph_yolo_detect if version == 3 else lib().tb200_graph_yolov5_detect
+        fn.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
+        _check(fn(self.h, C.byref(p), out, int(max_per_image), counts))
         res = []
         for i in range(n):
             if counts[i] < 0:
