@@ -204,6 +204,33 @@ TB200_API int tb200_graph_launch(tb200_graph* g);                 /* asynchronou
 TB200_API int tb200_graph_download(tb200_graph* g, int output_index, void* host_nchw);
 TB200_API int tb200_graph_sync(tb200_graph* g);
 
+/* ---- classification preprocessing on the device -----------------------------------------------------------------------------
+ * Decoded 8-bit images in, the quantised graph input out.  Restates what examples/tm_classification_int8.c:43-62
+ * (get_input_int8_data) and examples/tm_classification_uint8.c:43-62 (get_input_uint8_data) do per image through
+ * examples/common/tengine_operations.c: load_image_stb (:51-82; RGBA loses its alpha byte), rgb2bgr_permute (:651-673; output plane k
+ * is source channel 2 - k), the fixed-point bilinear resize tengine_resize_f32 (:870-979, non-NEON branch; 11-bit weights from float
+ * positions, including its extrapolating first outputs of an upsample and its last output taking source pixel w - 2 with weight 1),
+ * imread2caffe (:101-115: (v - mean[k]) * scale[k]), then int8: round(x / scale) clamped to +-127, uint8: round(x / scale +
+ * zero_point) clamped to 0..255, with the graph input's own H, W, scale and zero point.  round() takes halfway cases away from zero; a
+ * quotient outside int's range (or NaN) converts to INT_MIN as on x86-64 and so clamps to -127 / 0. */
+typedef struct tb200_image
+{
+    uint64_t offset; /* byte offset of pixel (0,0) in the pixel buffer */
+    int32_t w, h, c; /* h rows of w pixels of c interleaved bytes, rows unpadded: what stbi_load returns; c = 3 (RGB) or 4 (RGBA) */
+} tb200_image;
+/* Fills graph input `input_index` ([N, 3, H, W], int8 or uint8) from images[0..N) on the device, byte for byte as the examples'
+ * get_input_int8_data / get_input_uint8_data would fill the host tensor for each image.  `mean` and `scale` index the B, G, R planes,
+ * as the examples' -w / -s options do.  Images may have different sizes and lie anywhere in the buffer.
+ * pixels: HOST memory, page-locked in place like tb200_graph_run's buffers; it must stay unchanged until a tb200_graph_sync has
+ * returned after this call.  Asynchronous on the context stream, like tb200_graph_upload; follow with tb200_graph_launch.
+ * Checked before anything is copied: TB200_ERR_INVALID for a null argument, an input index out of range, an input whose dims[1] != 3,
+ * w or h outside 2..32767 (the resize reads column w - 2 and keeps positions in int16_t), an image not inside pixel_bytes, a
+ * non-finite mean or scale.  TB200_ERR_UNSUPPORTED for c other than 3 or 4: for c == 1 the example's gray2bgr (:694-713) writes three
+ * interleaved copies into an image it then reads as planar, so there is no meaningful result to reproduce; for c == 2
+ * rgb2bgr_permute writes plane 2 - c outside a two-plane image. */
+TB200_API int tb200_graph_upload_images(tb200_graph* g, int input_index, const void* pixels, size_t pixel_bytes,
+                                        const tb200_image* images, const float mean[3], const float scale[3]);
+
 /* interface->post_run (device.h:53) */
 TB200_API int tb200_graph_postrun(tb200_graph* g);
 

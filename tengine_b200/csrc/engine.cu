@@ -221,6 +221,13 @@ struct tb200_graph
     int first_image = 0, num_images = 0, total_images = 0;
     size_t act_unshared_bytes = 0; // what the arena would need without slot reuse (introspection)
     int pack_cache_state = 0;      // 0 no cache directory, 1 packed and written, 2 read from the cache
+    // tb200_graph_upload_images: device copy of this shard's pixel span, its image descriptors (staged through page-locked host
+    // memory that is rewritten only after img_ev, the previous descriptor copy, has completed); grown on demand
+    uint8_t* img_stage = nullptr;
+    size_t img_stage_bytes = 0;
+    ImageDesc *img_desc = nullptr, *img_desc_host = nullptr;
+    int img_desc_cap = 0;
+    cudaEvent_t img_ev = nullptr;
 };
 
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
@@ -530,6 +537,10 @@ static void destroy_graph(tb200_graph* g)
     for (auto p : g->out_nchw_dev) cudaFree(p);
     cudaFree(g->act_arena);
     cudaFree(g->w_arena);
+    cudaFree(g->img_stage);
+    cudaFree(g->img_desc);
+    cudaFreeHost(g->img_desc_host);
+    if (g->img_ev) cudaEventDestroy(g->img_ev);
     delete g;
 }
 
@@ -1959,6 +1970,71 @@ int tb200_graph_upload(tb200_graph* g, int input_index, const void* host_nchw)
         const int id = sh->input_ids[input_index];
         CUDA_OK(cudaMemcpyAsync(sh->in_nchw_dev[input_index], (const uint8_t*)host_nchw + (size_t)sh->first_image * image_bytes(sh, id),
                                 sh->tensors[id].nchw_bytes, cudaMemcpyHostToDevice, sh->ctx->stream));
+        return 0;
+    });
+    cudaSetDevice(g->ctx->device);
+    return rc;
+}
+
+// Every shard copies the byte span of its own images (in whatever order they lie in the caller's buffer) and their descriptors, then
+// one image_pre launch fills the shard's NCHW input buffer -- the buffer tb200_graph_upload fills -- so the captured graph runs as is.
+int tb200_graph_upload_images(tb200_graph* g, int input_index, const void* pixels, size_t pixel_bytes, const tb200_image* images, const float mean[3],
+                              const float scale[3])
+{
+    static_assert(sizeof(ImageDesc) == sizeof(tb200_image) && offsetof(ImageDesc, w) == offsetof(tb200_image, w), "image descriptor layout");
+    if (!g || !pixels || !images || !mean || !scale || input_index < 0 || input_index >= (int)g->input_ids.size())
+        return fail(TB200_ERR_INVALID, "bad upload_images arguments");
+    const tb200_tensor_desc& td = g->tensors[g->input_ids[input_index]].d;
+    if (td.dims[1] != 3) return fail(TB200_ERR_INVALID, "upload_images: input %d has %d channels, not 3", input_index, td.dims[1]);
+    if (td.data_type != TB200_DT_INT8 && td.data_type != TB200_DT_UINT8) return fail(TB200_ERR_INVALID, "upload_images: input %d is not int8 / uint8", input_index);
+    for (int k = 0; k < 3; k++)
+        if (!std::isfinite(mean[k]) || !std::isfinite(scale[k])) return fail(TB200_ERR_INVALID, "upload_images: mean / scale %d is not finite", k);
+    for (int i = 0; i < g->total_images; i++)
+    {
+        const tb200_image& im = images[i];
+        if (im.c != 3 && im.c != 4) return fail(TB200_ERR_UNSUPPORTED, "upload_images: image %d has %d channels (3 or 4 supported)", i, im.c);
+        if (im.w < 2 || im.h < 2 || im.w > 32767 || im.h > 32767) return fail(TB200_ERR_INVALID, "upload_images: image %d is %d x %d (2..32767)", i, im.w, im.h);
+        const uint64_t bytes = (uint64_t)im.w * (uint64_t)im.h * (uint64_t)im.c;
+        if (im.offset > pixel_bytes || bytes > pixel_bytes - im.offset)
+            return fail(TB200_ERR_INVALID, "upload_images: image %d (offset %llu, %llu bytes) lies outside the %zu-byte pixel buffer", i, (unsigned long long)im.offset,
+                        (unsigned long long)bytes, pixel_bytes);
+    }
+    CUDA_OK(cudaSetDevice(g->ctx->device));
+    host_pin(g->ctx, pixels, pixel_bytes);
+    const bool u8 = td.data_type == TB200_DT_UINT8;
+    const int rc = for_each_shard(g, [&](tb200_graph* sh, int) -> int {
+        CUDA_OK(cudaSetDevice(sh->ctx->device));
+        cudaGetLastError(); // the launch below reports cudaGetLastError(): a non-sticky error an earlier call left behind is not its own
+        const int n = sh->num_images;
+        const tb200_image* im = images + sh->first_image;
+        uint64_t lo = UINT64_MAX, hi = 0;
+        for (int i = 0; i < n; i++)
+            lo = std::min(lo, im[i].offset), hi = std::max(hi, im[i].offset + (uint64_t)im[i].w * im[i].h * im[i].c);
+        if (hi - lo > sh->img_stage_bytes)
+        {
+            cudaFree(sh->img_stage);
+            sh->img_stage = nullptr, sh->img_stage_bytes = 0;
+            CUDA_OK(cudaMalloc(&sh->img_stage, hi - lo));
+            sh->img_stage_bytes = hi - lo;
+        }
+        if (!sh->img_ev) CUDA_OK(cudaEventCreateWithFlags(&sh->img_ev, cudaEventDisableTiming));
+        CUDA_OK(cudaEventSynchronize(sh->img_ev)); // the previous descriptor copy has read the host staging
+        if (n > sh->img_desc_cap)
+        {
+            cudaFree(sh->img_desc), cudaFreeHost(sh->img_desc_host);
+            sh->img_desc = sh->img_desc_host = nullptr, sh->img_desc_cap = 0;
+            CUDA_OK(cudaMalloc(&sh->img_desc, sizeof(ImageDesc) * n));
+            CUDA_OK(cudaHostAlloc(&sh->img_desc_host, sizeof(ImageDesc) * n, cudaHostAllocDefault));
+            sh->img_desc_cap = n;
+        }
+        for (int i = 0; i < n; i++) sh->img_desc_host[i] = ImageDesc{im[i].offset - lo, im[i].w, im[i].h, im[i].c};
+        cudaStream_t st = sh->ctx->stream;
+        CUDA_OK(cudaMemcpyAsync(sh->img_stage, (const uint8_t*)pixels + lo, hi - lo, cudaMemcpyHostToDevice, st));
+        CUDA_OK(cudaMemcpyAsync(sh->img_desc, sh->img_desc_host, sizeof(ImageDesc) * n, cudaMemcpyHostToDevice, st));
+        CUDA_OK(cudaEventRecord(sh->img_ev, st));
+        const cudaError_t e = launch_image_pre(sh->img_stage, sh->img_desc, n, sh->in_nchw_dev[input_index], td.dims[2], td.dims[3], mean, scale, td.scale,
+                                               td.zero_point, u8, st);
+        if (e != cudaSuccess) return fail(TB200_ERR_CUDA, "upload_images: launch of image_pre failed: %s", cudaGetErrorString(e));
         return 0;
     });
     cudaSetDevice(g->ctx->device);

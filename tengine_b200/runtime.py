@@ -49,6 +49,8 @@ def lib():
                      "tb200_graph_work", "tb200_context_destroy"):
             getattr(L, name).restype = C.c_int
         L.tb200_graph_upload.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        L.tb200_graph_upload_images.restype = C.c_int
+        L.tb200_graph_upload_images.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]
         L.tb200_graph_download.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         L.tb200_graph_launch.argtypes = [C.c_void_p]
         L.tb200_graph_sync.argtypes = [C.c_void_p]
@@ -219,6 +221,33 @@ class Graph:
     def upload(self, i, x):
         _check(lib().tb200_graph_upload(self.h, i, x.ctypes.data))
 
+    def upload_images(self, i, images, mean, scale):
+        """Fill graph input i on the device from decoded images (tb200_graph_upload_images): one HxWxC uint8 array per image of the
+        batch, C = 3 (RGB) or 4 (RGBA), sizes may differ; mean and scale index the B, G, R planes.  The pixels are packed into a
+        page-locked buffer kept on the graph; since an earlier upload may still be reading it, packing first waits for the graph's
+        queued work.  Asynchronous like upload: follow with launch and download."""
+        imgs = [np.ascontiguousarray(a) for a in images]
+        if len(imgs) != self.gdef.dims(self.gdef.inputs[i])[0]:
+            raise ValueError(f"{len(imgs)} images for a batch of {self.gdef.dims(self.gdef.inputs[i])[0]}")
+        descs = (abi.Image * len(imgs))()
+        off = 0
+        for d, a in zip(descs, imgs):
+            if a.dtype != np.uint8 or a.ndim != 3:
+                raise ValueError(f"images must be HxWxC uint8 arrays, not {a.dtype} {a.shape}")
+            d.offset, d.h, d.w, d.c = off, a.shape[0], a.shape[1], a.shape[2]
+            off += a.nbytes
+        self.sync()
+        buf = getattr(self, "_pixels", None)
+        if buf is None or buf.nbytes < off:
+            if buf is not None:
+                buf.free()
+            buf = self._pixels = PinnedBuffer((off,), np.uint8)
+        for d, a in zip(descs, imgs):
+            buf.array[d.offset:d.offset + a.nbytes] = a.reshape(-1)
+        m = (C.c_float * 3)(*[float(v) for v in mean])
+        s = (C.c_float * 3)(*[float(v) for v in scale])
+        _check(lib().tb200_graph_upload_images(self.h, i, buf.ptr, buf.nbytes, descs, m, s))
+
     def launch(self):
         _check(lib().tb200_graph_launch(self.h))
 
@@ -304,3 +333,6 @@ class Graph:
         if self.h:
             lib().tb200_graph_postrun(self.h)
             self.h = C.c_void_p()
+        if getattr(self, "_pixels", None) is not None:
+            self._pixels.free()
+            self._pixels = None
