@@ -231,6 +231,49 @@ typedef struct tb200_image
 TB200_API int tb200_graph_upload_images(tb200_graph* g, int input_index, const void* pixels, size_t pixel_bytes,
                                         const tb200_image* images, const float mean[3], const float scale[3]);
 
+/* ---- detection preprocessing on the device ----------------------------------------------------------------------------------
+ * Decoded 8-bit images in, the quantised input of a YOLO graph out, byte for byte as the examples fill it after cv::imread(file, 1) and
+ * cv::cvtColor(BGR2RGB), so the planes are R, G, B and mean / scale index R, G, B (unlike tb200_graph_upload_images):
+ *   TB200_PRE_STRETCH    examples/tm_yolov3_tiny_uint8.cpp:136-170 (tm_yolov4_tiny_uint8.cpp:137-170): cv::resize to the input's W x H.
+ *   TB200_PRE_LETTERBOX  examples/tm_yolov5s.cpp:263-337 / :339-392: a float scale chosen by a double comparison, resized size
+ *                        int(scale * cols) (a float product truncated: it can be one short of the input size), cv::resize to it,
+ *                        borders top = (H - resize_h) / 2, left = (W - resize_w) / 2, filled by cv::copyMakeBorder with byte 0
+ *                        (its destination takes the 8-bit source type, so the grey float image built before it is unused).
+ * cv::resize is INTER_LINEAR on 8-bit images as OpenCV computes it: float positions from double arithmetic, 11-bit weights rounded to
+ * nearest, the horizontal position clamped to the image, the vertical one not (rows are clipped instead, so an upscale's first and last
+ * rows blend a row with itself), and the two-term fixed-point vertical sum of OpenCV's SIMD path.  Then (v - mean[c]) * scale[c] in
+ * float and round(x / s_in + (float)zero_point) clamped to +-127 (int8) or 0..255 (uint8), halfway cases away from zero, a quotient
+ * out of int's range (or NaN) -> INT_MIN as on x86-64 (tm_yolox_int8.cpp:336-341, tm_yolov3_tiny_uint8.cpp:164-168).
+ * focus = 1: the YOLOv5 (<= v5) Focus slicing of tm_yolov5s.cpp:317-337: the image is laid out at H x W and output channel
+ * (i * 2 + g) * 3 + c takes column offset i and row offset g of plane c; the graph input is then [N, 12, H/2, W/2]. */
+#define TB200_PRE_STRETCH 0
+#define TB200_PRE_LETTERBOX 1
+typedef struct tb200_detect_pre
+{
+    int32_t mode;     /* TB200_PRE_STRETCH | TB200_PRE_LETTERBOX */
+    int32_t focus;    /* 1: graph input [N, 12, H/2, W/2] from an H x W image; 0: graph input [N, 3, H, W] */
+    float mean[3];    /* R, G, B */
+    float scale[3];
+} tb200_detect_pre;
+/* Where image i landed in the H x W laid-out input, computed on the host with the example's own arithmetic.  Stretch: resize = W x H,
+ * left = top = 0, scale = 0.  Letterbox: the resized size, the left / top borders and scale_letterbox. */
+typedef struct tb200_detect_geometry
+{
+    int32_t src_w, src_h;       /* the image's size */
+    int32_t resize_w, resize_h; /* the size cv::resize produced */
+    int32_t left, top;          /* its position in the laid-out image */
+    float scale;
+} tb200_detect_geometry;
+/* Fills graph input `input_index` from images[0..N) on the device and writes each image's geometry to geometry_out[0..N) (host memory;
+ * NULL skips it).  Images, buffer and asynchrony are those of tb200_graph_upload_images; follow with tb200_graph_launch.  Checked before
+ * anything is copied: TB200_ERR_INVALID for a null argument, an input index out of range, an input that is not int8 / uint8, a mode
+ * other than the two, focus not 0 / 1, an input whose dims[1] is not 3 (12 with focus), w or h outside 2..32767,
+ * an image not inside pixel_bytes, a letterbox whose resized width or height would be 0, a non-finite mean or scale;
+ * TB200_ERR_UNSUPPORTED for c other than 3 or 4. */
+TB200_API int tb200_graph_upload_detect_images(tb200_graph* g, int input_index, const void* pixels, size_t pixel_bytes, const tb200_image* images,
+                                               const tb200_detect_pre* pre, tb200_detect_geometry* geometry_out);
+/* tb200_detections_to_source (after tb200_detection below) maps the boxes found in such an input back to source pixels. */
+
 /* interface->post_run (device.h:53) */
 TB200_API int tb200_graph_postrun(tb200_graph* g);
 
@@ -306,8 +349,17 @@ TB200_API int tb200_graph_yolo_detect(tb200_graph* g, const tb200_yolo_params* p
  *   centre = (sigmoid(tx) * 2 - 0.5 + w) * stride, size = sigmoid(tw) * sigmoid(tw) * 4 * anchor_w  (float, in that order).
  * Quantised heads are dequantised as ((float)q - zero_point) * scale.  Pass the heads in the example's proposal order:
  * stride 32, 16, 8 (:567-572), with anchors {116,90, 156,198, 373,326}, {30,61, 62,45, 59,119}, {10,13, 16,30, 33,23} (:143).
- * The example's letterbox back-mapping (:580-626) is left to the caller: boxes are in network-input pixels. */
+ * Boxes are in network-input pixels; tb200_detections_to_source applies the example's letterbox back-mapping (:580-626). */
 TB200_API int tb200_graph_yolov5_detect(tb200_graph* g, const tb200_yolo_params* p, tb200_detection* out, int max_per_image, int32_t* counts);
+/* Pure host function (no GPU needed), the step the examples take after NMS: rewrites dets[i * max_per_image + k], k < counts[i], from
+ * network-input pixels to source pixels of image i in place, `mode` and geometry[i] as tb200_graph_upload_detect_images used and returned
+ * them.  Stretch: tm_yolov3_tiny_uint8.cpp:501-532 (multiply by source size / input size).  Letterbox: tm_yolov5s.cpp:580-625 (subtract
+ * left / top, then multiply x by src_h / resize_h and y by src_w / resize_w -- the example's swap, kept).  Both then clamp the corners to
+ * [0, src_w - 1] x [0, src_h - 1] and rebuild w / h from them, in float.  Images with a negative (overflow) count are left as they are.
+ * TB200_ERR_INVALID for a bad mode, a null pointer, num_images < 0, max_per_image < 1, a count above max_per_image or a geometry size
+ * below 1. */
+TB200_API int tb200_detections_to_source(int mode, const tb200_detect_geometry* geometry, int num_images, tb200_detection* dets, int max_per_image,
+                                         const int32_t* counts);
 
 /* ---- kernel launchers (device pointers; NHWC with channels padded to tb200k_cpad(c)) --------------- */
 typedef struct tb200k_epilogue

@@ -59,7 +59,7 @@ EXPORTS = [
     "tb200_context_stream", "tb200_context_create_multi", "tb200_context_num_gpus", "tb200_context_gpu", "tb200_context_stream_of",
     "tb200_context_broadcast_kind", "tb200_shard_range", "tb200_graph_broadcast_weights", "tb200_graph_num_shards", "tb200_graph_shard", "tb200_graph_arena_bytes", "tb200_probe_int8_tops", "tb200_pack_cache_dir", "tb200_graph_pack_cache_state", "tb200_graph_yolo_detect", "tb200_graph_yolov5_detect", "tb200k_conv_winograd43_f32_workspace", "tb200k_conv_winograd43_f32", "tb200k_conv_dw3x3_f32",
     "tb200_host_alloc", "tb200_host_free", "tb200_graph_prerun", "tb200_graph_run",
-    "tb200_graph_upload", "tb200_graph_upload_images", "tb200_graph_launch", "tb200_graph_download", "tb200_graph_sync", "tb200_graph_postrun",
+    "tb200_graph_upload", "tb200_graph_upload_images", "tb200_graph_upload_detect_images", "tb200_detections_to_source", "tb200_graph_launch", "tb200_graph_download", "tb200_graph_sync", "tb200_graph_postrun",
     "tb200_graph_weight_arena", "tb200_graph_num_launches", "tb200_graph_layer_kernel", "tb200_graph_read_tensor",
     "tb200_graph_profile", "tb200_graph_work", "tb200k_cpad", "tb200k_conv_direct", "tb200k_conv_dw3x3",
     "tb200k_conv_stem_nchw", "tb200k_gemm_i8", "tb200k_nchw_to_nhwc", "tb200k_nhwc_to_nchw",
@@ -68,6 +68,18 @@ EXPORTS = [
 
 class Image(C.Structure):
     _fields_ = [("offset", C.c_uint64), ("w", C.c_int32), ("h", C.c_int32), ("c", C.c_int32)]
+
+
+PRE_STRETCH, PRE_LETTERBOX = 0, 1
+
+
+class DetectPre(C.Structure):
+    _fields_ = [("mode", C.c_int32), ("focus", C.c_int32), ("mean", C.c_float * 3), ("scale", C.c_float * 3)]
+
+
+class DetectGeometry(C.Structure):
+    _fields_ = [("src_w", C.c_int32), ("src_h", C.c_int32), ("resize_w", C.c_int32), ("resize_h", C.c_int32), ("left", C.c_int32),
+                ("top", C.c_int32), ("scale", C.c_float)]
 
 
 class YoloHead(C.Structure):

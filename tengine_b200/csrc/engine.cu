@@ -1976,37 +1976,41 @@ int tb200_graph_upload(tb200_graph* g, int input_index, const void* host_nchw)
     return rc;
 }
 
-// Every shard copies the byte span of its own images (in whatever order they lie in the caller's buffer) and their descriptors, then
-// one image_pre launch fills the shard's NCHW input buffer -- the buffer tb200_graph_upload fills -- so the captured graph runs as is.
-int tb200_graph_upload_images(tb200_graph* g, int input_index, const void* pixels, size_t pixel_bytes, const tb200_image* images, const float mean[3],
-                              const float scale[3])
+// Checks shared by the image upload entry points: every descriptor of the batch names a 3- or 4-channel image of 2..32767 pixels a side
+// inside the buffer, and mean / scale are finite.  `what` names the entry point in the message.
+static int check_images(const tb200_graph* g, const char* what, size_t pixel_bytes, const tb200_image* images, const float* mean, const float* scale)
 {
-    static_assert(sizeof(ImageDesc) == sizeof(tb200_image) && offsetof(ImageDesc, w) == offsetof(tb200_image, w), "image descriptor layout");
-    if (!g || !pixels || !images || !mean || !scale || input_index < 0 || input_index >= (int)g->input_ids.size())
-        return fail(TB200_ERR_INVALID, "bad upload_images arguments");
-    const tb200_tensor_desc& td = g->tensors[g->input_ids[input_index]].d;
-    if (td.dims[1] != 3) return fail(TB200_ERR_INVALID, "upload_images: input %d has %d channels, not 3", input_index, td.dims[1]);
-    if (td.data_type != TB200_DT_INT8 && td.data_type != TB200_DT_UINT8) return fail(TB200_ERR_INVALID, "upload_images: input %d is not int8 / uint8", input_index);
     for (int k = 0; k < 3; k++)
-        if (!std::isfinite(mean[k]) || !std::isfinite(scale[k])) return fail(TB200_ERR_INVALID, "upload_images: mean / scale %d is not finite", k);
+        if (!std::isfinite(mean[k]) || !std::isfinite(scale[k])) return fail(TB200_ERR_INVALID, "%s: mean / scale %d is not finite", what, k);
     for (int i = 0; i < g->total_images; i++)
     {
         const tb200_image& im = images[i];
-        if (im.c != 3 && im.c != 4) return fail(TB200_ERR_UNSUPPORTED, "upload_images: image %d has %d channels (3 or 4 supported)", i, im.c);
-        if (im.w < 2 || im.h < 2 || im.w > 32767 || im.h > 32767) return fail(TB200_ERR_INVALID, "upload_images: image %d is %d x %d (2..32767)", i, im.w, im.h);
+        if (im.c != 3 && im.c != 4) return fail(TB200_ERR_UNSUPPORTED, "%s: image %d has %d channels (3 or 4 supported)", what, i, im.c);
+        if (im.w < 2 || im.h < 2 || im.w > 32767 || im.h > 32767) return fail(TB200_ERR_INVALID, "%s: image %d is %d x %d (2..32767)", what, i, im.w, im.h);
         const uint64_t bytes = (uint64_t)im.w * (uint64_t)im.h * (uint64_t)im.c;
         if (im.offset > pixel_bytes || bytes > pixel_bytes - im.offset)
-            return fail(TB200_ERR_INVALID, "upload_images: image %d (offset %llu, %llu bytes) lies outside the %zu-byte pixel buffer", i, (unsigned long long)im.offset,
+            return fail(TB200_ERR_INVALID, "%s: image %d (offset %llu, %llu bytes) lies outside the %zu-byte pixel buffer", what, i, (unsigned long long)im.offset,
                         (unsigned long long)bytes, pixel_bytes);
     }
+    return 0;
+}
+
+// Every shard copies the byte span of its own images (in whatever order they lie in the caller's buffer) and their descriptors, then
+// `launch(shard, staged pixels, descriptors, n, stream)` fills the shard's NCHW input buffer -- the buffer tb200_graph_upload fills -- so
+// the captured graph runs as is.  geo: per image of the batch the detection geometry the descriptors carry, or null.
+extern "C++" {
+template <typename Launch>
+static int upload_staged_images(tb200_graph* g, const char* what, const void* pixels, size_t pixel_bytes, const tb200_image* images,
+                                const tb200_detect_geometry* geo, Launch launch)
+{
     CUDA_OK(cudaSetDevice(g->ctx->device));
     host_pin(g->ctx, pixels, pixel_bytes);
-    const bool u8 = td.data_type == TB200_DT_UINT8;
     const int rc = for_each_shard(g, [&](tb200_graph* sh, int) -> int {
         CUDA_OK(cudaSetDevice(sh->ctx->device));
         cudaGetLastError(); // the launch below reports cudaGetLastError(): a non-sticky error an earlier call left behind is not its own
         const int n = sh->num_images;
         const tb200_image* im = images + sh->first_image;
+        const tb200_detect_geometry* gm = geo ? geo + sh->first_image : nullptr;
         uint64_t lo = UINT64_MAX, hi = 0;
         for (int i = 0; i < n; i++)
             lo = std::min(lo, im[i].offset), hi = std::max(hi, im[i].offset + (uint64_t)im[i].w * im[i].h * im[i].c);
@@ -2027,18 +2031,130 @@ int tb200_graph_upload_images(tb200_graph* g, int input_index, const void* pixel
             CUDA_OK(cudaHostAlloc(&sh->img_desc_host, sizeof(ImageDesc) * n, cudaHostAllocDefault));
             sh->img_desc_cap = n;
         }
-        for (int i = 0; i < n; i++) sh->img_desc_host[i] = ImageDesc{im[i].offset - lo, im[i].w, im[i].h, im[i].c};
+        for (int i = 0; i < n; i++)
+            sh->img_desc_host[i] = gm ? ImageDesc{im[i].offset - lo, im[i].w, im[i].h, im[i].c, gm[i].resize_w, gm[i].resize_h, gm[i].left, gm[i].top}
+                                      : ImageDesc{im[i].offset - lo, im[i].w, im[i].h, im[i].c, 0, 0, 0, 0};
         cudaStream_t st = sh->ctx->stream;
         CUDA_OK(cudaMemcpyAsync(sh->img_stage, (const uint8_t*)pixels + lo, hi - lo, cudaMemcpyHostToDevice, st));
         CUDA_OK(cudaMemcpyAsync(sh->img_desc, sh->img_desc_host, sizeof(ImageDesc) * n, cudaMemcpyHostToDevice, st));
         CUDA_OK(cudaEventRecord(sh->img_ev, st));
-        const cudaError_t e = launch_image_pre(sh->img_stage, sh->img_desc, n, sh->in_nchw_dev[input_index], td.dims[2], td.dims[3], mean, scale, td.scale,
-                                               td.zero_point, u8, st);
-        if (e != cudaSuccess) return fail(TB200_ERR_CUDA, "upload_images: launch of image_pre failed: %s", cudaGetErrorString(e));
+        const cudaError_t e = launch(sh, sh->img_stage, sh->img_desc, n, st);
+        if (e != cudaSuccess) return fail(TB200_ERR_CUDA, "%s: launch of its kernel failed: %s", what, cudaGetErrorString(e));
         return 0;
     });
     cudaSetDevice(g->ctx->device);
     return rc;
+}
+} // extern "C++"
+
+int tb200_graph_upload_images(tb200_graph* g, int input_index, const void* pixels, size_t pixel_bytes, const tb200_image* images, const float mean[3],
+                              const float scale[3])
+{
+    static_assert(offsetof(ImageDesc, w) == offsetof(tb200_image, w) && offsetof(ImageDesc, c) == offsetof(tb200_image, c), "image descriptor layout");
+    if (!g || !pixels || !images || !mean || !scale || input_index < 0 || input_index >= (int)g->input_ids.size())
+        return fail(TB200_ERR_INVALID, "bad upload_images arguments");
+    const tb200_tensor_desc& td = g->tensors[g->input_ids[input_index]].d;
+    if (td.dims[1] != 3) return fail(TB200_ERR_INVALID, "upload_images: input %d has %d channels, not 3", input_index, td.dims[1]);
+    if (td.data_type != TB200_DT_INT8 && td.data_type != TB200_DT_UINT8) return fail(TB200_ERR_INVALID, "upload_images: input %d is not int8 / uint8", input_index);
+    if (const int rc = check_images(g, "upload_images", pixel_bytes, images, mean, scale)) return rc;
+    const bool u8 = td.data_type == TB200_DT_UINT8;
+    return upload_staged_images(g, "upload_images", pixels, pixel_bytes, images, nullptr,
+                                [&](tb200_graph* sh, const uint8_t* px, const ImageDesc* desc, int n, cudaStream_t st) {
+                                    return launch_image_pre(px, desc, n, sh->in_nchw_dev[input_index], td.dims[2], td.dims[3], mean, scale, td.scale,
+                                                            td.zero_point, u8, st);
+                                });
+}
+
+// Where an image of src_w x src_h lands in the W x H laid-out input: stretch fills it; letterbox restates examples/tm_yolov5s.cpp:274-295
+// (the scale compared in double and kept in float, the resized size a float product truncated, the borders halved downwards).
+static tb200_detect_geometry detect_geometry(int mode, int src_w, int src_h, int W, int H)
+{
+    tb200_detect_geometry r{src_w, src_h, W, H, 0, 0, 0.f};
+    if (mode == TB200_PRE_STRETCH) return r;
+    float scale_letterbox;
+    if ((H * 1.0 / src_h) < (W * 1.0 / src_w))
+        scale_letterbox = H * 1.0 / src_h;
+    else
+        scale_letterbox = W * 1.0 / src_w;
+    r.resize_w = int(scale_letterbox * (float)src_w);
+    r.resize_h = int(scale_letterbox * (float)src_h);
+    r.left = (W - r.resize_w) / 2, r.top = (H - r.resize_h) / 2;
+    r.scale = scale_letterbox;
+    return r;
+}
+
+int tb200_graph_upload_detect_images(tb200_graph* g, int input_index, const void* pixels, size_t pixel_bytes, const tb200_image* images,
+                                     const tb200_detect_pre* pre, tb200_detect_geometry* geometry_out)
+{
+    if (!g || !pixels || !images || !pre || input_index < 0 || input_index >= (int)g->input_ids.size())
+        return fail(TB200_ERR_INVALID, "bad upload_detect_images arguments");
+    if (pre->mode != TB200_PRE_STRETCH && pre->mode != TB200_PRE_LETTERBOX) return fail(TB200_ERR_INVALID, "upload_detect_images: mode %d", pre->mode);
+    if (pre->focus != 0 && pre->focus != 1) return fail(TB200_ERR_INVALID, "upload_detect_images: focus %d (0 or 1)", pre->focus);
+    const tb200_tensor_desc& td = g->tensors[g->input_ids[input_index]].d;
+    const bool focus = pre->focus == 1;
+    if (td.dims[1] != (focus ? 12 : 3))
+        return fail(TB200_ERR_INVALID, "upload_detect_images: input %d has %d channels, not %d", input_index, td.dims[1], focus ? 12 : 3);
+    if (td.data_type != TB200_DT_INT8 && td.data_type != TB200_DT_UINT8)
+        return fail(TB200_ERR_INVALID, "upload_detect_images: input %d is not int8 / uint8", input_index);
+    // the laid-out image: the input's own H x W, or twice it with Focus
+    const int H = focus ? td.dims[2] * 2 : td.dims[2], W = focus ? td.dims[3] * 2 : td.dims[3];
+    if (const int rc = check_images(g, "upload_detect_images", pixel_bytes, images, pre->mean, pre->scale)) return rc;
+    std::vector<tb200_detect_geometry> geo(g->total_images);
+    for (int i = 0; i < g->total_images; i++)
+    {
+        geo[i] = detect_geometry(pre->mode, images[i].w, images[i].h, W, H);
+        if (geo[i].resize_w < 1 || geo[i].resize_h < 1 || geo[i].resize_w > W || geo[i].resize_h > H)
+            return fail(TB200_ERR_INVALID, "upload_detect_images: image %d (%d x %d) letterboxes to %d x %d in %d x %d", i, images[i].w, images[i].h,
+                        geo[i].resize_w, geo[i].resize_h, W, H);
+    }
+    const bool u8 = td.data_type == TB200_DT_UINT8;
+    const int rc = upload_staged_images(g, "upload_detect_images", pixels, pixel_bytes, images, geo.data(),
+                                        [&](tb200_graph* sh, const uint8_t* px, const ImageDesc* desc, int n, cudaStream_t st) {
+                                            return launch_detect_pre(px, desc, n, sh->in_nchw_dev[input_index], H, W, focus, pre->mean, pre->scale, td.scale,
+                                                                     td.zero_point, u8, st);
+                                        });
+    if (rc == 0 && geometry_out) std::copy(geo.begin(), geo.end(), geometry_out);
+    return rc;
+}
+
+// examples/tm_yolov3_tiny_uint8.cpp:501-532 (stretch) / tm_yolov5s.cpp:580-625 (letterbox), one box at a time, in float as there
+static void box_to_source(int mode, const tb200_detect_geometry& gm, tb200_detection& d)
+{
+    float x0 = d.x, y0 = d.y, x1 = d.x + d.w, y1 = d.y + d.h;
+    if (mode == TB200_PRE_STRETCH)
+    {
+        const float ratio_x = (float)gm.src_w / gm.resize_w, ratio_y = (float)gm.src_h / gm.resize_h;
+        x0 = x0 * ratio_x, y0 = y0 * ratio_y, x1 = x1 * ratio_x, y1 = y1 * ratio_y;
+    }
+    else
+    {
+        const float ratio_x = (float)gm.src_h / gm.resize_h, ratio_y = (float)gm.src_w / gm.resize_w; // rows for x: the example's own
+        x0 = (x0 - gm.left) * ratio_x, y0 = (y0 - gm.top) * ratio_y;
+        x1 = (x1 - gm.left) * ratio_x, y1 = (y1 - gm.top) * ratio_y;
+    }
+    x0 = std::max(std::min(x0, (float)(gm.src_w - 1)), 0.f);
+    y0 = std::max(std::min(y0, (float)(gm.src_h - 1)), 0.f);
+    x1 = std::max(std::min(x1, (float)(gm.src_w - 1)), 0.f);
+    y1 = std::max(std::min(y1, (float)(gm.src_h - 1)), 0.f);
+    d.x = x0, d.y = y0, d.w = x1 - x0, d.h = y1 - y0;
+}
+
+int tb200_detections_to_source(int mode, const tb200_detect_geometry* geometry, int num_images, tb200_detection* dets, int max_per_image,
+                               const int32_t* counts)
+{
+    if (mode != TB200_PRE_STRETCH && mode != TB200_PRE_LETTERBOX) return fail(TB200_ERR_INVALID, "detections_to_source: mode %d", mode);
+    if (num_images < 0 || max_per_image < 1 || (num_images > 0 && (!geometry || !dets || !counts)))
+        return fail(TB200_ERR_INVALID, "bad detections_to_source arguments");
+    for (int i = 0; i < num_images; i++)
+    {
+        const tb200_detect_geometry& gm = geometry[i];
+        if (counts[i] > max_per_image) return fail(TB200_ERR_INVALID, "detections_to_source: image %d has %d boxes, more than %d", i, counts[i], max_per_image);
+        if (gm.src_w < 1 || gm.src_h < 1 || gm.resize_w < 1 || gm.resize_h < 1)
+            return fail(TB200_ERR_INVALID, "detections_to_source: image %d has geometry %d x %d -> %d x %d", i, gm.src_w, gm.src_h, gm.resize_w, gm.resize_h);
+    }
+    for (int i = 0; i < num_images; i++)
+        for (int k = 0; k < counts[i]; k++) box_to_source(mode, geometry[i], dets[(size_t)i * max_per_image + k]);
+    return 0;
 }
 
 static int launch_one(tb200_graph* g)

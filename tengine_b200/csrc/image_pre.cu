@@ -9,6 +9,7 @@
 // share a batch and no host tables exist.
 #include "common.cuh"
 #include "kernels.h"
+#include "preproc.cuh"
 
 namespace tb200 {
 
@@ -24,15 +25,6 @@ __device__ __forceinline__ void resize_coef(int i, int in, float scale, int& s, 
     if (s >= in - 1) s = in - 2, f = 0.f;
     c1 = (int)(int16_t)(int)__fmul_rn(f, 2048.f);
     c0 = (int)(int16_t)(int)__fmul_rn(__fsub_rn(1.f, f), 2048.f);
-}
-
-// round(x) of <math.h> (halfway cases away from zero), then the conversion to int of the x86-64 build: a value outside int's range,
-// or NaN, becomes INT_MIN (cvttsd2si), which the examples' clamps then send to their lower bound.
-__device__ __forceinline__ int round_to_int_x86(float x)
-{
-    float r = truncf(x);
-    if (fabsf(__fsub_rn(x, r)) >= 0.5f) r = __fadd_rn(r, copysignf(1.f, x));
-    return (r >= -2147483648.f && r < 2147483648.f) ? (int)r : INT_MIN;
 }
 
 // One CTA per output row (image n, row y); its threads walk the row's pixels and write the three planes' bytes, coalesced along x.

@@ -94,15 +94,21 @@ cudaError_t launch_yolo_decode(YoloBox f, const void* tensor, int cp, int h, int
 cudaError_t launch_yolo_nms(const YoloCand* cand, const int* count, int n_img, int max_cand, float nms_thr, YoloCand* sorted, YoloDet* out, int max_out,
                             int* out_count, cudaStream_t st);
 
-// ---- classification preprocessing (image_pre.cu) ---------------------------------------------------------------
-struct ImageDesc // the layout of tb200_image: h rows of w pixels of c interleaved bytes (c = 3 or 4), starting at `offset`
+// ---- input preprocessing (image_pre.cu, detect_pre.cu) ------------------------------------------------------------
+// One image of a staged batch: h rows of w pixels of c interleaved bytes (c = 3 or 4) at `offset` of the shard's staging buffer; for
+// detection also where its resized copy lies in the laid-out image (tb200_detect_geometry; unused by image_pre)
+struct ImageDesc
 {
     uint64_t offset;
     int32_t w, h, c;
+    int32_t resize_w, resize_h, left, top;
 };
 // out: [n][3][H][W] int8 (u8 = false) or uint8 bytes, as examples/tm_classification_{int8,uint8}.c would fill the input tensor
 cudaError_t launch_image_pre(const uint8_t* pixels, const ImageDesc* images, int n, uint8_t* out, int H, int W, const float mean[3], const float scale[3],
                              float s_in, int zp, bool u8, cudaStream_t st);
+// out: [n][3][H][W], or with focus [n][12][H/2][W/2], int8 or uint8 bytes as the YOLO examples fill the input tensor (tengine_b200.h)
+cudaError_t launch_detect_pre(const uint8_t* pixels, const ImageDesc* images, int n, uint8_t* out, int H, int W, bool focus, const float mean[3],
+                              const float scale[3], float s_in, int zp, bool u8, cudaStream_t st);
 
 // ---- small-Cin convolutions with a TMA-staged input window (conv_window.cu) -----------------------------------
 struct WindowPlan

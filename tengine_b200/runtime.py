@@ -51,6 +51,10 @@ def lib():
         L.tb200_graph_upload.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         L.tb200_graph_upload_images.restype = C.c_int
         L.tb200_graph_upload_images.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.tb200_graph_upload_detect_images.restype = C.c_int
+        L.tb200_graph_upload_detect_images.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.tb200_detections_to_source.restype = C.c_int
+        L.tb200_detections_to_source.argtypes = [C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p]
         L.tb200_graph_download.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         L.tb200_graph_launch.argtypes = [C.c_void_p]
         L.tb200_graph_sync.argtypes = [C.c_void_p]
@@ -95,6 +99,22 @@ def shard_range(n_images, world, rank):
     f, c = C.c_int(), C.c_int()
     _check(lib().tb200_shard_range(int(n_images), int(world), int(rank), C.byref(f), C.byref(c)))
     return f.value, c.value
+
+
+def detections_to_source(geometry, boxes, letterbox=True):
+    """Per image a list of (x, y, w, h, prob, label) in network-input pixels -> the same in source pixels of that image, mapped by
+    tb200_detections_to_source with the geometry Graph.upload_detect_images returned (letterbox: its mode)."""
+    n, m = len(boxes), max([1] + [len(b) for b in boxes])
+    if len(geometry) != n:
+        raise ValueError(f"{len(geometry)} geometries for {n} images")
+    dets = (abi.Detection * (n * m))()
+    counts = (C.c_int32 * n)(*[len(b) for b in boxes])
+    for i, img in enumerate(boxes):
+        for k, b in enumerate(img):
+            d = dets[i * m + k]
+            d.x, d.y, d.w, d.h, d.prob, d.label = b
+    _check(lib().tb200_detections_to_source(abi.PRE_LETTERBOX if letterbox else abi.PRE_STRETCH, geometry, n, dets, m, counts))
+    return [[(d.x, d.y, d.w, d.h, d.prob, d.label) for d in dets[i * m:i * m + counts[i]]] for i in range(n)]
 
 
 def device_count():
@@ -221,11 +241,9 @@ class Graph:
     def upload(self, i, x):
         _check(lib().tb200_graph_upload(self.h, i, x.ctypes.data))
 
-    def upload_images(self, i, images, mean, scale):
-        """Fill graph input i on the device from decoded images (tb200_graph_upload_images): one HxWxC uint8 array per image of the
-        batch, C = 3 (RGB) or 4 (RGBA), sizes may differ; mean and scale index the B, G, R planes.  The pixels are packed into a
-        page-locked buffer kept on the graph; since an earlier upload may still be reading it, packing first waits for the graph's
-        queued work.  Asynchronous like upload: follow with launch and download."""
+    def _stage_pixels(self, i, images):
+        """The images packed into a page-locked buffer kept on the graph (waiting first for the graph's queued work, which may still
+        read it) and their descriptors."""
         imgs = [np.ascontiguousarray(a) for a in images]
         if len(imgs) != self.gdef.dims(self.gdef.inputs[i])[0]:
             raise ValueError(f"{len(imgs)} images for a batch of {self.gdef.dims(self.gdef.inputs[i])[0]}")
@@ -244,9 +262,31 @@ class Graph:
             buf = self._pixels = PinnedBuffer((off,), np.uint8)
         for d, a in zip(descs, imgs):
             buf.array[d.offset:d.offset + a.nbytes] = a.reshape(-1)
+        return buf, descs
+
+    def upload_images(self, i, images, mean, scale):
+        """Fill graph input i on the device from decoded images (tb200_graph_upload_images): one HxWxC uint8 array per image of the
+        batch, C = 3 (RGB) or 4 (RGBA), sizes may differ; mean and scale index the B, G, R planes.  The pixels are packed into a
+        page-locked buffer kept on the graph; since an earlier upload may still be reading it, packing first waits for the graph's
+        queued work.  Asynchronous like upload: follow with launch and download."""
+        buf, descs = self._stage_pixels(i, images)
         m = (C.c_float * 3)(*[float(v) for v in mean])
         s = (C.c_float * 3)(*[float(v) for v in scale])
         _check(lib().tb200_graph_upload_images(self.h, i, buf.ptr, buf.nbytes, descs, m, s))
+
+    def upload_detect_images(self, i, images, mean, scale, letterbox=True, focus=False):
+        """Fill graph input i on the device from decoded images as the YOLO examples prepare them (tb200_graph_upload_detect_images):
+        letterboxed as tm_yolov5s.cpp or stretched as tm_yolov3_tiny_uint8.cpp, with the Focus slicing when focus (the input is then
+        [N, 12, H/2, W/2]).  Images as for upload_images, but mean and scale index the R, G, B planes.  Returns the per-image geometry
+        (a ctypes array of abi.DetectGeometry) that yolo_detect / detections_to_source take to map boxes back to the images."""
+        buf, descs = self._stage_pixels(i, images)
+        pre = abi.DetectPre()
+        pre.mode, pre.focus = (abi.PRE_LETTERBOX if letterbox else abi.PRE_STRETCH), int(bool(focus))
+        for k in range(3):
+            pre.mean[k], pre.scale[k] = float(mean[k]), float(scale[k])
+        geo = (abi.DetectGeometry * len(descs))()
+        _check(lib().tb200_graph_upload_detect_images(self.h, i, buf.ptr, buf.nbytes, descs, C.byref(pre), geo))
+        return geo
 
     def launch(self):
         _check(lib().tb200_graph_launch(self.h))
@@ -298,11 +338,13 @@ class Graph:
         _check(lib().tb200_graph_arena_bytes(self.h, C.byref(a), C.byref(u), C.byref(w)))
         return a.value, u.value, w.value
 
-    def yolo_detect(self, heads, num_classes=80, prob_threshold=0.4, nms_threshold=0.25, max_per_image=256, max_candidates=0, version=3):
+    def yolo_detect(self, heads, num_classes=80, prob_threshold=0.4, nms_threshold=0.25, max_per_image=256, max_candidates=0, version=3,
+                    geometry=None, letterbox=True):
         """Region decode + NMS on the device from the graph's output tensors of the last run: tb200_graph_yolo_detect (version=3,
         the box formula of examples/tm_yolov3_tiny_uint8.cpp) or tb200_graph_yolov5_detect (version=5, examples/tm_yolov5s.cpp).
         heads: [(graph output index, stride, six anchor values)] in proposal order.  Returns per image a list of
-        (x, y, w, h, prob, label)."""
+        (x, y, w, h, prob, label), in network-input pixels, or with `geometry` (from upload_detect_images, made with the same
+        `letterbox`) in source pixels of each image (tb200_detections_to_source)."""
         if version not in (3, 5):
             raise ValueError(f"version must be 3 or 5, not {version!r}")
         p = abi.YoloParams()
@@ -318,6 +360,10 @@ class Graph:
         fn = lib().tb200_graph_yolo_detect if version == 3 else lib().tb200_graph_yolov5_detect
         fn.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
         _check(fn(self.h, C.byref(p), out, int(max_per_image), counts))
+        if geometry is not None:
+            if len(geometry) != n:
+                raise ValueError(f"{len(geometry)} geometries for {n} images")
+            _check(lib().tb200_detections_to_source(abi.PRE_LETTERBOX if letterbox else abi.PRE_STRETCH, geometry, n, out, int(max_per_image), counts))
         res = []
         for i in range(n):
             if counts[i] < 0:
