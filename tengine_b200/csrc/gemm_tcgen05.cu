@@ -341,7 +341,7 @@ __device__ __forceinline__ void epilogue_unit_u8(const uint32_t (&v)[16], int32_
 // cut at the top (a), bottom (b), left (c), right (d); index into the table engine.cu builds
 __device__ __forceinline__ uint32_t padding_taps(const GemmArgs& g, int mt, int r)
 {
-    if (!g.conv || g.taps == 1 && g.pad_h == 0 && g.pad_w == 0) return 0;
+    if (!g.conv) return 0; // (a 1x1 convolution padded at the bottom / right only has border pixels too)
     int n0, oh0, ow0;
     tile_origin(g, mt, n0, oh0, ow0);
     const int t = (int)(((uint32_t)r * g.bw_rcp) >> 16), w = r - t * g.bw;
@@ -1248,8 +1248,10 @@ cudaError_t launch_gemm_i8(const GemmPlan& p, const EpiParams& e, const int32_t*
     memcpy(&tt, p.tmap_out_tail, sizeof tt);
     const int mode = !e.fast_ok ? 2 : ((!p.u8 && e.fuse_bias) ? 1 : 0);
     cudaError_t err = cudaErrorInvalidValue;
-    // uint8 border corrections only exist for convolutions with taps that can fall into the padding
-    const bool border = p.u8 && p.conv && !(p.taps == 1 && p.pad_h == 0 && p.pad_w == 0);
+    // uint8 border corrections only exist for convolutions with taps that can fall into the padding: any window larger than one
+    // pixel, or a 1x1 window whose last row / column lies past the image (bottom / right padding, e.g. TF-style (0, 1))
+    const bool pad_1x1 = p.pad_h || p.pad_w || (p.oh - 1) * p.cstride >= p.in_h || (p.ow - 1) * p.cstride >= p.in_w;
+    const bool border = p.u8 && p.conv && (p.taps > 1 || pad_1x1);
 #define TB200_GEMM_CASE(U, MD, C, B)                                                                                           \
     if ((p.u8 != 0) == U && mode == MD && p.cs == C && border == B)                                                            \
     {                                                                                                                          \
@@ -1260,8 +1262,8 @@ cudaError_t launch_gemm_i8(const GemmPlan& p, const EpiParams& e, const int32_t*
             if (err != cudaSuccess) return err;                                                                                \
         }                                                                                                                      \
         if (launch_dbg)                                                                                                        \
-            fprintf(stderr, "tengine_b200: launch gemm_i8_tcgen05_kernel<U8=%d,MODE=%d,CS=%d,BORDER=%d> out_mode=%d conv=%d n_tiles=%d b_res=%d fixq=%d\n", \
-                    (int)U, MD, C, (int)B, p.out_mode, p.conv, p.n_tiles, p.b_res, p.fixq != nullptr);                      \
+            fprintf(stderr, "tengine_b200: launch gemm_i8_tcgen05_kernel<U8=%d,MODE=%d,CS=%d,BORDER=%d> out_mode=%d conv=%d n_tiles=%d b_res=%d fixq=%d mt=%d par_all=%d\n", \
+                    (int)U, MD, C, (int)B, p.out_mode, p.conv, p.n_tiles, p.b_res, p.fixq != nullptr, p.mt, g.par_all);     \
         gemm_i8_tcgen05_kernel<U, MD, C, B><<<grid, U ? GEMM_THREADS_U8 : GEMM_THREADS, smem, st>>>(ta, tb, to, tt, g, e);                           \
         if (trace_on) gemm_trace_report(p, g, grid, st);                                                                       \
         err = cudaGetLastError();                                                                                              \

@@ -266,7 +266,7 @@ def _expected_instantiations():
                 exp.add(f"conv_window_tc_kernel<MODE={m},U8={u8},LAYOUT={ly}>")
     for m in (0, 1, 2):
         exp.add(f"gemm_simple_kernel<MODE={m}>")
-    for k in ("conv_dw3x3_tma_pack3_kernel", "conv_dw3x3_tma_kernel<4,2>"):
+    for k in ("conv_dw3x3_tma_pack3_kernel", "conv_dw3x3_tma_kernel<4,2>", "conv_dw3x3_tma_kernel<8,1>"):
         for m in (0, 1, 2):
             exp.add(f"{k} MODE={m}")
     return exp
@@ -281,15 +281,21 @@ UNREACHABLE = {
 }
 
 
+# the stride-1 depthwise cases once more with TB200_DW_NO_PACK3 (read once per process): conv_dw3x3_tma_kernel<8,1>
+NO_PACK3 = [n for n in CASES if n.startswith("dw3x3_i8_s1")]
+
+
 def test_every_reachable_instantiation_is_launched():
-    """All cases in one child process with TB200_DEBUG_LAUNCH: every instantiation a launcher can select appears in its report."""
-    r = _child([n for n in CASES if n not in PW_EXACT], {"TB200_DEBUG_LAUNCH": "1"}, timeout=1800)
-    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
+    """All cases in one child process with TB200_DEBUG_LAUNCH (and the stride-1 depthwise ones in a second, without the packed
+    kernel): every instantiation a launcher can select appears in their report."""
     launched = set()
-    for line in r.stderr.splitlines():
-        m = re.match(r"tengine_b200: launch (\S+(?: MODE=\d)?)", line)
-        if m:
-            launched.add(m.group(1))
+    for names, env in (([n for n in CASES if n not in PW_EXACT], {}), (NO_PACK3, {"TB200_DW_NO_PACK3": "1"})):
+        r = _child(names, {"TB200_DEBUG_LAUNCH": "1", **env}, timeout=1800)
+        assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
+        for line in r.stderr.splitlines():
+            m = re.match(r"tengine_b200: launch (\S+(?: MODE=\d)?)", line)
+            if m:
+                launched.add(m.group(1))
     exp = _expected_instantiations()
     missing = sorted(exp - launched - set(UNREACHABLE))
     print("launched:", sorted(launched))
