@@ -275,18 +275,13 @@ cudaError_t launch_conv_dw_tma(const DwPlan& p, const void* w, void* out, const 
     dim3 grid((s.cp + DW_CH - 1) / DW_CH, (s.oh + p.rows_per_cta - 1) / p.rows_per_cta, s.n);
     CUtensorMap tm;
     memcpy(&tm, p.tmap_in, sizeof tm);
-    static const bool pack3 = getenv("TB200_DW_NO_PACK3") == nullptr;
     // not templated on the epilogue: MODE is the run-time choice of the same rule as the other launchers (2 = exact)
     if (debug_launch())
-        fprintf(stderr, "tengine_b200: launch %s MODE=%d\n",
-                s.sh == 1 ? (pack3 ? "conv_dw3x3_tma_pack3_kernel" : "conv_dw3x3_tma_kernel<8,1>") : "conv_dw3x3_tma_kernel<4,2>",
+        fprintf(stderr, "tengine_b200: launch %s MODE=%d\n", s.sh == 1 ? "conv_dw3x3_tma_pack3_kernel" : "conv_dw3x3_tma_kernel<4,2>",
                 !e.fast_ok ? 2 : (!e.is_uint8 && e.fuse_bias ? 1 : 0));
-    if (s.sh == 1 && pack3)
+    if (s.sh == 1)
         conv_dw3x3_tma_pack3_kernel<<<grid, DW_THREADS, p.smem_bytes, st>>>(tm, (const uint8_t*)w, (uint8_t*)out, s, e, p.rows_per_cta, p.gpr,
                                                                            p.tile_cols, p.tile_rows);
-    else if (s.sh == 1)
-        conv_dw3x3_tma_kernel<8, 1><<<grid, DW_THREADS, p.smem_bytes, st>>>(tm, (const uint8_t*)w, (uint8_t*)out, s, e, p.rows_per_cta, p.gpr,
-                                                                            p.tile_cols, p.tile_rows);
     else
         conv_dw3x3_tma_kernel<4, 2><<<grid, DW_THREADS, p.smem_bytes, st>>>(tm, (const uint8_t*)w, (uint8_t*)out, s, e, p.rows_per_cta, p.gpr,
                                                                             p.tile_cols, p.tile_rows);

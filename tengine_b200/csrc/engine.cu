@@ -27,7 +27,7 @@ using namespace tb200;
 
 #define TB200_OP_NOP_ (-1)  // planner-internal: a node folded into its producer
 #define TB200_OP_LUT2_ (-2) // planner-internal: Sigmoid + Eltwise-PROD with the Sigmoid's input, as one byte table
-#define TB200_PACK_FORMAT 4  // bump whenever the layout or content of the packed weight arena changes (pack cache key)
+#define TB200_PACK_FORMAT 5  // bump whenever the layout or content of the packed weight arena changes (pack cache key)
 
 // ---- packed-weight cache directory (SURVEY.md 8(f)-3): tb200_pack_cache_dir() or the environment ----
 static std::string g_pack_cache_dir;
@@ -467,11 +467,11 @@ static EpiParams make_epi(const tb200_layer_desc& L, const tb200_tensor_desc& ti
     return e;
 }
 
-// bytes of the packed B operand of the tensor-core paths: [n_tiles][block_n (+16 for uint8: the ones-row)][K]
-static size_t gemm_weight_bytes(int ocp, int k, bool u8)
+// bytes of the packed B operand of the tensor-core paths: [n_tiles][block_n][K]
+static size_t gemm_weight_bytes(int ocp, int k)
 {
-    const int bn = gemm_block_n(ocp, u8), nt = (ocp + bn - 1) / bn;
-    return (size_t)nt * (bn + (u8 ? 16 : 0)) * k;
+    const int bn = gemm_block_n(ocp), nt = (ocp + bn - 1) / bn;
+    return (size_t)nt * bn * k;
 }
 
 struct WeightBlob
@@ -794,10 +794,10 @@ static int plan_conv(int li, const tb200_layer_desc& L, const TensorInfo& tin, c
     else if (L.group == C && OC == C && C > 1)
         P.kind = K_CONV_DW, wsize = (size_t)L.kernel_h * L.kernel_w * tin.cp;
     else if (tc && u8_tc_on && L.kernel_h == 1 && L.kernel_w == 1 && L.stride_h == 1 && L.stride_w == 1 && !L.pad_h0 && !L.pad_h1 && !L.pad_w0 && !L.pad_w1)
-        P.kind = K_GEMM, wsize = gemm_weight_bytes(tout.cp, tin.cp, u8);
+        P.kind = K_GEMM, wsize = gemm_weight_bytes(tout.cp, tin.cp);
     else if (tc && u8_tc_on && plain && (L.stride_h == 1 || L.stride_h == 2) && (L.kernel_h * L.kernel_w == 1 || tin.cp % 32 == 0) &&
              tout.d.dims[3] <= 4096 && L.kernel_h * L.kernel_w <= 64 && !getenv("TB200_NO_IGEMM"))
-        P.kind = K_IGEMM, wsize = gemm_weight_bytes(tout.cp, L.kernel_h * L.kernel_w * tin.cp, u8);
+        P.kind = K_IGEMM, wsize = gemm_weight_bytes(tout.cp, L.kernel_h * L.kernel_w * tin.cp);
     else
     {
         if (L.group > 1 && ((cg % 4) || ((OC / L.group) % 4)))
@@ -840,7 +840,7 @@ static int plan_kernels(tb200_graph* g, std::vector<LayerPlan>& plan)
             if (no_tc || (u8 && getenv("TB200_NO_U8_TC")))
                 P.kind = K_CONV_DIRECT, P.blob.w_size = (size_t)tout.cp * H * W * tin.cp; // FC == conv with kernel HxW over the whole input
             else
-                P.kind = K_GEMM, P.blob.w_size = gemm_weight_bytes(tout.cp, H * W * tin.cp, u8);
+                P.kind = K_GEMM, P.blob.w_size = gemm_weight_bytes(tout.cp, H * W * tin.cp);
         }
         else if (L.op == TB200_OP_POOL)
             P.kind = K_POOL;
@@ -1146,30 +1146,25 @@ static void pack_conv_weights(const tb200_layer_desc& L, const LayerPlan& P, con
         return;
     }
     // One row of `taps` groups of cgp bytes per output channel; an FC is a conv with kernel HxW over the whole input
-    // ([OC][C*H*W], the NCHW flatten of fc_ref.c:313-359 -> [row][H][W][Cp]).  Output channel o sits in row brow(o): uint8
-    // tensor-core tiles carry 16 extra rows each.
+    // ([OC][C*H*W], the NCHW flatten of fc_ref.c:313-359 -> [row][H][W][Cp]).
     const bool fc = L.op == TB200_OP_FC, gemm = P.kind == K_GEMM || P.kind == K_IGEMM, u8 = tin.d.data_type == TB200_DT_UINT8;
     const int taps = fc ? tin.d.dims[2] * tin.d.dims[3] : KH * KW, cin = fc ? C : cg;
     const int cgp = P.kind == K_CONV_STEM ? 4 : ((fc || L.group == 1) ? tin.cp : cg);
     const size_t krow = (size_t)taps * cgp;
-    const int bn = gemm ? gemm_block_n(tout.cp, u8) : tout.cp, bnx = gemm ? gemm_tile_rows(tout.cp, P.gemm_zp) : bn;
-    auto brow = [&](int o) -> size_t { return (size_t)(o / bn) * bnx + (o % bn); };
     for (int o = 0; o < OC; o++)
         for (int c = 0; c < cin; c++)
-            for (int t = 0; t < taps; t++) dst[(brow(o) * taps + t) * cgp + c] = src[((size_t)o * cin + c) * taps + t];
+            for (int t = 0; t < taps; t++) dst[((size_t)o * taps + t) * cgp + c] = src[((size_t)o * cin + c) * taps + t];
     if (!(gemm && u8)) return;
-    // the tensor cores form sum x*(w - zw) themselves: B = w - 128 as int8 (plus a constant tile of 128 - zw in the kernel), or
-    // plain w when zw == 0.  Real K positions only; pad positions stay 0 (x is 0 there anyway).
+    // the tensor cores form sum x*(w - 128): B = w - 128 as int8 (the epilogue adds (128 - zw) * sum(x)), or plain w when
+    // zw == 0.  Real K positions only; pad positions stay 0 (x is 0 there anyway).
     if (L.weight_zero != 0)
         for (int o = 0; o < OC; o++)
             for (int t = 0; t < taps; t++)
                 for (int c = 0; c < cin; c++)
                 {
-                    uint8_t& w = dst[brow(o) * krow + (size_t)t * cgp + c];
+                    uint8_t& w = dst[(size_t)o * krow + (size_t)t * cgp + c];
                     w = (uint8_t)(int8_t)((int)w - 128);
                 }
-    if (bnx != bn) // sum(x) of every pixel from the main MMA: 16 rows of ones close every B tile (gemm_tcgen05.cu, sx_mode 0)
-        for (int tile = 0; tile * bn < tout.cp; tile++) memset(dst + ((size_t)tile * bnx + bn) * krow, 1, (size_t)16 * krow);
 }
 
 // uint8 K_IGEMM: what the taps that fall into the padding must give back.  A tap t contributes zx*(sum_c w - Cin*zw) when it is
@@ -1317,7 +1312,7 @@ static uint64_t pack_cache_key(const tb200_graph* g, const std::vector<LayerPlan
     uint64_t h = kFnvBasis;
     auto mix = [&](const void* p, size_t n) { h = fnv1a(p, n, h); };
     const int num_layers = (int)g->layers.size();
-    const int ver = TB200_PACK_FORMAT * 16 + gemm_sx_mode();
+    const int ver = TB200_PACK_FORMAT;
     mix(&ver, sizeof ver), mix(&g->w_bytes, sizeof g->w_bytes), mix(&num_layers, sizeof num_layers);
     for (int li = 0; li < num_layers; li++)
     {
@@ -1505,7 +1500,7 @@ static int fill_conv_step(tb200_graph* g, int li, const LayerPlan& P, const Slic
     {
         const long long m = fc ? N : (long long)N * H * W;
         const int kdim = fc ? H * W * tin.cp : tin.cp;
-        int rc = gemm_plan_create(&s.gemm, s.in, kdim, s.w, s.out, m, kdim, OC, tout.cp, tout.cp, 0, P.gemm_zp);
+        int rc = gemm_plan_create(&s.gemm, s.in, kdim, s.w, s.out, m, kdim, OC, tout.cp, tout.cp, P.gemm_zp);
         if (rc) return fail(rc, "layer %d: TMA descriptor creation failed (m=%lld k=%d oc=%d)", li, m, kdim, OC);
         s.gemm.fixq = g->ctx->fixq, s.gemm.fixq_cap = FIXQ_CAP;
     }
@@ -2580,7 +2575,7 @@ int tb200k_gemm_i8(const void* in, const void* weight, void* out, int64_t m, int
     if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
         return fail(TB200_ERR_NO_DEVICE, "no CUDA device");
     GemmPlan plan;
-    int rc = gemm_plan_create(&plan, in, k_pad, weight, out, m, k_pad, oc, cpad(oc), cpad(oc), 0, 0);
+    int rc = gemm_plan_create(&plan, in, k_pad, weight, out, m, k_pad, oc, cpad(oc), cpad(oc), 0);
     if (rc) return fail(rc, "gemm plan failed");
     EpiParams p = epi_from_abi(e);
     K_LAUNCH(launch_gemm_i8(plan, p, nullptr, sms, (cudaStream_t)stream));

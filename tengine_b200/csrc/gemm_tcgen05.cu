@@ -13,7 +13,7 @@
 //               half of the N tile's 16-column chunks, issues wgmma per ring stage, releases the stage after
 //               wgmma.wait_group and finally writes its s32 fragments into the accumulator image ([128 rows][BN] in
 //               shared memory).  Epilogue: four warps per 32-row quarter of the image; a warp owns whole "store groups"
-//               = 32 rows x 16/32/64 channels: image -> registers -> requant_fast4_i8 -> bytes -> its own swizzled smem
+//               = 32 rows x 16/32 channels: image -> registers -> requant_fast4_i8 -> bytes -> its own swizzled smem
 //               buffer -> ONE TMA store per group (cp.async.bulk.tensor, double-buffered).  No address arithmetic for the
 //               stores, rows outside the tensor are clipped by the TMA unit.
 // The producer runs ahead through the ring while the epilogue works, so the next tile's operands are resident when its
@@ -44,8 +44,8 @@ static constexpr int GEMM_THREADS = 32 + EPI_THREADS;
 static constexpr int SUM_WARP0 = EPI_WARPS + 1, SUM_WARPS = 2; // uint8 kernels only: two warps that add up the rows of every A tile (sum x)
 static constexpr int GEMM_THREADS_U8 = GEMM_THREADS + 32 * SUM_WARPS;
 static constexpr int PRODUCER_WARP = EPI_WARPS;
-static constexpr int ACC_COLS_MAX = 144; // columns of the accumulator image (m-tiles per stage x B tile rows)
-static constexpr int MMA_CHUNKS = 5;     // 16-column chunks of one warpgroup: half of at most 144 columns
+static constexpr int ACC_COLS_MAX = 128; // columns of the accumulator image (m-tiles per stage x block_n)
+static constexpr int MMA_CHUNKS = 4;     // 16-column chunks of one warpgroup: half of at most 128 columns
 static constexpr int PAR_MAX = 2048; // channels whose epilogue constants stay resident in smem for the whole kernel
 static constexpr int MAX_STAGES = 24;
 static constexpr int B_RESIDENT_MAX = 96 * 1024; // weights of the CTA's N tile stay in smem when they fit in this many bytes
@@ -80,11 +80,10 @@ struct GemmArgs
     // uint8 (unsigned A): B holds w - 128 as int8 (plain w when zw == 0), so the accumulator is sum x*(w - 128); what is left of
     // sum x*(w - zw) is cplane * sum(x) with cplane = 128 - zw, and the epilogue adds cplane * sum(x) inside the IADD3 that also
     // adds the per-channel constant.
-    int u8, bnx, taps, in_h, in_w, b_signed, cplane;
-    int sx_mode; // where sum(x) comes from when cplane != 0: 3 = two extra warps add up the rows of every A tile in shared memory (default), 0 = 16 rows of ones inside every B tile (TB200_U8_SX=0)
-    int tcols; // accumulator image columns per m-tile: bnx (block_n, + 16 when 16 rows of ones in B form sum(x))
+    // sum(x) comes from two extra warps that add up the rows of every A tile in shared memory (cplane != 0 only).
+    int u8, taps, in_h, in_w, b_signed, cplane;
     // epilogue / stores
-    int cs, ngroups; // 16-column chunks per store group (1, 2 or 4) and groups per m-tile
+    int cs, ngroups; // 16-column chunks per store group (1 or 2) and groups per m-tile
     int rows_valid;  // rows of an m-tile that are output pixels (128, or bw*bh*bn of a smaller conv patch)
     int out_mode;    // coordinates of the output map: 0 (c, row, 0)  1 (c, pixel in image, image)  2 (c, x, image row)
     int par_all;     // the constants of every channel are resident (loaded once); else reloaded per N tile
@@ -356,9 +355,7 @@ __device__ __forceinline__ uint32_t padding_taps(const GemmArgs& g, int mt, int 
 }
 
 // MODE: 0 fast epilogue, 1 fast epilogue with the bias folded into the FMA (int8 only), 2 exact epilogue.
-// CS: 16-column chunks per store group (1, 2, 4 or 8).  Compile-time so that each kernel carries exactly one epilogue body.
-// CS == 8: a group is 32 rows x 128 bytes filled by a PAIR of warps (64 bytes each) and stored by one of them: the TMA
-// unit's cost is per row (~4 cycles for anything up to 128 bytes), so 128-byte rows halve the store side's share of it.
+// CS: 16-column chunks per store group (1 or 2).  Compile-time so that each kernel carries exactly one epilogue body.
 template <bool U8, int MODE, int CS, bool BORDER>
 __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
     gemm_i8_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
@@ -369,19 +366,18 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
     // operand ring first (1024-byte aligned for the 128B swizzle), then the per-warp output staging buffers (1024-byte
     // aligned: their TMA swizzle pattern is a function of the address), the control block and the epilogue constants
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    const uint32_t a_bytes = BLOCK_M * g.block_k, b_bytes = g.bnx * g.block_k;
+    const uint32_t a_bytes = BLOCK_M * g.block_k, b_bytes = g.block_n * g.block_k;
     const uint32_t b_al = (b_bytes + 1023) & ~1023u;
     const uint32_t stage_bytes = a_bytes + (g.b_res ? 0u : b_al);
     uint8_t* b_region = smem + (size_t)g.stages * stage_bytes; // resident-B mode: [k_blocks][b_al]
     constexpr uint32_t buf_bytes = 512u * CS; // 32 rows x 16*CS bytes
-    constexpr int WCH = CS == 8 ? 4 : CS;     // chunks one warp requantises per group
     uint8_t* sxs = b_region + (g.b_res ? (size_t)g.k_blocks * b_al : 0); // uint8: sum(x) of the rows, [2 accumulator stages][4 m-tiles][128] int32
     uint8_t* stg = sxs + (g.cplane ? 4096u : 0u);
     const uint32_t sx_base = smem_u32(sxs);
     const uint32_t stg_base = smem_u32(stg);
-    GemmSmemCtl* ctl = reinterpret_cast<GemmSmemCtl*>(stg + (size_t)(CS == 8 ? EPI_WARPS / 2 : EPI_WARPS) * 2 * buf_bytes);
+    GemmSmemCtl* ctl = reinterpret_cast<GemmSmemCtl*>(stg + (size_t)EPI_WARPS * 2 * buf_bytes);
     const uint32_t par_base = smem_u32(ctl) + (uint32_t)sizeof(GemmSmemCtl); // [par channels] x 8 bytes (see FastPar4)
-    const int acc_cols = g.mt * g.tcols; // accumulator image columns of one stage
+    const int acc_cols = g.mt * g.block_n; // accumulator image columns of one stage
     const uint32_t img_pitch = acc_pitch(acc_cols);
     const uint32_t img_base = (par_base + (uint32_t)(g.par_all ? g.n_tiles * g.block_n : g.block_n) * 8u + 15u) & ~15u;
 
@@ -399,7 +395,7 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
 
     if (threadIdx.x == 0)
     {
-        const uint32_t sumw = (U8 && g.sx_mode == 3) ? SUM_WARPS : 0; // the row-sum warps read every operand stage and publish with the accumulators
+        const uint32_t sumw = (U8 && g.cplane) ? SUM_WARPS : 0; // the row-sum warps read every operand stage and publish with the accumulators
         for (int s = 0; s < g.stages; s++) mbar_init(&ctl->full[s], 1), mbar_init(&ctl->empty[s], EPI_WARPS + sumw);
         for (int s = 0; s < 2; s++) mbar_init(&ctl->sx_full[s], sumw ? sumw : 1), mbar_init(&ctl->sx_empty[s], EPI_WARPS);
         mbar_init(&ctl->b_full, 1);
@@ -421,7 +417,7 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
             {
                 // the grid is a multiple of n_tiles, so this CTA only ever sees N tile blockIdx.x % n_tiles: load its
                 // weights (every k-block) once
-                const int nb = (blockIdx.x % g.n_tiles) * g.bnx;
+                const int nb = (blockIdx.x % g.n_tiles) * g.block_n;
                 mbar_expect_tx(&ctl->b_full, (uint32_t)g.k_blocks * b_bytes);
                 for (int kb = 0; kb < g.k_blocks; kb++)
                 {
@@ -434,7 +430,7 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
                 const int msup = st / g.n_tiles;
                 const int mt0 = msup * g.mt;
                 const int ntile = st - msup * g.n_tiles;
-                const int n0 = ntile * g.bnx; // row of this N tile in the packed weight matrix
+                const int n0 = ntile * g.block_n; // row of this N tile in the packed weight matrix
                 for (int i = 0; i < g.mt && mt0 + i < g.m_tiles; i++)
                 {
                     const int m0 = (mt0 + i) * BLOCK_M;
@@ -477,7 +473,7 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
         // lane), reads them with 16-byte loads (chunk order rotated per lane so that a quarter-warp covers all banks), dp4a against
         // 0x01010101, and publishes the sums through shared memory together with the accumulator stage.  This keeps the uint8 tiling
         // identical to the int8 one: no extra B rows, no extra accumulator columns, no second MMA.
-        if (g.sx_mode == 3)
+        if (g.cplane)
         {
             const int sw = warp - SUM_WARP0;
             const int cpr = g.block_k >> 4;                  // 16-byte chunks per row: 2, 4 or 8
@@ -532,25 +528,19 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
         const int sub = warp >> 2;
         const int ngroups = g.ngroups;
         // MMA share of this warpgroup (= sub): rows 64*mh.., chunks [c_lo, c_lo + c_n) of every B tile
-        const int mh = sub & 1, nch = g.tcols >> 4, chalf = (nch + 1) >> 1;
+        const int mh = sub & 1, nch = g.block_n >> 4, chalf = (nch + 1) >> 1;
         const int c_lo = (sub >> 1) ? chalf : 0, c_n = (sub >> 1) ? nch - chalf : chalf;
-        const uint32_t a_bytes_mma = BLOCK_M * g.block_k, b_al_mma = (g.bnx * g.block_k + 1023) & ~1023u;
+        const uint32_t a_bytes_mma = BLOCK_M * g.block_k, b_al_mma = (g.block_n * g.block_k + 1023) & ~1023u;
         int stage = 0;
         uint32_t phase = 0;
         if (g.b_res) mbar_wait(&ctl->b_full, 0);
         int qrows = g.rows_valid - q * 32; // rows of this quarter that are output pixels
         qrows = qrows < 0 ? 0 : (qrows > 32 ? 32 : qrows);
         const CUtensorMap* tm_out = (qrows == 32) ? &tmap_out : &tmap_out_tail;
-        const int half = CS == 8 ? (sub & 1) : 0;        // which 64-byte half of the pair's 128-byte rows this warp fills
-        const int pair = q * 2 + (sub >> 1);             // CS == 8: staging buffers and the named barrier are per pair
-        const uint32_t buf0 = stg_base + (uint32_t)(CS == 8 ? pair : warp) * 2u * buf_bytes;
-        // swizzle of the staging buffer = the output map's swizzle: 16-byte chunk index ^= row bits (Swizzle<1|2|3,4,3>)
-        const uint32_t xl = CS == 8   ? (uint32_t)(lane & 7) << 4
-                            : CS == 4 ? (uint32_t)((lane >> 1) & 3) << 4
-                                      : (CS == 2 ? (uint32_t)((lane >> 2) & 1) << 4 : 0u);
+        const uint32_t buf0 = stg_base + (uint32_t)warp * 2u * buf_bytes;
+        // swizzle of the staging buffer = the output map's swizzle: 16-byte chunk index ^= row bit 2 (Swizzle<1,4,3>, CS 2 only)
+        const uint32_t xl = CS == 2 ? (uint32_t)((lane >> 2) & 1) << 4 : 0u;
         const uint32_t row_off = (uint32_t)lane * 16u * CS;
-        const int gfirst = CS == 8 ? (sub >> 1) : sub, gstep = CS == 8 ? 2 : 4;
-        auto pair_sync = [&]() { asm volatile("bar.sync %0, 64;" ::"r"(2 + pair) : "memory"); };
         uint32_t ucount = 0; // groups this warp has stored (buffer parity)
         const int par_ch = g.n_tiles * g.block_n;
         const bool fast = MODE != 2;
@@ -615,29 +605,28 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
                 }
 #pragma unroll
                 for (int j = 0; j < MMA_CHUNKS; j++)
-                    if (j < c_n) frag_to_image(acc[j], img_base, img_pitch, mh * 64, i * g.tcols + (c_lo + j) * 16);
+                    if (j < c_n) frag_to_image(acc[j], img_base, img_pitch, mh * 64, i * g.block_n + (c_lo + j) * 16);
             }
             epilogue_bar_sync(); // the image is complete
-            if (U8 && g.sx_mode == 3) mbar_wait(&ctl->sx_full[as], aphase); // the row sums of this stage
+            if (U8 && g.cplane) mbar_wait(&ctl->sx_full[as], aphase); // the row sums of this stage
             TLOG_E(0);
             const uint32_t tbase = img_base + (uint32_t)(q * 32 + lane) * img_pitch;
             if (qrows > 0)
             {
                 // groups of this warp: flattened index u = i * ngroups + grp, u = sub, sub + 4, ...
                 uint32_t v0[16], v1[16];
-                int i = 0, grp = gfirst;
+                int i = 0, grp = sub;
                 while (grp >= ngroups) grp -= ngroups, i++;
                 if (CS > 1 && i < mtc)
-                    acc_ld16(tbase + 4u * (i * g.tcols + grp * (CS * 16) + half * 64), reinterpret_cast<uint32_t(&)[16]>(v0));
+                    acc_ld16(tbase + 4u * (i * g.block_n + grp * (CS * 16)), reinterpret_cast<uint32_t(&)[16]>(v0));
                 while (i < mtc)
                 {
-                    int i2 = i, g2 = grp + gstep; // the group after this one
+                    int i2 = i, g2 = grp + 4; // the group after this one
                     while (g2 >= ngroups) g2 -= ngroups, i2++;
                     const uint32_t buf = buf0 + (ucount & 1u) * buf_bytes;
                     // the store issued two groups ago has finished reading this buffer
-                    if (lane == 0 && half == 0) bulk_wait_read<1>();
-                    if (CS == 8) pair_sync();
-                    else __syncwarp();
+                    if (lane == 0) bulk_wait_read<1>();
+                    __syncwarp();
                     uint32_t pad = 0;
                     int32_t rowc = 0;
                     if (U8)
@@ -645,24 +634,19 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
                         // the pixel's sum(x), once per group
                         if (g.cplane)
                         {
-                            if (g.sx_mode == 3)
-                            {
-                                int32_t sx;
-                                asm volatile("ld.shared.b32 %0, [%1];" : "=r"(sx) : "r"(sx_base + (uint32_t)(((as * 4 + i) * 128 + q * 32 + lane) * 4)));
-                                rowc = g.cplane * sx;
-                            }
-                            else
-                                rowc = g.cplane * (int32_t)acc_ld1(tbase + 4u * (i * g.tcols + g.block_n)); // the column of the ones rows in B
+                            int32_t sx;
+                            asm volatile("ld.shared.b32 %0, [%1];" : "=r"(sx) : "r"(sx_base + (uint32_t)(((as * 4 + i) * 128 + q * 32 + lane) * 4)));
+                            rowc = g.cplane * sx;
                         }
                         if (BORDER) pad = padding_taps(g, mt0 + i, q * 32 + lane);
                     }
-                    const uint32_t tg = tbase + 4u * (i * g.tcols + grp * (CS * 16) + half * 64);
+                    const uint32_t tg = tbase + 4u * (i * g.block_n + grp * (CS * 16));
                     const int cg0 = grp * (CS * 16); // first column of the group inside the N tile
                     const uint32_t sdst = buf + row_off;
                     auto unit = [&](const uint32_t (&v)[16], int k)
                     {
-                        const int c = cg0 + half * 64 + k * 16;
-                        const uint32_t dst = sdst + (((uint32_t)(half * 4 + k) << 4) ^ xl);
+                        const int c = cg0 + k * 16;
+                        const uint32_t dst = sdst + (((uint32_t)k << 4) ^ xl);
                         if (U8) epilogue_unit_u8<MODE == 2, BORDER>(v, rowc, pad, g, par_s + c * 8, dst, n0 + c, (uint32_t)(mt0 + i), e);
                         else if (MODE == 2) epilogue_unit_exact(v, dst, n0 + c, g.oc, e);
                         else epilogue_unit_fast<MODE == 1>(v, par_s + c * 8, dst, n0 + c, (uint32_t)(mt0 + i), e);
@@ -675,20 +659,19 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
                     else
                     {
 #pragma unroll
-                        for (int k = 0; k < WCH; k++)
+                        for (int k = 0; k < CS; k++)
                         {
                             TLOG_E(3);
                             // the next chunk's accumulators are in flight while this one is requantised
-                            if (k + 1 < WCH) acc_ld16(tg + (k + 1) * 64, reinterpret_cast<uint32_t(&)[16]>(*((k & 1) ? v0 : v1)));
-                            else if (i2 < mtc) acc_ld16(tbase + 4u * (i2 * g.tcols + g2 * (CS * 16) + half * 64), reinterpret_cast<uint32_t(&)[16]>(v0));
+                            if (k + 1 < CS) acc_ld16(tg + (k + 1) * 64, reinterpret_cast<uint32_t(&)[16]>(*((k & 1) ? v0 : v1)));
+                            else if (i2 < mtc) acc_ld16(tbase + 4u * (i2 * g.block_n + g2 * (CS * 16)), reinterpret_cast<uint32_t(&)[16]>(v0));
                             unit(reinterpret_cast<const uint32_t(&)[16]>(*((k & 1) ? v1 : v0)), k);
                             TLOG_E(4);
                         }
                     }
                     fence_proxy_async_smem(); // generic-proxy writes -> visible to the TMA unit
-                    if (CS == 8) pair_sync();
-                    else __syncwarp();
-                    if (lane == 0 && half == 0)
+                    __syncwarp();
+                    if (lane == 0)
                     {
                         int x1, x2 = 0;
                         if (!g.conv)
@@ -722,101 +705,6 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
             epilogue_bar_sync();
             fixq_drain<U8>(g, e);
         }
-    }
-}
-
-// ---- small-K pointwise GEMM: many small CTAs instead of one warp-specialised persistent CTA ---------------------------
-// For K <= 256 (the first pointwise layers: K = 32..128, one or two k-blocks) the persistent kernel above spends more
-// time in hand-overs between its roles than in work (timeline: the epilogue warps idle ~50% of the time).  Here a CTA is
-// one warpgroup; it keeps the N tile's weights in shared memory, double-buffers the A tile (TMA), and per m-tile does:
-// wait A -> the warpgroup's MMAs into the accumulator image -> everybody requantises its own accumulator row and writes its
-// bn contiguous output bytes straight to global memory.  There is no pipelining inside a CTA beyond the A prefetch; several
-// CTAs are resident per SM (bounded by shared memory) and overlap each other, as in the window kernel (conv_window.cu).
-struct SimpleArgs
-{
-    uint8_t* out;
-    long long m;
-    int m_tiles, n_tiles, k_blocks, block_n, block_k, swizzle, ocp, oc, ldo;
-};
-
-template <int MODE> // 0 fast, 1 fast + fused bias, 2 exact
-__global__ void __launch_bounds__(128) gemm_simple_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                                                           const SimpleArgs g, const __grid_constant__ EpiParams e)
-{
-    extern __shared__ __align__(1024) uint8_t simple_smem[];
-    uint8_t* sm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(simple_smem) + 1023) & ~(uintptr_t)1023);
-    const uint32_t a_bytes = BLOCK_M * g.block_k, b_bytes = g.block_n * g.block_k, b_al = (b_bytes + 1023) & ~1023u;
-    uint8_t* sA = sm;                                               // [2][k_blocks][a_bytes]
-    uint8_t* sB = sA + 2u * (size_t)g.k_blocks * a_bytes;           // [k_blocks][b_al]
-    const uint32_t sPar = smem_u32(sB) + (uint32_t)g.k_blocks * b_al; // [block_n] x 8 bytes
-    const uint32_t pitch = acc_pitch(g.block_n), sImg = sPar + (uint32_t)g.block_n * 8u; // accumulator image [128][pitch]
-    __shared__ __align__(8) uint64_t a_full[2], b_full;
-    const int tid = threadIdx.x;
-    const int ntile = blockIdx.x % g.n_tiles, n0 = ntile * g.block_n;
-    const int mfirst = blockIdx.x / g.n_tiles, mstep = gridDim.x / g.n_tiles; // the grid is a multiple of n_tiles
-
-    if (tid == 0)
-    {
-        mbar_init(&a_full[0], 1), mbar_init(&a_full[1], 1), mbar_init(&b_full, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    if (tid == 0)
-    {
-        mbar_expect_tx(&b_full, (uint32_t)g.k_blocks * b_bytes);
-        for (int kb = 0; kb < g.k_blocks; kb++) tma_load_2d(&tmap_b, &b_full, sB + (size_t)kb * b_al, kb * g.block_k, n0);
-        if (mfirst < g.m_tiles)
-        {
-            mbar_expect_tx(&a_full[0], (uint32_t)g.k_blocks * a_bytes);
-            for (int kb = 0; kb < g.k_blocks; kb++) tma_load_2d(&tmap_a, &a_full[0], sA + (size_t)kb * a_bytes, kb * g.block_k, mfirst * BLOCK_M);
-        }
-    }
-    for (int c = tid; c < g.block_n; c += 128)
-        sts_f2(sPar + c * 8, (MODE != 2 && n0 + c < g.ocp) ? __ldg(e.fast_par + n0 + c) : make_float2(0.f, 0.f));
-    __syncthreads();
-    const uint32_t tb = sImg + (uint32_t)tid * pitch;
-
-    uint32_t it = 0;
-    for (int mt = mfirst; mt < g.m_tiles; mt += mstep, it++)
-    {
-        const int buf = it & 1;
-        // the other buffer was read by the MMAs of the previous tile, which have completed: prefetch the next tile
-        if (tid == 0 && mt + mstep < g.m_tiles)
-        {
-            mbar_expect_tx(&a_full[buf ^ 1], (uint32_t)g.k_blocks * a_bytes);
-            for (int kb = 0; kb < g.k_blocks; kb++)
-                tma_load_2d(&tmap_a, &a_full[buf ^ 1], sA + ((size_t)(buf ^ 1) * g.k_blocks + kb) * a_bytes, kb * g.block_k, (mt + mstep) * BLOCK_M);
-        }
-        if (it == 0) mbar_wait(&b_full, 0);
-        mbar_wait(&a_full[buf], (it >> 1) & 1);
-        wg_mma_to_image<false, false>(smem_u32(sA + (size_t)buf * g.k_blocks * a_bytes), a_bytes, smem_u32(sB), b_al, g.k_blocks, g.swizzle,
-                                      g.block_n, sImg, pitch);
-        __syncthreads();
-
-        // ---- epilogue: thread = output row, 16 channels per load, straight to global memory ----
-        const long long row = (long long)mt * BLOCK_M + tid;
-        uint8_t* op = g.out + (size_t)(row < g.m ? row : 0) * g.ldo + n0;
-        uint32_t v0[16], v1[16];
-        acc_ld16(tb, v0);
-        const int nch = g.block_n >> 4;
-        for (int c = 0; c < nch; c += 2)
-        {
-            if (c + 1 < nch) acc_ld16(tb + (c + 1) * 64, v1);
-            {
-                uint32_t w[4];
-                tc_unit16<MODE, false>(v0, 0, sPar + c * 128, n0 + c * 16, g.oc, e, w);
-                if (row < g.m && n0 + c * 16 < g.ocp) *reinterpret_cast<uint4*>(op + c * 16) = make_uint4(w[0], w[1], w[2], w[3]);
-            }
-            if (c + 1 >= nch) break;
-            if (c + 2 < nch) acc_ld16(tb + (c + 2) * 64, v0);
-            {
-                uint32_t w[4];
-                tc_unit16<MODE, false>(v1, 0, sPar + (c + 1) * 128, n0 + (c + 1) * 16, g.oc, e, w);
-                if (row < g.m && n0 + (c + 1) * 16 < g.ocp) *reinterpret_cast<uint4*>(op + (c + 1) * 16) = make_uint4(w[0], w[1], w[2], w[3]);
-            }
-        }
-        // the next tile's MMAs overwrite the accumulator image
-        __syncthreads();
     }
 }
 
@@ -926,62 +814,41 @@ static int encode_2d(void* tmap, const void* base, uint64_t inner, uint64_t rows
     return tmap_encode(tmap, base, 2, dims, strides, box, nullptr, swizzle);
 }
 
-// Where the uint8 path's sum(x) comes from (TB200_U8_SX, A/B switch): 3 (default) = two extra warps add up the rows of the A tiles,
-// 0 = 16 rows of ones in every B tile (sum(x) is then a 17th..32nd accumulator column; costs image columns and m-tiles per stage).
 bool debug_launch()
 {
     static const bool on = getenv("TB200_DEBUG_LAUNCH") != nullptr;
     return on;
 }
 
-int gemm_sx_mode()
+int gemm_block_n(int ocp)
 {
-    static const int mode = [] { const char* e = getenv("TB200_U8_SX"); return (e && atoi(e) == 0) ? 0 : 3; }();
-    return mode;
-}
-
-// rows of one packed B tile: block_n, + 16 rows of ones for uint8 layers with a weight zero point (u8 = 1 + zero point) in mode 0
-int gemm_tile_rows(int ocp, int u8) { return gemm_block_n(ocp, u8) + ((u8 > 1 && gemm_sx_mode() == 0) ? 16 : 0); }
-
-int gemm_block_n(int ocp, int u8)
-{
-    // N tiles of at most 128 channels (+ 16 ones rows in mode 0): the accumulator image of a stage shares shared memory with
-    // the operand ring; the channels are dealt evenly to the fewest such tiles
-    (void)u8;
+    // N tiles of at most 128 channels: the accumulator image of a stage shares shared memory with the operand ring; the
+    // channels are dealt evenly to the fewest such tiles
     const int nt = (ocp + 127) / 128;
     return ((ocp + nt - 1) / nt + 15) & ~15;
 }
 
-// Store-group width and output tensor maps.  A group is 32 rows x 16*cs channels; cs is the largest of 4 / 2 / 1 that
-// divides the N tile's chunk count and deals the stage's groups evenly to the four warps of a 32-row image quarter.
-static void plan_store_groups(GemmPlan* p)
+// m-tiles per accumulator stage and the store-group width.  Several m-tiles share a stage when the CTA stays on one N tile
+// anyway (a single N tile): that amortises the per-stage synchronisation over up to ACC_COLS_MAX image columns of work.  A
+// store group is 32 rows x 16*cs channels; cs is 2 when that divides the N tile's chunk count and deals the stage's groups
+// evenly to the four warps of a 32-row image quarter, else 1.
+static void plan_stage(GemmPlan* p)
 {
+    p->mt = 1;
+    if (p->n_tiles == 1)
+        while (p->mt < 4 && (p->mt * 2) * p->block_n <= ACC_COLS_MAX && p->mt * 2 <= p->m_tiles) p->mt *= 2;
     const int nch = p->block_n / 16;
-    int cs = 1;
-    for (int c = 4; c >= 1; c >>= 1)
-        if (nch % c == 0 && ((p->mt * (nch / c)) % 4 == 0 || c == 1))
-        {
-            cs = c;
-            break;
-        }
-    // 128-byte rows filled by warp pairs when the stage deals an even number of 128-column groups to each quarter
-    // (measured on MobileNet-v1, batch 256: the pair hand-over costs more than the halved row count saves -- 0.75 ms vs
-    //  0.68 ms for all GEMMs -- so this mode is opt-in)
-    if (nch % 8 == 0 && (p->mt * (nch / 8)) % 2 == 0 && getenv("TB200_GEMM_PAIR")) cs = 8;
-    if (const char* ev = getenv("TB200_GEMM_STORE_CS"))
-    {
-        const int f = atoi(ev);
-        if ((f == 1 || f == 2 || f == 4) && nch % f == 0) cs = f;
-    }
-    p->cs = cs, p->ngroups = nch / cs;
+    p->cs = (nch % 2 == 0 && (p->mt * (nch / 2)) % 4 == 0) ? 2 : 1;
+    p->ngroups = nch / p->cs;
 }
 
+// Output tensor maps: a box of 32 rows x one store group; 32-byte groups are swizzled like the warp's staging buffer.
 static int plan_epilogue(GemmPlan* p, const void* out, uint64_t d1, uint64_t d2)
 {
     const int cs = p->cs;
     const uint64_t dims[3] = {(uint64_t)p->ocp, d1, d2};
     const uint64_t strides[2] = {(uint64_t)p->ldo, (uint64_t)p->ldo * d1};
-    const int swz = cs == 8 ? 128 : (cs == 4 ? 64 : (cs == 2 ? 32 : 0));
+    const int swz = cs == 2 ? 32 : 0;
     const uint32_t box[3] = {(uint32_t)(16 * cs), 32u, 1u};
     int rc = tmap_encode(p->tmap_out, out, 3, dims, strides, box, nullptr, swz);
     if (rc) return rc;
@@ -994,8 +861,8 @@ static int plan_epilogue(GemmPlan* p, const void* out, uint64_t d1, uint64_t d2)
 static int epilogue_smem_bytes(const GemmPlan* p)
 {
     const int par_ch = p->n_tiles * p->block_n;
-    return EPI_WARPS * 2 * 512 * (p->cs == 8 ? 4 : p->cs) + (par_ch <= PAR_MAX ? par_ch : p->block_n) * 8 + (int)sizeof(GemmSmemCtl) + 2048 +
-           128 * (int)acc_pitch(p->mt * p->bnx) + 16;
+    return EPI_WARPS * 2 * 512 * p->cs + (par_ch <= PAR_MAX ? par_ch : p->block_n) * 8 + (int)sizeof(GemmSmemCtl) + 2048 +
+           128 * (int)acc_pitch(p->mt * p->block_n) + 16;
 }
 
 // Operand ring depth and the resident-B decision.  With the N tile's weights resident the ring carries A tiles only,
@@ -1003,9 +870,9 @@ static int epilogue_smem_bytes(const GemmPlan* p)
 // of prefetch distance.
 static int plan_ring(GemmPlan* p)
 {
-    const int a_bytes = BLOCK_M * p->block_k, b_al = (p->bnx * p->block_k + 1023) & ~1023;
+    const int a_bytes = BLOCK_M * p->block_k, b_al = (p->block_n * p->block_k + 1023) & ~1023;
     const int budget = 224 * 1024 - epilogue_smem_bytes(p) - (p->cplane ? 4096 : 0);
-    p->b_res = ((long long)p->k_blocks * b_al <= B_RESIDENT_MAX && !getenv("TB200_GEMM_NO_BRES")) ? 1 : 0;
+    p->b_res = (long long)p->k_blocks * b_al <= B_RESIDENT_MAX ? 1 : 0;
     int stages = p->b_res ? (budget - p->k_blocks * b_al) / a_bytes : budget / (a_bytes + b_al);
     if (p->b_res && stages < 3) p->b_res = 0, stages = budget / (a_bytes + b_al);
     if (stages > MAX_STAGES) stages = MAX_STAGES;
@@ -1014,55 +881,30 @@ static int plan_ring(GemmPlan* p)
     return 0;
 }
 
-int gemm_plan_create(GemmPlan* p, const void* a, long long lda, const void* b, void* out, long long m, int k, int oc, int ocp, int ldo,
-                     int variant, int u8)
+int gemm_plan_create(GemmPlan* p, const void* a, long long lda, const void* b, void* out, long long m, int k, int oc, int ocp, int ldo, int u8)
 {
     if (m <= 0 || k <= 0 || (k & 15) || (ocp & 15) || (lda & 15) || (ldo & 15)) return TB200_ERR_INVALID;
     memset(p, 0, sizeof *p);
-    p->m = m, p->k = k, p->oc = oc, p->ocp = ocp, p->ldo = ldo, p->variant = variant, p->out = out;
+    p->m = m, p->k = k, p->oc = oc, p->ocp = ocp, p->ldo = ldo, p->out = out;
     p->block_k = k <= 32 ? 32 : (k <= 64 ? 64 : 128);
     p->swizzle = p->block_k;
     p->k_blocks = (k + p->block_k - 1) / p->block_k;
     p->u8 = u8 != 0; // u8 = 1 + weight zero point for uint8 layers
     p->b_signed = !p->u8 || u8 != 1;
     p->cplane = (p->u8 && u8 != 1 && !getenv("TB200_DEBUG_NO_CPLANE")) ? 128 - (u8 - 1) : 0; // (debug switch: WRONG results, timing experiments only)
-    p->block_n = gemm_block_n(ocp, u8);
-    p->bnx = gemm_tile_rows(ocp, u8);
+    p->block_n = gemm_block_n(ocp);
     p->taps = 1;
     p->n_tiles = (ocp + p->block_n - 1) / p->block_n;
     p->m_tiles = (m + BLOCK_M - 1) / BLOCK_M;
-    // m-tiles per accumulator stage: amortise the per-stage synchronisation over up to ACC_COLS_MAX image columns of work
-    p->mt = 1;
-    {
-        // several m-tiles per stage when the CTA stays on one N tile anyway (single tile, or resident weights)
-        const bool resident = (long long)p->k_blocks * ((p->bnx * p->block_k + 1023) & ~1023) <= B_RESIDENT_MAX;
-        if (p->n_tiles == 1 || (resident && getenv("TB200_GEMM_PAIR")))
-            while (p->mt < 4 && (p->mt * 2) * p->bnx <= ACC_COLS_MAX && (long long)(p->mt * 2) * 132 <= p->m_tiles * (p->n_tiles == 1 ? 132 : 1)) p->mt *= 2;
-    }
-    plan_store_groups(p);
+    plan_stage(p);
     int rc = plan_ring(p);
     if (rc) return rc;
     rc = encode_2d(p->tmap_a, a, (uint64_t)k, (uint64_t)m, (uint64_t)lda, p->block_k, BLOCK_M, p->swizzle);
     if (rc) return rc;
-    rc = encode_2d(p->tmap_b, b, (uint64_t)k, (uint64_t)p->n_tiles * p->bnx, (uint64_t)k, p->block_k, p->bnx, p->swizzle);
+    rc = encode_2d(p->tmap_b, b, (uint64_t)k, (uint64_t)p->n_tiles * p->block_n, (uint64_t)k, p->block_k, p->block_n, p->swizzle);
     if (rc) return rc;
     p->rows_valid = BLOCK_M, p->out_mode = 0;
-    rc = plan_epilogue(p, out, (uint64_t)m, 1);
-    if (rc) return rc;
-    // small-K layers: the many-small-CTAs kernel (gemm_simple_kernel), N tiles of at most 128 channels
-    p->simple = 0;
-    static const int maxk = getenv("TB200_GEMM_SIMPLE_MAXK") ? atoi(getenv("TB200_GEMM_SIMPLE_MAXK")) : 256;
-    // Opt-in (TB200_GEMM_SIMPLE=1): the cross-check implementation of the same contraction.
-    if (!u8 && k <= maxk && getenv("TB200_GEMM_SIMPLE"))
-    {
-        const int bn = ocp <= 128 ? ocp : 128;
-        const int a_bytes = BLOCK_M * p->block_k, b_al = (bn * p->block_k + 1023) & ~1023;
-        const int smem = p->k_blocks * (2 * a_bytes + b_al) + bn * 8 + 128 * (int)acc_pitch(bn) + 2048;
-        if (smem <= 200 * 1024 &&
-            encode_2d(p->tmap_b_s, b, (uint64_t)k, (uint64_t)ocp, (uint64_t)k, p->block_k, bn, p->swizzle) == 0)
-            p->simple = 1, p->s_block_n = bn, p->s_n_tiles = (ocp + bn - 1) / bn, p->s_smem = smem, p->out = out;
-    }
-    return 0;
+    return plan_epilogue(p, out, (uint64_t)m, 1);
 }
 
 // Implicit-GEMM plan for a dense (group 1, dilation 1) convolution with any kernel size and stride 1 or 2:
@@ -1074,7 +916,7 @@ int gemm_plan_create_conv(GemmPlan* p, const void* in, const void* w, void* out,
     if (taps > 1 && (s.cp % 32)) return TB200_ERR_UNSUPPORTED; // a k-block must not straddle two taps
     memset(p, 0, sizeof *p);
     p->conv = 1;
-    p->m = (long long)s.n * s.oh * s.ow, p->oc = s.oc, p->ocp = s.ocp, p->ldo = s.ocp, p->variant = 0, p->out = out;
+    p->m = (long long)s.n * s.oh * s.ow, p->oc = s.oc, p->ocp = s.ocp, p->ldo = s.ocp, p->out = out;
     if (taps == 1) p->block_k = s.cp <= 32 ? 32 : (s.cp <= 64 ? 64 : 128);
     else p->block_k = (s.cp % 128 == 0) ? 128 : ((s.cp % 64 == 0) ? 64 : 32);
     p->swizzle = p->block_k;
@@ -1084,8 +926,7 @@ int gemm_plan_create_conv(GemmPlan* p, const void* in, const void* w, void* out,
     p->u8 = u8 != 0; // u8 = 1 + weight zero point for uint8 layers
     p->b_signed = !p->u8 || u8 != 1;
     p->cplane = (p->u8 && u8 != 1 && !getenv("TB200_DEBUG_NO_CPLANE")) ? 128 - (u8 - 1) : 0; // (debug switch: WRONG results, timing experiments only)
-    p->block_n = gemm_block_n(s.ocp, u8);
-    p->bnx = gemm_tile_rows(s.ocp, u8);
+    p->block_n = gemm_block_n(s.ocp);
     p->taps = taps, p->in_h = s.h, p->in_w = s.w;
     if (taps > 64) return TB200_ERR_UNSUPPORTED;
     p->n_tiles = (s.ocp + p->block_n - 1) / p->block_n;
@@ -1106,14 +947,7 @@ int gemm_plan_create_conv(GemmPlan* p, const void* in, const void* w, void* out,
     p->m_tiles = (long long)p->tiles_w * p->tiles_h * tiles_n;
     p->kw_n = s.kw, p->pad_h = s.ph0, p->pad_w = s.pw0, p->cstride = s.sh, p->cp = s.cp, p->oh = s.oh, p->ow = s.ow, p->nimg = s.n;
     p->a_tx_bytes = (uint32_t)(p->block_k * p->bw * p->bh * p->bn);
-    p->mt = 1;
-    {
-        // several m-tiles per stage when the CTA stays on one N tile anyway (single tile, or resident weights)
-        const bool resident = (long long)p->k_blocks * ((p->bnx * p->block_k + 1023) & ~1023) <= B_RESIDENT_MAX;
-        if (p->n_tiles == 1 || (resident && getenv("TB200_GEMM_PAIR")))
-            while (p->mt < 4 && (p->mt * 2) * p->bnx <= ACC_COLS_MAX && (long long)(p->mt * 2) * 132 <= p->m_tiles * (p->n_tiles == 1 ? 132 : 1)) p->mt *= 2;
-    }
-    plan_store_groups(p);
+    plan_stage(p);
     int rc = plan_ring(p);
     if (rc) return rc;
     const uint64_t dims[4] = {(uint64_t)s.cp, (uint64_t)s.w, (uint64_t)s.h, (uint64_t)s.n};
@@ -1123,7 +957,7 @@ int gemm_plan_create_conv(GemmPlan* p, const void* in, const void* w, void* out,
     if (box[1] > 256 || box[2] > 256 || box[3] > 256) return TB200_ERR_UNSUPPORTED;
     rc = tmap_encode(p->tmap_a, in, 4, dims, strides, box, estr, p->swizzle);
     if (rc) return rc;
-    rc = encode_2d(p->tmap_b, w, (uint64_t)p->k, (uint64_t)p->n_tiles * p->bnx, (uint64_t)p->k, p->block_k, p->bnx, p->swizzle);
+    rc = encode_2d(p->tmap_b, w, (uint64_t)p->k, (uint64_t)p->n_tiles * p->block_n, (uint64_t)p->k, p->block_k, p->block_n, p->swizzle);
     if (rc) return rc;
     // The rows of an m-tile are consecutive output pixels along one axis of the NHWC output (see the patch shapes above):
     //   bn > 1 (whole images)   : rows = pixels of bn consecutive images        -> map (C, N*OH*OW, 1), clipped at the end
@@ -1169,53 +1003,16 @@ static void gemm_trace_report(const GemmPlan& p, const GemmArgs& g, int grid, cu
         }
 }
 
-static cudaError_t launch_gemm_simple(const GemmPlan& p, const EpiParams& e, int num_sms, cudaStream_t st)
-{
-    SimpleArgs g;
-    g.out = (uint8_t*)p.out, g.m = p.m, g.m_tiles = (int)p.m_tiles, g.n_tiles = p.s_n_tiles, g.k_blocks = p.k_blocks, g.block_n = p.s_block_n;
-    g.block_k = p.block_k, g.swizzle = p.swizzle, g.ocp = p.ocp, g.oc = p.oc, g.ldo = p.ldo;
-    int per_sm = (220 * 1024) / (p.s_smem + 1024);
-    if (per_sm > 16) per_sm = 16;
-    if (per_sm < 1) per_sm = 1;
-    long long want = p.m_tiles * p.s_n_tiles, cap = (long long)num_sms * per_sm;
-    int grid = (int)(want < cap ? want : cap);
-    grid -= grid % p.s_n_tiles;
-    if (grid < p.s_n_tiles) grid = p.s_n_tiles;
-    CUtensorMap ta, tb;
-    memcpy(&ta, p.tmap_a, sizeof ta);
-    memcpy(&tb, p.tmap_b_s, sizeof tb);
-    const int mode = !e.fast_ok ? 2 : (e.fuse_bias ? 1 : 0);
-    const size_t smem = (size_t)p.s_smem;
-#define TB200_SIMPLE_CASE(MD)                                                                                                  \
-    if (mode == MD)                                                                                                            \
-    {                                                                                                                          \
-        /* the opt-in is per device AND per context: set it before every launch (launches happen at graph capture only) */ \
-        {                                                                                                                      \
-            cudaError_t err = cudaFuncSetAttribute(gemm_simple_kernel<MD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-            if (err != cudaSuccess) return err;                                                                                \
-        }                                                                                                                      \
-        if (debug_launch()) fprintf(stderr, "tengine_b200: launch gemm_simple_kernel<MODE=%d>\n", MD);                          \
-        gemm_simple_kernel<MD><<<grid, 128, smem, st>>>(ta, tb, g, e);                                                         \
-        return cudaGetLastError();                                                                                             \
-    }
-    TB200_SIMPLE_CASE(0) TB200_SIMPLE_CASE(1) TB200_SIMPLE_CASE(2)
-#undef TB200_SIMPLE_CASE
-    return cudaErrorInvalidValue;
-}
-
 cudaError_t launch_gemm_i8(const GemmPlan& p, const EpiParams& e, const int32_t* btab, int num_sms, cudaStream_t st)
 {
-    if (p.simple) return launch_gemm_simple(p, e, num_sms, st);
     if (p.block_n <= 0 || p.mt <= 0 || p.stages <= 0 || p.cs <= 0) return cudaErrorInvalidValue; // plan was never created
     GemmArgs g;
     g.m_tiles = (int)p.m_tiles, g.k_blocks = p.k_blocks, g.n_tiles = p.n_tiles, g.block_n = p.block_n;
     g.conv = p.conv, g.cblocks = p.cblocks, g.kw_n = p.kw_n, g.pad_h = p.pad_h, g.pad_w = p.pad_w, g.cstride = p.cstride, g.cp = p.cp;
     g.bw = p.bw, g.bh = p.bh, g.bn = p.bn, g.tiles_w = p.tiles_w, g.tiles_h = p.tiles_h, g.oh = p.oh, g.ow = p.ow, g.nimg = p.nimg;
     g.a_tx_bytes = p.a_tx_bytes;
-    g.u8 = p.u8, g.bnx = p.bnx, g.taps = p.taps, g.in_h = p.in_h, g.in_w = p.in_w, g.btab = btab, g.b_signed = p.b_signed, g.cplane = p.cplane;
-    g.sx_mode = !p.cplane ? -1 : (p.bnx != p.block_n ? 0 : 3);
+    g.u8 = p.u8, g.taps = p.taps, g.in_h = p.in_h, g.in_w = p.in_w, g.btab = btab, g.b_signed = p.b_signed, g.cplane = p.cplane;
     g.fixq = (uint4*)p.fixq, g.fixq_cap = p.fixq_cap, g.out_base = (uint8_t*)p.out, g.ldo = p.ldo, g.m_rows = (int)p.m;
-    g.tcols = p.bnx;
     g.mt = p.mt;
     g.num_super = (int)(((p.m_tiles + p.mt - 1) / p.mt) * p.n_tiles);
     g.bw_rcp = p.conv ? (65536u + (uint32_t)p.bw - 1) / (uint32_t)p.bw : 0;
@@ -1224,11 +1021,11 @@ cudaError_t launch_gemm_i8(const GemmPlan& p, const EpiParams& e, const int32_t*
     g.cs = p.cs, g.ngroups = p.ngroups, g.rows_valid = p.rows_valid, g.out_mode = p.out_mode;
     const int par_ch = p.n_tiles * p.block_n;
     g.par_all = par_ch <= PAR_MAX ? 1 : 0;
-    const int a_bytes = BLOCK_M * p.block_k, b_bytes = (p.bnx * p.block_k + 1023) & ~1023;
+    const int a_bytes = BLOCK_M * p.block_k, b_bytes = (p.block_n * p.block_k + 1023) & ~1023;
     g.b_res = p.b_res;
     const size_t smem = (size_t)p.stages * (a_bytes + (p.b_res ? 0 : b_bytes)) + (p.b_res ? (size_t)p.k_blocks * b_bytes : 0) + (p.cplane ? 4096 : 0) +
-                        (size_t)EPI_WARPS * 2 * 512 * (p.cs == 8 ? 4 : p.cs) + sizeof(GemmSmemCtl) +
-                        (size_t)(g.par_all ? par_ch : p.block_n) * 8 + 16 + 128 * (size_t)acc_pitch(p.mt * g.tcols) + 1024;
+                        (size_t)EPI_WARPS * 2 * 512 * p.cs + sizeof(GemmSmemCtl) +
+                        (size_t)(g.par_all ? par_ch : p.block_n) * 8 + 16 + 128 * (size_t)acc_pitch(p.mt * p.block_n) + 1024;
     static const bool trace_on = getenv("TB200_GEMM_TRACE") != nullptr;
     const bool launch_dbg = debug_launch();
     static unsigned long long* trace_buf = nullptr;
@@ -1270,7 +1067,7 @@ cudaError_t launch_gemm_i8(const GemmPlan& p, const EpiParams& e, const int32_t*
         if (launch_dbg || err != cudaSuccess) gemm_launch_debug((const void*)gemm_i8_tcgen05_kernel<U, MD, C, B>, "launch", err, grid, smem, st); \
         return err;                                                                                                            \
     }
-#define TB200_GEMM_CS(U, MD, B) TB200_GEMM_CASE(U, MD, 1, B) TB200_GEMM_CASE(U, MD, 2, B) TB200_GEMM_CASE(U, MD, 4, B) TB200_GEMM_CASE(U, MD, 8, B)
+#define TB200_GEMM_CS(U, MD, B) TB200_GEMM_CASE(U, MD, 1, B) TB200_GEMM_CASE(U, MD, 2, B)
     TB200_GEMM_CS(false, 0, false)
     TB200_GEMM_CS(false, 1, false)
     TB200_GEMM_CS(false, 2, false)

@@ -142,20 +142,16 @@ struct GemmPlan
     // conv mode (implicit GEMM over a 4-D tensor map)
     int conv, cblocks, kw_n, pad_h, pad_w, cstride, cp, bw, bh, bn, tiles_w, tiles_h, oh, ow, nimg;
     unsigned a_tx_bytes;
-    int u8, bnx, taps, in_h, in_w; // uint8: unsigned A operand
-    int b_signed, cplane;          // uint8: B holds w - 128 as int8, a constant tile of value 128 - zw folds the rest (gemm_tcgen05.cu)
+    int u8, taps, in_h, in_w; // uint8: unsigned A operand
+    int b_signed, cplane;     // uint8: B holds w - 128 as int8, the epilogue adds (128 - zw) * sum(x) (gemm_tcgen05.cu)
     long long m_tiles;
     int swizzle; // 32 / 64 / 128
     int cs, ngroups, rows_valid, out_mode; // epilogue store groups, see gemm_tcgen05.cu plan_epilogue
     int b_res;                             // weights of the N tile resident in smem (ring carries A only)
-    // small-K variant (gemm_simple_kernel): its own B map (N tiles of <= 128 channels), shared memory per CTA
-    alignas(64) unsigned char tmap_b_s[128];
-    int simple, s_block_n, s_n_tiles, s_smem;
     void* out;
     // deferred rare path (gemm_tcgen05.cu fixq_*): per-context scratch of fixq_cap 16-byte entries per CTA; null = fix inline
     void* fixq;
     int fixq_cap;
-    int variant; // debug: descriptor variant selector (0 = default)
 };
 // Build TMA descriptors for fixed device pointers. Returns 0 or a negative TB200_ERR_*.
 // ordinal of the calling thread's current CUDA device (launchers keep per-device state: cudaFuncSetAttribute is per device)
@@ -165,14 +161,11 @@ static inline int current_device()
     cudaGetDevice(&d);
     return d;
 }
-int gemm_block_n(int ocp, int u8);
-int gemm_sx_mode();                  // TB200_U8_SX: where the uint8 path's sum(x) comes from (gemm_tcgen05.cu)
+int gemm_block_n(int ocp); // channels of one N tile = rows of one packed B tile
 // TB200_DEBUG_LAUNCH (read once per process): the templated launchers print one stderr line per launch naming the instantiation,
 // "tengine_b200: launch <kernel><ARG=value,...>"; diagnostic only, changes nothing else
 bool debug_launch();
-int gemm_tile_rows(int ocp, int u8); // rows of one packed B tile (u8 = 1 + weight zero point, 0 for int8)
-int gemm_plan_create(GemmPlan* plan, const void* a, long long lda, const void* b, void* out, long long m, int k, int oc, int ocp, int ldo,
-                     int variant, int u8);
+int gemm_plan_create(GemmPlan* plan, const void* a, long long lda, const void* b, void* out, long long m, int k, int oc, int ocp, int ldo, int u8);
 int gemm_plan_create_conv(GemmPlan* plan, const void* in, const void* w, void* out, const ConvShape& s, int u8);
 cudaError_t launch_gemm_i8(const GemmPlan& plan, const EpiParams& e, const int32_t* btab, int num_sms, cudaStream_t st);
 // measured peak of wgmma m64n128k32 s8 (two warpgroups per SM) on this GPU, in TOP/s: the tensor roofline's denominator

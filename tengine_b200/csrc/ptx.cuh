@@ -139,12 +139,6 @@ __device__ __forceinline__ void acc_ld16(uint32_t addr, uint32_t (&v)[16])
         v[4 * j] = u.x, v[4 * j + 1] = u.y, v[4 * j + 2] = u.z, v[4 * j + 3] = u.w;
     }
 }
-__device__ __forceinline__ uint32_t acc_ld1(uint32_t addr)
-{
-    uint32_t v;
-    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr));
-    return v;
-}
 
 __device__ __forceinline__ void tma_load_4d(const void* tmap, uint64_t* bar, void* smem, int c0, int c1, int c2, int c3)
 {

@@ -24,7 +24,7 @@ def cpad(c):
 
 
 # ---- gemm_tcgen05.cu: plan geometry of the persistent GEMM ------------------------------------------------------------------
-BLOCK_M, ACC_COLS_MAX, PAR_MAX, MAX_STAGES, B_RESIDENT_MAX = 128, 144, 2048, 24, 96 * 1024
+BLOCK_M, ACC_COLS_MAX, PAR_MAX, MAX_STAGES, B_RESIDENT_MAX = 128, 128, 2048, 24, 96 * 1024
 EPI_WARPS, SMEM_CTL = 16, 432  # sizeof(GemmSmemCtl): (2 * MAX_STAGES + 5) uint64, 16-byte aligned
 
 
@@ -35,13 +35,11 @@ def _block_n(ocp):
 
 def gemm_geometry(ocp, u8zp, m=None, k=None, conv=None):
     """The plan of gemm_plan_create (flat: m rows, k = K) or gemm_plan_create_conv (conv = dict(n, h, w, cp, oh, ow, kh, kw,
-    stride, ph0, pw0)), with the default switches (TB200_U8_SX 3, no TB200_GEMM_PAIR / _STORE_CS / _NO_BRES).  u8zp is the
-    planners' `u8` argument: 0 for int8, 1 + weight zero point for uint8.  Restates gemm_tcgen05.cu gemm_block_n, gemm_tile_rows,
-    gemm_plan_create (:1017-1050), gemm_plan_create_conv (:1070-1144), plan_store_groups (:957-976), epilogue_smem_bytes /
-    plan_ring (:994-1015), and launch_gemm_i8's par_all and BORDER."""
+    stride, ph0, pw0)).  u8zp is the planners' `u8` argument: 0 for int8, 1 + weight zero point for uint8.  Restates
+    gemm_tcgen05.cu gemm_block_n (:823-829), gemm_plan_create (:884-908), gemm_plan_create_conv (:912-979), plan_stage
+    (:835-843), epilogue_smem_bytes / plan_ring (:861-882), and launch_gemm_i8's par_all and BORDER (:1023, :1051)."""
     G = dict(ocp=ocp)
     bn = G["block_n"] = _block_n(ocp)
-    bnx = bn  # + 16 rows of ones only under TB200_U8_SX=0
     G["n_tiles"] = n_tiles = (ocp + bn - 1) // bn
     G["n_uneven"] = ocp % bn != 0
     if conv is None:
@@ -86,22 +84,17 @@ def gemm_geometry(ocp, u8zp, m=None, k=None, conv=None):
     G["tail"] = G["rows_valid"] % 32
     mt = 1
     if n_tiles == 1:
-        while mt < 4 and mt * 2 * bnx <= ACC_COLS_MAX and mt * 2 * 132 <= m_tiles * 132:
+        while mt < 4 and mt * 2 * bn <= ACC_COLS_MAX and mt * 2 <= m_tiles:
             mt *= 2
     G["mt"] = mt
     nch = bn // 16
-    cs = 1
-    for cc in (4, 2, 1):
-        if nch % cc == 0 and ((mt * (nch // cc)) % 4 == 0 or cc == 1):
-            cs = cc
-            break
-    G["cs"] = cs
+    G["cs"] = cs = 2 if nch % 2 == 0 and (mt * (nch // 2)) % 4 == 0 else 1
     par_ch = n_tiles * bn
     G["par_all"] = 1 if par_ch <= PAR_MAX else 0
     cplane = u8zp > 1
-    epi = EPI_WARPS * 2 * 512 * cs + (par_ch if par_ch <= PAR_MAX else bn) * 8 + SMEM_CTL + 2048 + 128 * (mt * bnx * 4 + 16) + 16
+    epi = EPI_WARPS * 2 * 512 * cs + (par_ch if par_ch <= PAR_MAX else bn) * 8 + SMEM_CTL + 2048 + 128 * (mt * bn * 4 + 16) + 16
     budget = 224 * 1024 - epi - (4096 if cplane else 0)
-    a_bytes, b_al = BLOCK_M * bk, (bnx * bk + 1023) & ~1023
+    a_bytes, b_al = BLOCK_M * bk, (bn * bk + 1023) & ~1023
     b_res = 1 if kb * b_al <= B_RESIDENT_MAX else 0
     if b_res and (budget - kb * b_al) // a_bytes < 3:
         b_res = 0
@@ -538,6 +531,3 @@ def gemm_entries():
 def uint8_gemm_entries():
     return [n for n in gemm_entries() if "_u8_" in n or n.startswith("fc_u8")]
 
-
-def dw_s1_tma_entries():
-    return [n for n, e in ENTRIES.items() if e.kernel == D_ and e.edges.get("stride", 1) == 1 and n.startswith("dw3x3s1")]

@@ -1,10 +1,9 @@
 """The edge cases of tests/kernel_edges.py on the device: every layer bit-exact against the exact reference (or the oracle, for
 ops outside ties.exact_layer), with the kernel each entry is meant to reach asserted by name.
 
-Three child processes (`python -m tests.test_gpu_kernel_edges <entry>...`) cover what the library reads once per process:
+Two child processes (`python -m tests.test_gpu_kernel_edges <entry>...`) cover what the library reads once per process:
   - TB200_DEBUG_LAUNCH: the GEMM's printed plan equals kernel_edges.gemm_geometry for every GEMM entry, so the Python
     restatement cannot drift from the code unnoticed;
-  - TB200_DW_NO_PACK3: the stride-1 depthwise entries through conv_dw3x3_tma_kernel<8,1>;
   - TB200_DEBUG_NO_CPLANE (documented to give wrong uint8 results): the uint8 GEMM entries must FAIL there -- a sweep that passed
     under a known-wrong kernel would prove nothing."""
 import os
@@ -101,14 +100,6 @@ def test_gemm_plan_equals_restatement():
         if not got or any(x != want for x in got):
             bad.append(f"{name}: printed (cs, border, out_mode, conv, n_tiles, b_res, mt, par_all) {got}, restated {want}")
     assert not bad, "\n".join(bad)
-
-
-def test_depthwise_without_pack3():
-    names = ke.dw_s1_tma_entries()
-    r = _child(names, {"TB200_DW_NO_PACK3": "1", "TB200_DEBUG_LAUNCH": "1"})
-    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
-    assert r.stdout.count("ok ") == len(names), r.stdout
-    assert r.stderr.count("launch conv_dw3x3_tma_kernel<8,1>") >= len(names), r.stderr[-3000:]
 
 
 def test_negative_control_without_the_uint8_correction():

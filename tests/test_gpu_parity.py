@@ -123,7 +123,7 @@ GEMM_CASES = [
                                               (-1, abi.RECIPE_HCL, abi.DT_INT8), (0, abi.RECIPE_HCL, abi.DT_UINT8),
                                               (-1, abi.RECIPE_REF, abi.DT_UINT8)])
 def test_tcgen05_gemm_1x1_bit_exact(ctx, oracle, case, act, recipe, dtype):
-    """uint8 runs the same UMMA with unsigned operands; the zero points are folded exactly (ones-row sum of x,
+    """uint8 runs the same UMMA with unsigned operands; the zero points are folded exactly (row-sum warps' sum of x,
     per-channel sum of w): bit-exact against the exact-integer oracle."""
     from tengine_b200 import runtime as rt
 

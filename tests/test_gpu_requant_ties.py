@@ -5,7 +5,7 @@ the reference's round-half-away: each case first shows that round half to even w
 byte of every layer to equal the exact reference.  So a tie guard or rare path that is missing, writes the wrong byte or the
 wrong address, fails here by construction -- not by chance on a few elements of a big network.
 
-Switches that the library reads once per process (TB200_NO_FIXQ, TB200_U8_SX, TB200_DEBUG_LAUNCH) are exercised in child
+Switches that the library reads once per process (TB200_NO_FIXQ, TB200_POINTWISE_EXACT, TB200_DEBUG_LAUNCH) are exercised in child
 processes (`python -m tests.test_gpu_requant_ties <case>...`); the ones read per plan are set around the graph's lifetime."""
 import ctypes as C
 import os
@@ -47,14 +47,13 @@ def _add(name, build, env=None, flags=0):
 
 
 # ---- persistent GEMM (gemm_i8_tcgen05_kernel<U8, MODE, CS, BORDER>) ----
-# 1x1 (flat GEMM), ragged M (2*15*15 = 450 rows), 128-channel N tile (8 chunks: CS 1 / 2 / 4 all admissible), odd OC
-for cs in (1, 2, 4):
-    for mode in (0, 1, 2):
-        _add(f"gemm1x1_i8_m{mode}_cs{cs}", _i8(2, 64, 15, 15, 125, mode=mode), {"TB200_GEMM_STORE_CS": str(cs)})
-    for mode in (0, 2):
-        _add(f"gemm1x1_u8_m{mode}_cs{cs}", _u8(2, 64, 15, 15, 125, mode=mode), {"TB200_GEMM_STORE_CS": str(cs)})
-        # uint8 with padding: BORDER corrections (implicit GEMM, 3x3, out_mode 1)
-        _add(f"igemm3x3_u8_border_m{mode}_cs{cs}", _u8(2, 64, 17, 19, 61, k=3, pad=1, mode=mode), {"TB200_GEMM_STORE_CS": str(cs)})
+# 1x1 (flat GEMM), ragged M (2*15*15 = 450 rows), 128-channel N tile (8 chunks: the planner picks CS 2), odd OC
+for mode in (0, 1, 2):
+    _add(f"gemm1x1_i8_m{mode}_cs2", _i8(2, 64, 15, 15, 125, mode=mode))
+for mode in (0, 2):
+    _add(f"gemm1x1_u8_m{mode}_cs2", _u8(2, 64, 15, 15, 125, mode=mode))
+    # uint8 with padding: BORDER corrections (implicit GEMM, 3x3, out_mode 1; 64-channel N tile, 2 m-tiles a stage: CS 2)
+    _add(f"igemm3x3_u8_border_m{mode}_cs2", _u8(2, 64, 17, 19, 61, k=3, pad=1, mode=mode))
 # implicit GEMM output modes: 0 (several images per m-tile), 1 (ow <= 128), 2 (ow > 128, ragged last tile of each row)
 for mode in (0, 1, 2):
     _add(f"igemm_i8_outmode0_m{mode}", _i8(5, 64, 7, 7, 48, k=3, pad=1, mode=mode))
@@ -68,7 +67,6 @@ for mode in (0, 2):
 # several N tiles: weights resident (K = 64) and streamed (K = 1024)
 _add("gemm_i8_ntiles2_resident", _i8(2, 64, 13, 11, 250, mode=1))
 _add("gemm_i8_ntiles2_streamed", _i8(1, 1024, 9, 9, 250, mode=0, m_exps=(2, 2, 2, 3, 4, 5, 6, 7, 8)))  # (M = 2^-1 fails the proof at K = 1024)
-_add("gemm_i8_ntiles2_no_bres", _i8(2, 64, 13, 11, 250, mode=1), {"TB200_GEMM_NO_BRES": "1"})
 _add("gemm_u8_ntiles2_streamed", _u8(1, 512, 9, 9, 250))
 # ---- FC (persistent GEMM over one row per image) ----
 for mode in (0, 2):
@@ -83,7 +81,6 @@ for mode in (0, 1, 2):
         _add(f"stem7x7_i8_{tag}_m{mode}", _i8(2, 3, 30, 32, 24, k=7, stride=2, pad=3, mode=mode), env)
         _add(f"nhwc16_3x3_i8_{tag}_m{mode}", _i8(2, 16, 15, 17, 40, k=3, pad=1, mode=mode, recipe=R), env)
     _add(f"nhwc32_3x3_i8_window_m{mode}", _i8(2, 32, 18, 18, 40, k=3, stride=2, pad=1, mode=mode))
-    _add(f"gemm_simple_i8_m{mode}", _i8(2, 64, 15, 15, 72, mode=mode), {"TB200_GEMM_SIMPLE": "1"})
 for mode in (0, 2):
     for tag, env in (("window", {}), ("gather", {"TB200_NO_WINDOW_CONV": "1"})):
         _add(f"stem3x3_u8_{tag}_m{mode}", _u8(2, 3, 24, 32, 40, k=3, stride=2, pad=1, mode=mode), env)
@@ -135,12 +132,10 @@ _add("queue_dense", _i8(8, 64, 96, 96, 128, mode=0, m_exps=(1,)))
 _add("queue_dense_u8", lambda r: ties.uint8_conv(r, 8, 64, 96, 96, 128, s_out=2.0 ** -6))
 
 QUEUE = ["queue_sparse", "queue_dense", "queue_dense_u8"]
-NO_FIXQ = QUEUE + ["gemm1x1_i8_m0_cs4", "gemm1x1_u8_m0_cs4", "igemm3x3_u8_border_m0_cs2", "igemm_i8_outmode2_m1",
+NO_FIXQ = QUEUE + ["gemm1x1_i8_m0_cs2", "gemm1x1_u8_m0_cs2", "igemm3x3_u8_border_m0_cs2", "igemm_i8_outmode2_m1",
                    "igemm_u8_outmode2_m0", "fc_i8_m0"]
 # TB200_POINTWISE_EXACT (read once per process by the fast pointwise launcher): the literal per-element kernel
 PW_EXACT = [n for n in CASES if n.endswith("_pwexact")]
-U8_SX0 = ["gemm1x1_u8_m0_cs4", "igemm3x3_u8_border_m0_cs2", "igemm_u8_outmode0_m0", "igemm_u8_outmode2_m2", "fc_u8_m0",
-          "queue_dense_u8"]
 
 
 def build(name):
@@ -243,8 +238,8 @@ def _child(names, env, timeout=900):
     return r
 
 
-@pytest.mark.parametrize("env,names", [({"TB200_NO_FIXQ": "1"}, NO_FIXQ), ({"TB200_U8_SX": "0"}, U8_SX0),
-                                       ({"TB200_POINTWISE_EXACT": "1"}, PW_EXACT)], ids=["no_fixq", "u8_sx0", "pointwise_exact"])
+@pytest.mark.parametrize("env,names", [({"TB200_NO_FIXQ": "1"}, NO_FIXQ), ({"TB200_POINTWISE_EXACT": "1"}, PW_EXACT)],
+                         ids=["no_fixq", "pointwise_exact"])
 def test_once_per_process_switches(env, names):
     r = _child(names, env)
     assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
@@ -256,7 +251,7 @@ def _expected_instantiations():
     exp = set()
     for u8, modes in ((0, (0, 1, 2)), (1, (0, 2))):
         for m in modes:
-            for cs in (1, 2, 4, 8):
+            for cs in (1, 2):
                 for border in ((0,) if not u8 else (0, 1)):
                     exp.add(f"gemm_i8_tcgen05_kernel<U8={u8},MODE={m},CS={cs},BORDER={border}>")
         for m in modes:
@@ -264,43 +259,24 @@ def _expected_instantiations():
                 exp.add(f"conv_gather_tc_kernel<MODE={m},U8={u8},KHW={k}>")
             for ly in (0, 1, 2, 3):
                 exp.add(f"conv_window_tc_kernel<MODE={m},U8={u8},LAYOUT={ly}>")
-    for m in (0, 1, 2):
-        exp.add(f"gemm_simple_kernel<MODE={m}>")
-    for k in ("conv_dw3x3_tma_pack3_kernel", "conv_dw3x3_tma_kernel<4,2>", "conv_dw3x3_tma_kernel<8,1>"):
+    for k in ("conv_dw3x3_tma_pack3_kernel", "conv_dw3x3_tma_kernel<4,2>"):
         for m in (0, 1, 2):
             exp.add(f"{k} MODE={m}")
     return exp
 
 
-# Instantiations no graph can reach, and why.
-UNREACHABLE = {
-    # CS 8 (warp pairs filling 128-byte rows) needs a 128-channel N tile AND an even number of m-tiles per accumulator stage;
-    # with the 144-column accumulator image (ACC_COLS_MAX) a 128-column N tile always runs one m-tile per stage
-    **{f"gemm_i8_tcgen05_kernel<U8={u},MODE={m},CS=8,BORDER={b}>": "CS 8 needs two m-tiles of a 128-channel N tile per stage"
-       for u, ms, bs in ((0, (0, 1, 2), (0,)), (1, (0, 2), (0, 1))) for m in ms for b in bs},
-}
-
-
-# the stride-1 depthwise cases once more with TB200_DW_NO_PACK3 (read once per process): conv_dw3x3_tma_kernel<8,1>
-NO_PACK3 = [n for n in CASES if n.startswith("dw3x3_i8_s1")]
-
-
-def test_every_reachable_instantiation_is_launched():
-    """All cases in one child process with TB200_DEBUG_LAUNCH (and the stride-1 depthwise ones in a second, without the packed
-    kernel): every instantiation a launcher can select appears in their report."""
+def test_every_compiled_instantiation_is_launched():
+    """All cases in one child process with TB200_DEBUG_LAUNCH: every instantiation the library compiles appears in its report."""
+    r = _child([n for n in CASES if n not in PW_EXACT], {"TB200_DEBUG_LAUNCH": "1"}, timeout=1800)
+    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
     launched = set()
-    for names, env in (([n for n in CASES if n not in PW_EXACT], {}), (NO_PACK3, {"TB200_DW_NO_PACK3": "1"})):
-        r = _child(names, {"TB200_DEBUG_LAUNCH": "1", **env}, timeout=1800)
-        assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
-        for line in r.stderr.splitlines():
-            m = re.match(r"tengine_b200: launch (\S+(?: MODE=\d)?)", line)
-            if m:
-                launched.add(m.group(1))
-    exp = _expected_instantiations()
-    missing = sorted(exp - launched - set(UNREACHABLE))
+    for line in r.stderr.splitlines():
+        m = re.match(r"tengine_b200: launch (\S+(?: MODE=\d)?)", line)
+        if m:
+            launched.add(m.group(1))
+    missing = sorted(_expected_instantiations() - launched)
     print("launched:", sorted(launched))
     assert not missing, f"never launched: {missing}"
-    assert not (set(UNREACHABLE) & launched), sorted(set(UNREACHABLE) & launched)
 
 
 # ---- the literal-arithmetic kernel entry points (tb200k_*) on tie-dense layers: the control, pad lanes included ----

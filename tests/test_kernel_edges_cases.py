@@ -69,4 +69,3 @@ def test_gemm_entries_are_listed():
     assert len(ke.gemm_entries()) >= 30
     u8 = ke.uint8_gemm_entries()
     assert u8 and all(ke.build(n).g.data_type == ke.abi.DT_UINT8 for n in u8)
-    assert ke.dw_s1_tma_entries()
