@@ -361,6 +361,36 @@ TB200_API int tb200_graph_yolov5_detect(tb200_graph* g, const tb200_yolo_params*
 TB200_API int tb200_detections_to_source(int mode, const tb200_detect_geometry* geometry, int num_images, tb200_detection* dets, int max_per_image,
                                          const int32_t* counts);
 
+/* ---- classification post-processing on the device ---------------------------------------------------------------------------
+ * The last step of examples/tm_classification_int8.c and examples/tm_classification_uint8.c on the graph's quantised output tensor
+ * where it lies in HBM (after tb200_graph_run / tb200_graph_launch): k (score, id) pairs per image come back instead of every class.
+ *   classes  The classes of image i are its E = C*H*W elements in NCHW order, id = c*H*W + h*W + w: what the examples read from
+ *            get_tensor_buffer at batch 1.  The usual tensor is [N, classes, 1, 1].
+ *   score    int8: (float)q * scale (tm_classification_int8.c:163-164; the zero point is not used).  uint8: ((float)q -
+ *            (float)zero_point) * scale (tm_classification_uint8.c:169-170).  Float arithmetic, one rounding per operation.  Scale and
+ *            zero point are the output tensor's own.
+ *   order    print_topk (examples/common/tengine_operations.c:1021-1038) fills an array with (id, score) in buffer order, sorts all of
+ *            it with sort_cls_score(array, 0, E - 1) (:991-1019) and prints entries 0..k-1; out holds exactly those entries.  The sort
+ *            is an unstable quicksort and a quantised output is mostly equal scores, so which of several equal classes is reported, and
+ *            in which order, is the example's choice and is reproduced.  Every comparison is the example's own operator on the
+ *            dequantised floats, so the result is the example's for any finite scale: zero, negative, overflowing to infinity.  (A NaN
+ *            score fails both comparisons of sort_cls_score and its loop never ends, so a scale that is not finite is refused.)
+ * tb200_class_score carries the two fields of cls_score (tengine_operations.h:57-61), score first. */
+#define TB200_TOPK_MAX 64            /* largest k */
+#define TB200_TOPK_MAX_CLASSES 32768 /* largest E: an image's scores and ids are staged in shared memory (6 bytes per class of the
+                                        227 KB a thread block may use on sm_90) */
+typedef struct tb200_class_score
+{
+    float score;
+    int32_t id;
+} tb200_class_score;
+/* out[image * k + r], r < k: entry r of the example's sorted array for that image of graph output `output_index`; HOST memory for
+ * N * k entries.  Synchronous, like tb200_graph_yolo_detect; on a multi-GPU context every shard writes its own images' rows.
+ * Checked before any work, `out` left untouched: TB200_ERR_INVALID for a null pointer, an output index out of range, k < 1, k > E (the
+ * example asserts total_num >= topk), k > TB200_TOPK_MAX, an output that is not int8 / uint8, a scale that is not finite; TB200_ERR_UNSUPPORTED for
+ * E > TB200_TOPK_MAX_CLASSES. */
+TB200_API int tb200_graph_topk(tb200_graph* g, int output_index, int k, tb200_class_score* out);
+
 /* ---- kernel launchers (device pointers; NHWC with channels padded to tb200k_cpad(c)) --------------- */
 typedef struct tb200k_epilogue
 {
@@ -403,6 +433,10 @@ TB200_API int tb200k_gemm_i8(const void* in, const void* weight, void* out, int6
 /* layout conversion host-NCHW <-> device-NHWC(pad) */
 TB200_API int tb200k_nchw_to_nhwc(const void* in, void* out, int n, int c, int h, int w, void* stream);
 TB200_API int tb200k_nhwc_to_nchw(const void* in, void* out, int n, int c, int h, int w, void* stream);
+/* tb200_graph_topk's kernel on a DEVICE tensor in the device layout ([n][h][w][tb200k_cpad(c)] bytes; pad lanes are not read):
+ * out is a DEVICE pointer to n * k entries; asynchronous on `stream`.  Same semantics and the same checks. */
+TB200_API int tb200k_class_topk(const void* in, int n, int c, int h, int w, int is_uint8, float scale, int32_t zero_point, int k,
+                                tb200_class_score* out, void* stream);
 
 /* ---- fp32 members of the path (north star: "fp32 paths within 1e-4 rel"); NCHW fp32 DEVICE pointers as Tengine lays them out.
  * Winograd F(4x4, 3x3): 3x3, stride 1, dilation 1, group 1 -- what winograd_support() admits (conv_kernel_x86.c:1896-1915;

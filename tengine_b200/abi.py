@@ -57,12 +57,12 @@ class KConvShape(C.Structure):
 EXPORTS = [
     "tb200_abi_version", "tb200_last_error", "tb200_device_count", "tb200_context_create", "tb200_context_destroy",
     "tb200_context_stream", "tb200_context_create_multi", "tb200_context_num_gpus", "tb200_context_gpu", "tb200_context_stream_of",
-    "tb200_context_broadcast_kind", "tb200_shard_range", "tb200_graph_broadcast_weights", "tb200_graph_num_shards", "tb200_graph_shard", "tb200_graph_arena_bytes", "tb200_probe_int8_tops", "tb200_pack_cache_dir", "tb200_graph_pack_cache_state", "tb200_graph_yolo_detect", "tb200_graph_yolov5_detect", "tb200k_conv_winograd43_f32_workspace", "tb200k_conv_winograd43_f32", "tb200k_conv_dw3x3_f32",
+    "tb200_context_broadcast_kind", "tb200_shard_range", "tb200_graph_broadcast_weights", "tb200_graph_num_shards", "tb200_graph_shard", "tb200_graph_arena_bytes", "tb200_probe_int8_tops", "tb200_pack_cache_dir", "tb200_graph_pack_cache_state", "tb200_graph_yolo_detect", "tb200_graph_yolov5_detect", "tb200_graph_topk", "tb200k_conv_winograd43_f32_workspace", "tb200k_conv_winograd43_f32", "tb200k_conv_dw3x3_f32",
     "tb200_host_alloc", "tb200_host_free", "tb200_graph_prerun", "tb200_graph_run",
     "tb200_graph_upload", "tb200_graph_upload_images", "tb200_graph_upload_detect_images", "tb200_detections_to_source", "tb200_graph_launch", "tb200_graph_download", "tb200_graph_sync", "tb200_graph_postrun",
     "tb200_graph_weight_arena", "tb200_graph_num_launches", "tb200_graph_layer_kernel", "tb200_graph_read_tensor",
     "tb200_graph_profile", "tb200_graph_work", "tb200k_cpad", "tb200k_conv_direct", "tb200k_conv_dw3x3",
-    "tb200k_conv_stem_nchw", "tb200k_gemm_i8", "tb200k_nchw_to_nhwc", "tb200k_nhwc_to_nchw",
+    "tb200k_conv_stem_nchw", "tb200k_gemm_i8", "tb200k_nchw_to_nhwc", "tb200k_nhwc_to_nchw", "tb200k_class_topk",
 ]
 
 
@@ -93,3 +93,10 @@ class YoloParams(C.Structure):
 
 class Detection(C.Structure):
     _fields_ = [("x", C.c_float), ("y", C.c_float), ("w", C.c_float), ("h", C.c_float), ("prob", C.c_float), ("label", C.c_int32)]
+
+
+TOPK_MAX, TOPK_MAX_CLASSES = 64, 32768
+
+
+class ClassScore(C.Structure):
+    _fields_ = [("score", C.c_float), ("id", C.c_int32)]

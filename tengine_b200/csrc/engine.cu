@@ -2510,6 +2510,48 @@ int tb200_graph_yolov5_detect(tb200_graph* g, const tb200_yolo_params* p, tb200_
     return yolo_detect(g, p, out, max_per_image, counts, YoloBox::V5);
 }
 
+// The argument checks tb200_graph_topk and tb200k_class_topk share; 0 when the launch may go ahead.
+static int class_topk_check(int data_type, float scale, long long e, int k)
+{
+    static_assert(CLASS_TOPK_MAX_K == TB200_TOPK_MAX && CLASS_TOPK_MAX_CLASSES == TB200_TOPK_MAX_CLASSES, "top-k limits");
+    static_assert(sizeof(ClassScore) == sizeof(tb200_class_score) && offsetof(ClassScore, id) == offsetof(tb200_class_score, id), "class score record layout");
+    if (data_type != TB200_DT_INT8 && data_type != TB200_DT_UINT8) return fail(TB200_ERR_INVALID, "topk: data type %d is not int8 / uint8", data_type);
+    if (k < 1 || k > TB200_TOPK_MAX) return fail(TB200_ERR_INVALID, "topk: k = %d outside 1..%d", k, TB200_TOPK_MAX);
+    if (k > e) return fail(TB200_ERR_INVALID, "topk: k = %d of %lld classes", k, e);
+    // a NaN score fails both of sort_cls_score's comparisons, so neither scan moves and the example's loop never ends: there is no
+    // result to reproduce.  A finite scale cannot produce one (scores are finite or infinite, which compare like any number).
+    if (!std::isfinite(scale)) return fail(TB200_ERR_INVALID, "topk: scale %g is not finite", (double)scale);
+    if (e > TB200_TOPK_MAX_CLASSES) return fail(TB200_ERR_UNSUPPORTED, "topk: %lld classes per image, at most %d are staged", e, TB200_TOPK_MAX_CLASSES);
+    return 0;
+}
+
+int tb200_graph_topk(tb200_graph* g, int output_index, int k, tb200_class_score* out)
+{
+    if (!g || !out || output_index < 0 || output_index >= (int)g->output_ids.size()) return fail(TB200_ERR_INVALID, "bad topk arguments");
+    {
+        const tb200_tensor_desc& d = g->tensors[g->output_ids[output_index]].d;
+        if (const int rc = class_topk_check(d.data_type, d.scale, (long long)d.dims[1] * d.dims[2] * d.dims[3], k)) return rc;
+    }
+    const int rc = for_each_shard(g, [&](tb200_graph* sh, int) -> int {
+        const TensorInfo& t = sh->tensors[sh->output_ids[output_index]];
+        CUDA_OK(cudaSetDevice(sh->ctx->device));
+        cudaGetLastError(); // the launch below reports cudaGetLastError(): a non-sticky error an earlier call left behind is not its own
+        cudaStream_t st = sh->ctx->stream;
+        const size_t bytes = sizeof(ClassScore) * (size_t)sh->num_images * k;
+        ClassScore* dev = nullptr;
+        cudaError_t e = cudaMalloc(&dev, bytes);
+        if (e == cudaSuccess)
+            e = launch_class_topk(t.dev, sh->num_images, t.d.dims[1], t.d.dims[2], t.d.dims[3], t.d.data_type == TB200_DT_UINT8, t.d.scale, t.d.zero_point, k, dev, st);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(out + (size_t)sh->first_image * k, dev, bytes, cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+        cudaFree(dev);
+        if (e != cudaSuccess) return fail(TB200_ERR_CUDA, "topk: %s", cudaGetErrorString(e));
+        return 0;
+    });
+    cudaSetDevice(g->ctx->device);
+    return rc;
+}
+
 int tb200_graph_work(tb200_graph* g, double* ops, double* bytes)
 {
     if (!g) return fail(TB200_ERR_INVALID, "null graph");
@@ -2606,4 +2648,10 @@ int tb200k_nhwc_to_nchw(const void* in, void* out, int n, int c, int h, int w, v
     K_LAUNCH(launch_nhwc_to_nchw(in, out, n, c, h, w, (cudaStream_t)stream));
 }
 
+int tb200k_class_topk(const void* in, int n, int c, int h, int w, int is_uint8, float scale, int32_t zero_point, int k, tb200_class_score* out, void* stream)
+{
+    K_CHECK(in && out && n > 0 && c > 0 && h > 0 && w > 0);
+    if (const int rc = class_topk_check(is_uint8 ? TB200_DT_UINT8 : TB200_DT_INT8, scale, (long long)c * h * w, k)) return rc;
+    K_LAUNCH(launch_class_topk(in, n, c, h, w, is_uint8 != 0, scale, zero_point, k, (ClassScore*)out, (cudaStream_t)stream));
+}
 } // extern "C"

@@ -94,6 +94,18 @@ cudaError_t launch_yolo_decode(YoloBox f, const void* tensor, int cp, int h, int
 cudaError_t launch_yolo_nms(const YoloCand* cand, const int* count, int n_img, int max_cand, float nms_thr, YoloCand* sorted, YoloDet* out, int max_out,
                             int* out_count, cudaStream_t st);
 
+// ---- classification post-processing (classify_topk.cu) ---------------------------------------------------------
+struct ClassScore // tb200_class_score
+{
+    float score;
+    int32_t id;
+};
+constexpr int CLASS_TOPK_MAX_K = 64;          // TB200_TOPK_MAX
+constexpr int CLASS_TOPK_MAX_CLASSES = 32768; // TB200_TOPK_MAX_CLASSES: one image's scores and ids are staged in shared memory
+// in: [n][h][w][cpad(c)] int8 (u8 = false) or uint8 bytes; out[image * k + r]: entry r of the array the classification examples' print_topk
+// holds after sorting the image's c*h*w dequantised scores (ids in NCHW order)
+cudaError_t launch_class_topk(const void* in, int n, int c, int h, int w, bool u8, float scale, int zero_point, int k, ClassScore* out, cudaStream_t st);
+
 // ---- input preprocessing (image_pre.cu, detect_pre.cu) ------------------------------------------------------------
 // One image of a staged batch: h rows of w pixels of c interleaved bytes (c = 3 or 4) at `offset` of the shard's staging buffer; for
 // detection also where its resized copy lies in the laid-out image (tb200_detect_geometry; unused by image_pre)

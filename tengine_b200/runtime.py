@@ -80,6 +80,8 @@ def lib():
         L.tb200_graph_broadcast_weights.argtypes = [C.c_void_p]
         L.tb200_pack_cache_dir.argtypes = [C.c_char_p]
         L.tb200_graph_pack_cache_state.argtypes = [C.c_void_p]
+        L.tb200_graph_topk.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
+        L.tb200k_class_topk.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int32, C.c_int, C.c_void_p, C.c_void_p]
         _lib = L
     return _lib
 
@@ -115,6 +117,12 @@ def detections_to_source(geometry, boxes, letterbox=True):
             d.x, d.y, d.w, d.h, d.prob, d.label = b
     _check(lib().tb200_detections_to_source(abi.PRE_LETTERBOX if letterbox else abi.PRE_STRETCH, geometry, n, dets, m, counts))
     return [[(d.x, d.y, d.w, d.h, d.prob, d.label) for d in dets[i * m:i * m + counts[i]]] for i in range(n)]
+
+
+def class_topk(in_ptr, n, c, h, w, is_uint8, scale, zero_point, k, out_ptr, stream=None):
+    """tb200k_class_topk on DEVICE pointers: `in_ptr` an [n, h, w, cpad(c)] int8 / uint8 tensor, `out_ptr` room for n * k
+    abi.ClassScore records; asynchronous on `stream`."""
+    _check(lib().tb200k_class_topk(in_ptr, int(n), int(c), int(h), int(w), int(bool(is_uint8)), float(scale), int(zero_point), int(k), out_ptr, stream))
 
 
 def device_count():
@@ -370,6 +378,16 @@ class Graph:
                 raise TB200Error(abi.ERR_INVALID, f"image {i}: {-counts[i]} boxes / candidates do not fit")
             res.append([(d.x, d.y, d.w, d.h, d.prob, d.label) for d in out[i * max_per_image:i * max_per_image + counts[i]]])
         return res
+
+    def topk(self, output_index=0, k=5):
+        """What the classification examples print for every image of the last run (tb200_graph_topk): graph output `output_index`
+        dequantised and ranked on the device in print_topk's order, its tie order included.  Returns (scores [N, k] float32,
+        ids [N, k] int32); an id is the class's position among the image's elements in NCHW order."""
+        n = self.gdef.dims(self.gdef.outputs[output_index])[0]
+        out = np.zeros((n, max(int(k), 0)), np.dtype([("score", np.float32), ("id", np.int32)]))
+        assert out.dtype.itemsize == C.sizeof(abi.ClassScore)
+        _check(lib().tb200_graph_topk(self.h, int(output_index), int(k), out.ctypes.data))
+        return np.ascontiguousarray(out["score"]), np.ascontiguousarray(out["id"])
 
     def pack_cache_state(self):
         """0: no cache directory, 1: packed and written to the cache, 2: arena image read from the cache."""
