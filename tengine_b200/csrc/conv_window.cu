@@ -251,7 +251,6 @@ bool window_nhwc_fits(int cp, int ocp, int stride)
 int window_plan_create(WindowPlan* p, const void* in, const ConvShape& s, int nhwc)
 {
     memset(p, 0, sizeof *p);
-    if (getenv("TB200_NO_WINDOW_CONV")) return -1;
     if (s.group != 1 || s.dh != 1 || s.dw != 1 || s.sh != s.sw || s.sh < 1 || s.sh > 2 || s.kh != s.kw || s.ocp > 256) return -1;
     if (nhwc)
     {
@@ -330,7 +329,7 @@ cudaError_t launch_conv_window(const WindowPlan& p, const void* w, void* out, co
 
 // ---- gather convolution on the tensor cores (NCHW stems, 3x3 convolutions over 16-channel NHWC tensors) ----------------
 // The window kernel's layers when it has no plan: NCHW inputs whose width is not a multiple of 16 (a tensor map's global
-// strides must be), windows too large for shared memory, TB200_NO_WINDOW_CONV.  Same skeleton, without the staged window:
+// strides must be), windows too large for shared memory.  Same skeleton, without the staged window:
 // every thread gathers the K bytes of its output pixel itself -- NCHW: 27 / 147 byte loads; NHWC16: nine 16-byte loads, one
 // per tap -- and writes them as one row of `ks` SW32 K-major k-block tiles; `ks`
 // k-steps (K = 32 each) accumulate.  uint8: taps outside the image are filled with the input zero point (they then contribute

@@ -287,8 +287,7 @@ static int context_create_one(int cuda_device, tb200_context** out)
     c->device = cuda_device;
     c->num_sms = sms;
     c->stream = st;
-    static const bool no_fixq = getenv("TB200_NO_FIXQ") != nullptr; // A/B switch: guarded elements fixed inline
-    if (!no_fixq) CUDA_OK(cudaMalloc(&c->fixq, (size_t)sms * FIXQ_CAP * 16));
+    CUDA_OK(cudaMalloc(&c->fixq, (size_t)sms * FIXQ_CAP * 16));
     *out = c;
     return 0;
 }
@@ -767,7 +766,6 @@ static int setup_tensors(tb200_graph* g, const tb200_tensor_desc* tensors, int n
 // The kernel of a convolution and the bytes of its packed weights: each kind's predicate next to its weight size.
 static int plan_conv(int li, const tb200_layer_desc& L, const TensorInfo& tin, const TensorInfo& tout, bool no_tc, LayerPlan& P)
 {
-    const bool u8 = tin.d.data_type == TB200_DT_UINT8;
     const int C = tin.d.dims[1], H = tin.d.dims[2], W = tin.d.dims[3], OC = tout.d.dims[1];
     if (!L.weight || !L.weight_scales) return fail(TB200_ERR_INVALID, "layer %d: conv without weight/scales", li);
     if (L.group < 1 || C % L.group || OC % L.group) return fail(TB200_ERR_INVALID, "layer %d: bad group %d", li, L.group);
@@ -779,8 +777,8 @@ static int plan_conv(int li, const tb200_layer_desc& L, const TensorInfo& tin, c
     const bool nchw_input = tin.input_index >= 0 && C <= 3; // an RGB / grey stem over the NCHW graph input
     const bool tc = !no_tc && L.group == 1;                                                       // a tensor-core kernel may take it
     const bool plain = L.dilation_h == 1 && L.dilation_w == 1 && L.stride_h == L.stride_w;         // no dilation, one stride
-    const bool k3 = L.kernel_h == 3 && L.kernel_w == 3, u8_tc_on = !(u8 && getenv("TB200_NO_U8_TC"));
-    const bool gather = tc && plain && tout.cp <= 256 && !getenv("TB200_NO_GATHER_TC");
+    const bool k3 = L.kernel_h == 3 && L.kernel_w == 3;
+    const bool gather = tc && plain && tout.cp <= 256;
     size_t& wsize = P.blob.w_size;
     if (nchw_input && gather && L.kernel_h == L.kernel_w && (L.kernel_h == 3 || L.kernel_h == 7))
         // 3x3 and 7x7 (ResNet) stems: K = C*KH*KW padded to 32*ks (one k-step for a 3x3 stem); uint8 taps outside the image = zero point
@@ -789,14 +787,14 @@ static int plan_conv(int li, const tb200_layer_desc& L, const TensorInfo& tin, c
         P.kind = K_CONV_STEM, P.reads_nchw = true, wsize = (size_t)tout.cp * L.kernel_h * L.kernel_w * 4;
     else if (gather && k3 && tin.cp == 16)
         P.kind = K_GATHER_TC, P.nhwc16 = 1, wsize = (size_t)tout.cp * 160; // 16-channel input: nine 16-byte taps per pixel, five k-steps
-    else if (gather && k3 && tin.cp == 32 && (L.stride_h == 1 || L.stride_h == 2) && window_nhwc_fits(32, tout.cp, L.stride_h) && !getenv("TB200_NO_WINDOW_CONV"))
+    else if (gather && k3 && tin.cp == 32 && (L.stride_h == 1 || L.stride_h == 2) && window_nhwc_fits(32, tout.cp, L.stride_h))
         P.kind = K_GATHER_TC, P.nhwc16 = 1, wsize = (size_t)tout.cp * 288; // 32-channel input through the window kernel: nine 32-byte taps = nine k-steps
     else if (L.group == C && OC == C && C > 1)
         P.kind = K_CONV_DW, wsize = (size_t)L.kernel_h * L.kernel_w * tin.cp;
-    else if (tc && u8_tc_on && L.kernel_h == 1 && L.kernel_w == 1 && L.stride_h == 1 && L.stride_w == 1 && !L.pad_h0 && !L.pad_h1 && !L.pad_w0 && !L.pad_w1)
+    else if (tc && L.kernel_h == 1 && L.kernel_w == 1 && L.stride_h == 1 && L.stride_w == 1 && !L.pad_h0 && !L.pad_h1 && !L.pad_w0 && !L.pad_w1)
         P.kind = K_GEMM, wsize = gemm_weight_bytes(tout.cp, tin.cp);
-    else if (tc && u8_tc_on && plain && (L.stride_h == 1 || L.stride_h == 2) && (L.kernel_h * L.kernel_w == 1 || tin.cp % 32 == 0) &&
-             tout.d.dims[3] <= 4096 && L.kernel_h * L.kernel_w <= 64 && !getenv("TB200_NO_IGEMM"))
+    else if (tc && plain && (L.stride_h == 1 || L.stride_h == 2) && (L.kernel_h * L.kernel_w == 1 || tin.cp % 32 == 0) &&
+             tout.d.dims[3] <= 4096 && L.kernel_h * L.kernel_w <= 64)
         P.kind = K_IGEMM, wsize = gemm_weight_bytes(tout.cp, L.kernel_h * L.kernel_w * tin.cp);
     else
     {
@@ -837,7 +835,7 @@ static int plan_kernels(tb200_graph* g, std::vector<LayerPlan>& plan)
         else if (L.op == TB200_OP_FC)
         {
             if (!L.weight || !L.weight_scales) return fail(TB200_ERR_INVALID, "layer %d: fc without weight/scales", li);
-            if (no_tc || (u8 && getenv("TB200_NO_U8_TC")))
+            if (no_tc)
                 P.kind = K_CONV_DIRECT, P.blob.w_size = (size_t)tout.cp * H * W * tin.cp; // FC == conv with kernel HxW over the whole input
             else
                 P.kind = K_GEMM, P.blob.w_size = gemm_weight_bytes(tout.cp, H * W * tin.cp);
@@ -917,7 +915,7 @@ static int plan_kernels(tb200_graph* g, std::vector<LayerPlan>& plan)
 static void plan_activation_arena(tb200_graph* g, std::vector<LayerPlan>& plan)
 {
     const int num_layers = (int)g->layers.size(), num_tensors = (int)g->tensors.size();
-    const bool reuse = !(g->flags & TB200_PRERUN_NO_GRAPH) && !getenv("TB200_NO_ARENA_REUSE");
+    const bool reuse = !(g->flags & TB200_PRERUN_NO_GRAPH);
     for (int li = 0; li < num_layers; li++)
         for (int k = 0; k < g->layers[li].num_inputs; k++) g->tensors[g->layers[li].inputs[k]].last_use = li;
     struct Blk { size_t off, bytes; };
@@ -1022,7 +1020,6 @@ static int alloc_device_buffers(tb200_graph* g)
 //      reaches the same arena format. ----
 static void prove_fast_epilogues(const tb200_graph* g, std::vector<LayerPlan>& plan)
 {
-    const bool no_fuse_bias = getenv("TB200_NO_FUSE_BIAS") != nullptr;
     for (size_t li = 0; li < g->layers.size(); li++)
     {
         const tb200_layer_desc& L = g->layers[li];
@@ -1033,7 +1030,7 @@ static void prove_fast_epilogues(const tb200_graph* g, std::vector<LayerPlan>& p
         const bool u8 = tin.d.data_type == TB200_DT_UINT8;
         const int OC = tout.d.dims[1];
         // may the int8 fast epilogue fold the bias add into its FMA?  (common.cuh requant_fast_bits<.., FUSE>)
-        if (L.op == TB200_OP_CONV && !u8 && !no_fuse_bias)
+        if (L.op == TB200_OP_CONV && !u8)
         {
             bool fuse = true;
             for (int o = 0; o < OC; o++)
@@ -1386,8 +1383,8 @@ static int upload_weights(tb200_graph* g, const std::vector<LayerPlan>& plan)
     return 0;
 }
 
-// ---- pipeline chunks: the batch is cut into K chunks (images are independent units) so that `run` can overlap the H2D copy
-//      of chunk i+1 with the kernels of chunk i; each chunk owns a slice of every tensor ----
+// ---- pipeline chunks: an even batch of 32 or more is cut into two chunks (images are independent units) so that `run` can
+//      overlap the H2D copy of the second with the kernels of the first; each chunk owns a slice of every tensor ----
 static void plan_chunks(tb200_graph* g)
 {
     const int Ntot = g->tensors[0].d.dims[0];
@@ -1395,41 +1392,13 @@ static void plan_chunks(tb200_graph* g)
     for (auto& t : g->tensors) same_batch &= (t.d.dims[0] == Ntot);
     int K = 1;
     std::vector<int> cfirst{0}, ccount{Ntot};
-    if (same_batch && !(g->flags & TB200_PRERUN_NO_GRAPH))
+    if (same_batch && !(g->flags & TB200_PRERUN_NO_GRAPH) && Ntot >= 32 && Ntot % 2 == 0)
     {
-        K = Ntot >= 32 ? 2 : 1;
-        if (const char* ev = getenv("TB200_PIPELINE_CHUNKS")) K = atoi(ev) > 0 ? atoi(ev) : K;
-        while (K > 1 && Ntot % K) K--;
-        cfirst.clear(), ccount.clear();
-        for (int k = 0; k < K; k++) cfirst.push_back(k * (Ntot / K)), ccount.push_back(Ntot / K);
-        if (K == 2 && Ntot >= 64 && !getenv("TB200_PIPELINE_CHUNKS"))
-        {
-            // two chunks of 1/4 and 3/4: the kernels only ever wait for the first quarter of the input (measured on MobileNet-v1
-            // b=256 through tb200_graph_run: 1.78 ms vs 1.92 ms for two halves; three-way splits 1.85-1.87 ms)
-            const int a = ((Ntot / 4 + 7) / 8) * 8;
-            cfirst = {0, a}, ccount = {a, Ntot - a};
-        }
-        // TB200_PIPELINE_SPLIT="40,88,128": explicit (uneven) chunk sizes in images -- a small first chunk shortens the time the
-        // kernels wait for the first H2D copy; must sum to the batch
-        if (const char* ev = getenv("TB200_PIPELINE_SPLIT"))
-        {
-            std::vector<int> sz;
-            int sum = 0;
-            for (const char* p = ev; *p;)
-            {
-                char* end;
-                const long v = strtol(p, &end, 10);
-                if (end == p || v <= 0) break;
-                sz.push_back((int)v), sum += (int)v;
-                p = (*end == ',') ? end + 1 : end;
-            }
-            if (sum == Ntot && sz.size() >= 1 && sz.size() <= 16)
-            {
-                cfirst.clear(), ccount.clear(), K = (int)sz.size();
-                int f = 0;
-                for (int v : sz) cfirst.push_back(f), ccount.push_back(v), f += v;
-            }
-        }
+        K = 2;
+        // from 64 images two chunks of 1/4 and 3/4: the kernels only ever wait for the first quarter of the input (measured on
+        // MobileNet-v1 b=256 through tb200_graph_run: 1.78 ms vs 1.92 ms for two halves; three-way splits 1.85-1.87 ms)
+        const int a = Ntot >= 64 ? ((Ntot / 4 + 7) / 8) * 8 : Ntot / 2;
+        cfirst = {0, a}, ccount = {a, Ntot - a};
     }
     g->chunks = K;
     g->chunk_first = cfirst, g->chunk_count = ccount;
@@ -1566,7 +1535,7 @@ static int fill_concat_steps(const tb200_graph* g, int li, const LayerPlan& P, c
         p.s_in = tk.d.scale, p.z_in = tk.d.zero_point, p.s_out = tout.d.scale, p.z_out = tout.d.zero_point;
         p.c_write = (k + 1 == L.num_inputs) ? tout.cp - coff : tk.d.dims[1];
         // vectorised table path when everything is 16-channel aligned; identical quantisation -> no table at all
-        p.scale = (tk.d.dims[1] % 16 == 0 && coff % 16 == 0 && !getenv("TB200_CONCAT_BYTEWISE")) ? 1 : 0;
+        p.scale = (tk.d.dims[1] % 16 == 0 && coff % 16 == 0) ? 1 : 0;
         p.w = (tk.d.scale == tout.d.scale && tk.d.zero_point == tout.d.zero_point) ? nullptr : g->w_arena + P.blob.w_off + 256 * k;
         coff += tk.d.dims[1];
         if (k + 1 < L.num_inputs) steps.push_back(p);
@@ -1700,7 +1669,7 @@ static int prerun_one(tb200_context* ctx, const tb200_tensor_desc* tensors, int 
     g->layers.assign(layers, layers + num_layers);
     g->layer_kernel.assign(num_layers, kStepName[K_NONE]); // build_steps names every layer that was not folded away
     std::vector<LayerPlan> plan(num_layers);
-    if (!(flags & TB200_PRERUN_NO_GRAPH) && !getenv("TB200_NO_FUSION")) fuse_nodes(layers, tensors, num_tensors, output_ids, num_outputs, g->layers, plan);
+    if (!(flags & TB200_PRERUN_NO_GRAPH)) fuse_nodes(layers, tensors, num_tensors, output_ids, num_outputs, g->layers, plan);
     int rc;
     if ((rc = setup_tensors(g, tensors, num_tensors, input_ids, num_inputs, output_ids, num_outputs)) != 0) return rc;
     if ((rc = plan_kernels(g, plan)) != 0) return rc;
@@ -1729,8 +1698,7 @@ static int prerun_one(tb200_context* ctx, const tb200_tensor_desc* tensors, int 
 // Returns true when [p, p+bytes) is page-locked.  Failure is not an error: the copy then takes the driver's pageable path.
 static bool host_pin(tb200_context* root, const void* ptr, size_t bytes)
 {
-    static const bool off = getenv("TB200_NO_HOST_REGISTER") != nullptr;
-    if (off || !ptr || !bytes) return false;
+    if (!ptr || !bytes) return false;
     const uint8_t* p = (const uint8_t*)ptr;
     for (const HostReg& r : root->host_regs)
         if (p >= r.p && p + bytes <= r.p + r.bytes) return true;

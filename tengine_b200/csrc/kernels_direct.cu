@@ -825,7 +825,7 @@ __global__ void __launch_bounds__(256) pool_max_same_scale_kernel(const uint4* _
 
 cudaError_t launch_pool(const void* in, void* out, const PoolShape& p, bool u8, cudaStream_t st)
 {
-    if (p.method == TB200_POOL_MAX && (p.lut || (p.in_scale == p.out_scale && (!u8 || p.in_zero == p.out_zero) && !getenv("TB200_POOL_EXACT"))))
+    if (p.method == TB200_POOL_MAX && (p.lut || (p.in_scale == p.out_scale && (!u8 || p.in_zero == p.out_zero))))
     {
         const long long tot = (long long)p.n * p.oh * p.ow * (p.cp / 16);
         TB200_CHECK_32BIT(tot * 16);
@@ -860,8 +860,7 @@ __global__ void __launch_bounds__(256) relu_same_scale_kernel(const uint4* __res
 cudaError_t launch_pointwise(const void* a, const void* b, void* out, long long bytes, const PointwiseParams& p, bool u8, cudaStream_t st)
 {
     const long long nvec = bytes / 16;
-    if (p.mode == 0 && p.negative_slope == 0.f && p.scale0 == p.out_scale && (!u8 || (p.zero0 == p.out_zero && p.c == p.cp)) &&
-        !getenv("TB200_POINTWISE_EXACT"))
+    if (p.mode == 0 && p.negative_slope == 0.f && p.scale0 == p.out_scale && (!u8 || (p.zero0 == p.out_zero && p.c == p.cp)))
     {
         const unsigned grid = (unsigned)blocks_for(nvec, 256);
         if (u8) relu_same_scale_kernel<true><<<grid, 256, 0, st>>>((const uint4*)a, (uint4*)out, nvec, (uint32_t)(p.out_zero & 0xff) * 0x01010101u);
@@ -877,8 +876,7 @@ cudaError_t launch_pointwise(const void* a, const void* b, void* out, long long 
         else if (p.mode == 1) tmax = in0 * (a0 + a1) / so;
         else tmax = in0 * a0 * in0 * a1 / so;
         const bool slope_ok = p.mode != 0 || (p.negative_slope >= 0.f && p.negative_slope < 1.f);
-        static const bool off = getenv("TB200_POINTWISE_EXACT") != nullptr;
-        if (!off && so > 1e-30 && so < 1e30 && tmax + 256.0 < 32000.0 && slope_ok && p.c >= 16)
+        if (so > 1e-30 && so < 1e30 && tmax + 256.0 < 32000.0 && slope_ok && p.c >= 16)
         {
             PointwiseFast q;
             q.r_out = 1.0f / p.out_scale;

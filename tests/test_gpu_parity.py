@@ -346,28 +346,36 @@ def test_eltwise_relu_fusion_is_used_and_exact(ctx, oracle):
 
 
 def test_pipelined_run_equals_unpipelined(ctx):
-    """tb200_graph_run cuts the batch into chunks and overlaps H2D / kernels / D2H; same bytes as the single-chunk plan."""
-    import os
+    """tb200_graph_run cuts the batch into chunks and overlaps H2D / kernels / D2H: two halves at batch 32, 16 + 48 images at
+    batch 64.  Same bytes as the whole-batch graph (upload / launch / download) and as one chunk without capture (NO_GRAPH).
+    Every graph runs twice: buffers are reused."""
     from tengine_b200 import runtime as rt
 
-    g, b = workloads.mobilenet_v1(abi.DT_INT8, batch=32, res=96, width=0.5, classes=50)
+    g64, b = workloads.mobilenet_v1(abi.DT_INT8, batch=64, res=96, width=0.5, classes=50)
+    g32, _ = workloads.mobilenet_v1(abi.DT_INT8, batch=32, res=96, width=0.5, classes=50)
     x = b.random_input(7)
+
+    def run(gr):
+        return gr.run([x])[0]
+
+    def halves(gr):  # the batch-32 graph over each half of x
+        return np.concatenate([gr.run([x[:32]])[0], gr.run([x[32:]])[0]])
+
+    def launch(gr):
+        y = np.empty(g64.dims(g64.outputs[0]), g64.np_dtype)
+        gr.upload(0, x)
+        gr.launch()
+        gr.download(0, y)
+        gr.sync()
+        return y
+
+    ways = [(g64, abi.PRERUN_NO_GRAPH, run), (g64, abi.PRERUN_DEFAULT, run), (g64, abi.PRERUN_DEFAULT, launch), (g32, abi.PRERUN_DEFAULT, halves)]
     outs = []
-    for chunks in ("1", "4", "2"):
-        os.environ["TB200_PIPELINE_CHUNKS"] = chunks
+    for g, flags, way in ways:
+        gr = rt.Graph(ctx, g, flags)
         try:
-            gr = rt.Graph(ctx, g)
-            outs.append(gr.run([x])[0])
-            outs.append(gr.run([x])[0])  # twice: buffers are reused
-            gr.close()
+            outs += [way(gr), way(gr)]
         finally:
-            os.environ.pop("TB200_PIPELINE_CHUNKS", None)
-    os.environ["TB200_PIPELINE_SPLIT"] = "5,11,16"  # uneven chunks
-    try:
-        gr = rt.Graph(ctx, g)
-        outs.append(gr.run([x])[0])
-        gr.close()
-    finally:
-        os.environ.pop("TB200_PIPELINE_SPLIT", None)
+            gr.close()
     for o in outs[1:]:
         assert np.array_equal(o, outs[0])

@@ -66,6 +66,39 @@ def test_zero_point_placement_matters_at_negative_ties():
         assert (r.exact() != r.zp_swapped()).sum() >= 8, case.name
 
 
+def _pointwise_kernel(g, L):
+    """The kernel launch_pointwise runs for a ReLU / eltwise layer: the same-scale ReLU (kernels_direct.cu:863), the fast kernel
+    whose value range is proven (:879), else the literal per-element pointwise_kernel."""
+    u8 = g.data_type == abi.DT_UINT8
+    t0, to = g.tensors[L["inputs"][0]], g.tensors[L["output"]]
+    c = t0["dims"][1]
+    s0, so, slope = np.float32(t0["scale"]), np.float32(to["scale"]), np.float32(L["negative_slope"])
+    mode, s1 = 0, np.float32(0)
+    if L["op"] == abi.OP_ELTWISE:
+        mode, s1 = (1 if L["elt_type"] == abi.ELT_SUM else 2), np.float32(g.tensors[L["inputs"][1]]["scale"])
+    if mode == 0 and slope == 0 and s0 == so and (not u8 or (t0["zero_point"] == to["zero_point"] and c % 16 == 0)):
+        return "relu_same_scale_kernel"
+    in0, a0, a1, so = (255.0 if u8 else 128.0), abs(float(s0)), abs(float(s1)), float(so)
+    tmax = (in0 * a0 / so, in0 * (a0 + a1) / so, in0 * a0 * in0 * a1 / so)[mode]
+    if 1e-30 < so < 1e30 and tmax + 256.0 < 32000.0 and (mode != 0 or 0 <= slope < 1) and c >= 16:
+        return "pointwise_fast_kernel"
+    return "pointwise_kernel"
+
+
+def test_pointwise_cases_reach_their_kernels():
+    """The *_pwexact cases of the device tie tests reach the literal pointwise_kernel by their channel count, the other ReLU /
+    eltwise cases a fast kernel; all of them are tie-dense."""
+    from tests.test_gpu_requant_ties import CASES as DEVICE_CASES, build
+
+    names = [n for n in DEVICE_CASES if n.startswith(("eltwise_", "relu_", "leaky_relu_"))]
+    assert sum(n.endswith("_pwexact") for n in names) == 6
+    for name in names:
+        case, _ = build(name)
+        assert (_pointwise_kernel(case.g, case.g.layers[0]) == "pointwise_kernel") == name.endswith("_pwexact"), name
+        _, rs = ties.exact_run(case.g, case.inputs)
+        ties.check_not_vacuous(case, rs[case.g.outputs[0]])
+
+
 @pytest.mark.parametrize("case", CASES, ids=lambda c: c.name)
 def test_oracle_equals_unmodified_reference(reference, oracle, case):
     want = oracle.run(case.g, case.inputs, uint8_mode=0)

@@ -59,7 +59,6 @@ VARIANTS = {  # name -> (devices as a function of n, net, extra environment)
     "nccl_yolo_u8": (lambda n: list(range(n)), "yolo", {}),
     "memcpy_peer_mobilenet": (lambda n: list(range(n)), "mobilenet", {"TB200_NO_NCCL": "1"}),
     "gpu1_alone": (lambda n: [1], "mobilenet", {}),
-    "nccl_inline_fix": (lambda n: list(range(n)), "mobilenet", {"TB200_NO_FIXQ": "1"}),
     "nccl_no_graph_capture": (lambda n: list(range(n)), "mobilenet", {"DEBUG_MULTI_FLAGS": "nograph"}),
 }
 

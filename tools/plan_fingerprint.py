@@ -7,7 +7,7 @@ plan, pack and compute alike print identical output, so a change to the planner 
     TB200_LIB=/path/to/parent.so python tools/plan_fingerprint.py > parent.jsonl
     python tools/plan_fingerprint.py > new.jsonl && cmp parent.jsonl new.jsonl
 
-Run each library in its own process: the library reads its environment switches once per process.  Needs an H100.
+Needs an H100.
 """
 import hashlib
 import json
