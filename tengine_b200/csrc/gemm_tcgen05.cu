@@ -1,4 +1,4 @@
-// gemm_tcgen05.cu -- int8 x int8 -> int32 GEMM on the Hopper tensor cores (wgmma.mma_async .s32.s8/.u8, m64n16k32)
+// gemm_tcgen05.cu -- int8 x int8 -> int32 GEMM on the Hopper tensor cores (wgmma.mma_async .s32.s8/.u8, m64nNk32, N = block_n)
 // with TMA-staged operands, a shared-memory accumulator image and the fused requantising epilogue.
 //
 //   out[m][oc] = requant( sum_k A[m][k] * B[oc][k] ),   A = NHWC activations (row = pixel, K = padded Cin),
@@ -7,18 +7,23 @@
 // (source/device/cpu/op/conv/x86/conv_kernel_x86.c:187-242, 1008-1631, 1796-1893) and of ref_fc_int8
 // (fc/fc_ref.c:209-297): with NHWC activations a 1x1 convolution IS this GEMM, no im2col pass exists.
 //
-// Structure (one persistent CTA per SM, 544 threads):
-//   warp 16   : TMA producer  (cp.async.bulk.tensor.2d -> 128B/64B/32B-swizzled smem ring, mbarrier expect_tx)
-//   warps 0-15: four warpgroups that first multiply, then requantise.  MMA: warpgroup w takes rows 64*(w & 1).. and one
-//               half of the N tile's 16-column chunks, issues wgmma per ring stage, releases the stage after
-//               wgmma.wait_group and finally writes its s32 fragments into the accumulator image ([128 rows][BN] in
-//               shared memory).  Epilogue: four warps per 32-row quarter of the image; a warp owns whole "store groups"
-//               = 32 rows x 16/32 channels: image -> registers -> requant_fast4_i8 -> bytes -> its own swizzled smem
-//               buffer -> ONE TMA store per group (cp.async.bulk.tensor, double-buffered).  No address arithmetic for the
-//               stores, rows outside the tensor are clipped by the TMA unit.
-// The producer runs ahead through the ring while the epilogue works, so the next tile's operands are resident when its
-// MMAs start.  K is small (32..1024), so these layers are bound by the epilogue's ALU-pipe issue rate, not by the tensor
-// pipe: see common.cuh (requant_fast4_i8) for the instruction budget.
+// Structure (one persistent CTA per SM, 512 threads = four warpgroups, int8 and uint8 alike):
+//   WG0, warp 0   : TMA producer  (cp.async.bulk.tensor.2d -> 128B/64B/32B-swizzled smem ring, mbarrier expect_tx)
+//   WG0, warps 1-2: uint8 only: the row sums sum(x) of every A tile (idle for int8); warp 3 idle
+//   WG1, warps 4-7: MMA.  One accumulator stage (mt m-tiles x block_n columns) in registers: per m-tile and k-step two
+//                   m64n<block_n>k32, rows 0-63 and 64-127; one commit group in flight, a ring stage is released when the
+//                   group after it has been committed and the one reading it has completed.  At the end of the stage the
+//                   fragments go into the accumulator image ([128 rows][mt * block_n] s32 in shared memory) as soon as the
+//                   epilogue has read the previous stage out of it (mbarriers img_empty / img_full).
+//   WG2-3, warps 8-15: epilogue.  Two warps per 32-row quarter of the image; a warp owns whole "store groups" = 32 rows x
+//                   16/32 channels: image -> registers -> requant_fast4_i8 -> bytes -> its own swizzled smem buffer -> ONE
+//                   TMA store per group (cp.async.bulk.tensor, double-buffered).  No address arithmetic for the stores,
+//                   rows outside the tensor are clipped by the TMA unit.
+// So the tensor cores multiply stage s+1 while the epilogue requantises stage s: the registers are the second accumulator
+// buffer.  Registers per thread (setmaxnreg): WG0 40, MMA 200 (at most 128 accumulators), epilogue 136.
+// The producer runs ahead through the ring, so the next tile's operands are resident when its MMAs start.  K is small
+// (32..1024), so these layers are bound by the epilogue's ALU-pipe issue rate, not by the tensor pipe: see common.cuh
+// (requant_fast4_i8) for the instruction budget.
 #include <cuda.h>
 
 #include "common.cuh"
@@ -32,20 +37,27 @@
 namespace tb200 {
 
 #ifdef TB200_GEMM_TIMELINE
-#define TLOG_E(tag) do { if (lane == 0 && (warp == 0 || warp == 15)) tlog(warp == 0 ? 2 : 3, tag); } while (0)
+#define TLOG_E(tag) do { if (lane == 0 && (warp == EPI_WARP0 || warp == 15)) tlog(warp == EPI_WARP0 ? 2 : 3, tag); } while (0)
 #else
 #define TLOG_E(tag) do { } while (0)
 #endif
 
 
-static constexpr int EPI_WARPS = 16; // four warpgroups; four warps per 32-row quarter of the accumulator image
-static constexpr int EPI_THREADS = EPI_WARPS * 32;
-static constexpr int GEMM_THREADS = 32 + EPI_THREADS;
-static constexpr int SUM_WARP0 = EPI_WARPS + 1, SUM_WARPS = 2; // uint8 kernels only: two warps that add up the rows of every A tile (sum x)
-static constexpr int GEMM_THREADS_U8 = GEMM_THREADS + 32 * SUM_WARPS;
-static constexpr int PRODUCER_WARP = EPI_WARPS;
+// warp roles (four warpgroups, int8 and uint8 alike)
+static constexpr int GEMM_THREADS = 512;
+static constexpr int PRODUCER_WARP = 0;
+static constexpr int SUM_WARP0 = 1, SUM_WARPS = 2; // uint8 kernels only: two warps that add up the rows of every A tile (sum x)
+static constexpr int MMA_THREAD0 = 128;            // the MMA warpgroup: threads 128..255
+static constexpr int EPI_WARP0 = 8, EPI_WARPS = 8; // two epilogue warpgroups; two warps per 32-row quarter of the accumulator image
+static constexpr int EPI_THREAD0 = EPI_WARP0 * 32, EPI_THREADS = EPI_WARPS * 32;
+// registers per thread of each role (setmaxnreg): the kernel launches with 128 (512 threads, the 64 K registers of the SM); WG0
+// gives registers back, the MMA warpgroup (up to 128 accumulators) and the epilogue warpgroups take them
+static constexpr int REG_LAUNCH = 128, REG_WG0 = 40, REG_MMA = 200, REG_EPI = 136;
+static_assert(REG_WG0 + REG_MMA + 2 * REG_EPI == 4 * REG_LAUNCH, "the register split must fill the register file");
 static constexpr int ACC_COLS_MAX = 128; // columns of the accumulator image (m-tiles per stage x block_n)
-static constexpr int MMA_CHUNKS = 4;     // 16-column chunks of one warpgroup: half of at most 128 columns
+// staging warps the planner budgets shared memory for: the ring depth and the resident-B decision were made against a 16-warp
+// epilogue, and keeping that budget keeps every plan as it was
+static constexpr int PLAN_STG_WARPS = 16;
 static constexpr int PAR_MAX = 2048; // channels whose epilogue constants stay resident in smem for the whole kernel
 static constexpr int MAX_STAGES = 24;
 static constexpr int B_RESIDENT_MAX = 96 * 1024; // weights of the CTA's N tile stay in smem when they fit in this many bytes
@@ -113,15 +125,17 @@ struct __align__(16) GemmSmemCtl
     uint64_t full[MAX_STAGES], empty[MAX_STAGES];
     uint64_t b_full; // resident-B mode: all k-blocks of the N tile's weights have landed
     uint64_t sx_full[2], sx_empty[2]; // uint8 row sums of stage s published by the row-sum warps / read by the epilogue
+    uint64_t img_full, img_empty;     // the accumulator image holds a complete stage (MMA -> epilogue) / has been read (epilogue -> MMA)
 };
 
+// named barrier 1 over the epilogue warps only (the MMA warpgroup never joins it)
 __device__ __forceinline__ void epilogue_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory"); }
 
 // ---- the rare path of the fast epilogue, deferred -----------------------------------------------------------------------------
 // An element whose t sits inside the tie guard needs the literal reference arithmetic (common.cuh requant(): divisions, per-channel
 // loads, every recipe).  Done inline it occupies ONE lane of an epilogue warp for hundreds of cycles while the other fifteen warps
 // finish their groups and then wait for it at the stage hand-over.  Instead the lane appends {m-tile, row, channel, accumulator} to the CTA's queue in
-// global memory (L2) and carries on with the fast byte; after the CTA's last tile all 512 epilogue threads recompute the queued
+// global memory (L2) and carries on with the fast byte; after the CTA's last tile all 256 epilogue threads recompute the queued
 // elements in parallel and patch the bytes in the output tensor (the tile's TMA store has completed by then).  A full or absent
 // queue falls back to the inline computation, so the result never depends on the queue.
 // (queue state in static shared memory, so that the rare-path functions need no extra arguments: passing the kernel arguments and a
@@ -173,12 +187,13 @@ __device__ __noinline__ uint32_t gemm_fix_word(uint32_t word, int32_t a0, int32_
     return word;
 }
 
-// After the CTA's last tile (every epilogue warp has waited for its own bulk stores): recompute the queued elements, one per thread.
+// After the CTA's last tile (every epilogue warp has waited for its own bulk stores): recompute the queued elements, one per epilogue
+// thread.
 template <bool U8>
 __device__ __forceinline__ void fixq_drain(const GemmArgs& g, const EpiParams& e)
 {
     const uint32_t n = s_fixq.count < s_fixq.cap ? s_fixq.count : s_fixq.cap;
-    for (uint32_t k = threadIdx.x; k < n; k += EPI_THREADS)
+    for (uint32_t k = threadIdx.x - EPI_THREAD0; k < n; k += EPI_THREADS)
     {
         const uint4 q = s_fixq.q[k];
         const int mt = (int)q.x, r = (int)(q.y & 127u), oc = (int)(q.y >> 8);
@@ -354,10 +369,114 @@ __device__ __forceinline__ uint32_t padding_taps(const GemmArgs& g, int mt, int 
     return (uint32_t)(((a * (khn + 1) + b) * (g.pad_w + 1) + c) * (g.kw_n + 1) + d);
 }
 
+// ---- the MMA warpgroup ---------------------------------------------------------------------------------------------------------
+// One accumulator stage (MT m-tiles x BN columns, MT * BN <= ACC_COLS_MAX) is computed in registers: per m-tile and k-step two
+// m64nBNk32, rows 0-63 and 64-127, into MT * BN s32 registers per thread.  One commit group per k-block stays in flight: after
+// committing k-block kb the warpgroup waits for the group of kb - 1 and releases the ring stage that group read; the pipe is
+// drained (wait_group 0) only at the end of the stage.  The registers are the second accumulator buffer: while this stage is
+// multiplied the epilogue drains the previous one from the image; the fragments are then written into the image once every
+// epilogue warp has read it (img_empty) and published with img_full.  BN, MT and the operand signs are template parameters so
+// that the accumulators are indexed statically and no wgmma sits in a branch the compiler cannot prove uniform.
+template <bool AU, bool BU, int BN, int MT, typename Log>
+__device__ __forceinline__ void gemm_mma(const GemmArgs& g, GemmSmemCtl* ctl, uint8_t* smem, uint32_t stage_bytes, uint32_t b_res_base,
+                                         uint32_t img_base, uint32_t img_pitch, Log&& tlog)
+{
+    constexpr int NR = BN / 2; // registers of one m64nBN fragment
+    uint32_t acc[MT][2][NR];
+#pragma unroll
+    for (int i = 0; i < MT; i++)
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+#pragma unroll
+            for (int r = 0; r < NR; r++) acc[i][h][r] = 0;
+    const bool elected = threadIdx.x == MMA_THREAD0; // arrives on the ring's empty barriers for the warpgroup
+    const uint32_t a_bytes = BLOCK_M * g.block_k, b_al = (BN * g.block_k + 1023) & ~1023u;
+    const int ks = g.block_k / 32;
+    const uint64_t half = (uint64_t)((64 * g.swizzle) >> 4); // A rows 64.. in descriptor units (16 bytes)
+    int stage = 0, held = -1; // held: the ring stage the group in flight reads
+    uint32_t phase = 0, iphase = 0;
+    if (g.b_res) mbar_wait(&ctl->b_full, 0);
+    for (int st = blockIdx.x; st < g.num_super; st += gridDim.x)
+    {
+        const int rem = g.m_tiles - (st / g.n_tiles) * MT;
+        const int mtc = rem < MT ? rem : MT;
+#pragma unroll
+        for (int i = 0; i < MT; i++)
+        {
+            if (i >= mtc) break;
+            for (int kb = 0; kb < g.k_blocks; kb++)
+            {
+                mbar_wait(&ctl->full[stage], phase); // TMA bytes have landed
+                const uint32_t sa = smem_u32(smem + (size_t)stage * stage_bytes);
+                const uint32_t sb = g.b_res ? b_res_base + (uint32_t)kb * b_al : sa + a_bytes;
+                const uint64_t da = make_smem_desc(sa, g.swizzle), db = make_smem_desc(sb, g.swizzle);
+                wgmma_fence();
+                for (int k = 0; k < ks; k++)
+                {
+                    // +32 bytes along K inside the swizzled rows: +2 in 16-byte units; the first k-step of the tile overwrites
+                    const uint32_t accumulate = (kb | k) != 0;
+                    wgmma_m64<BN, AU, BU>(acc[i][0], da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), accumulate);
+                    wgmma_m64<BN, AU, BU>(acc[i][1], da + half + (uint64_t)(k * 2), db + (uint64_t)(k * 2), accumulate);
+                }
+                wgmma_commit();
+                wgmma_wait<1>(); // the previous group has completed: the ring stage it read may be refilled
+                if (held >= 0 && elected) mbar_arrive(&ctl->empty[held]);
+                held = stage;
+                if (++stage == g.stages) stage = 0, phase ^= 1;
+            }
+        }
+        wgmma_wait<0>();
+        if (elected) mbar_arrive(&ctl->empty[held]);
+        held = -1;
+#pragma unroll
+        for (int i = 0; i < MT; i++)
+#pragma unroll
+            for (int h = 0; h < 2; h++)
+#pragma unroll
+                for (int r = 0; r < NR; r++) reg_fence(acc[i][h][r]);
+        tlog(1, 0);
+        mbar_wait(&ctl->img_empty, iphase ^ 1); // every epilogue warp has read the previous stage out of the image
+        tlog(1, 1);
+#pragma unroll
+        for (int i = 0; i < MT; i++)
+        {
+            if (i >= mtc) break;
+#pragma unroll
+            for (int h = 0; h < 2; h++)
+#pragma unroll
+                for (int c = 0; c < BN / 16; c++)
+                    frag_to_image(*reinterpret_cast<const uint32_t(*)[8]>(&acc[i][h][8 * c]), img_base, img_pitch, h * 64, i * BN + c * 16);
+        }
+        __syncwarp();
+        if ((threadIdx.x & 31) == 0) mbar_arrive(&ctl->img_full); // (release) this warp's rows of the stage are in the image
+        tlog(1, 2);
+        iphase ^= 1;
+    }
+}
+
+// (block_n, m-tiles per stage) of the launch -> the MMA warpgroup's code for it; uniform across the CTA
+template <bool AU, bool BU, typename Log>
+__device__ __forceinline__ void gemm_mma_dispatch(const GemmArgs& g, GemmSmemCtl* ctl, uint8_t* smem, uint32_t stage_bytes, uint32_t b_res_base,
+                                                  uint32_t img_base, uint32_t img_pitch, Log&& tlog)
+{
+#define TB200_MMA_CASE(BN, MT)                                                                                                 \
+    case BN * 4 + MT - 1: gemm_mma<AU, BU, BN, MT>(g, ctl, smem, stage_bytes, b_res_base, img_base, img_pitch, tlog); break;
+    switch (g.block_n * 4 + g.mt - 1)
+    {
+        TB200_MMA_CASE(16, 1) TB200_MMA_CASE(16, 2) TB200_MMA_CASE(16, 4)
+        TB200_MMA_CASE(32, 1) TB200_MMA_CASE(32, 2) TB200_MMA_CASE(32, 4)
+        TB200_MMA_CASE(48, 1) TB200_MMA_CASE(48, 2)
+        TB200_MMA_CASE(64, 1) TB200_MMA_CASE(64, 2)
+        TB200_MMA_CASE(80, 1) TB200_MMA_CASE(96, 1) TB200_MMA_CASE(112, 1) TB200_MMA_CASE(128, 1)
+        default: __trap(); // plan_stage never makes another (block_n, mt)
+    }
+#undef TB200_MMA_CASE
+}
+
 // MODE: 0 fast epilogue, 1 fast epilogue with the bias folded into the FMA (int8 only), 2 exact epilogue.
 // CS: 16-column chunks per store group (1 or 2).  Compile-time so that each kernel carries exactly one epilogue body.
 template <bool U8, int MODE, int CS, bool BORDER>
-__global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
     gemm_i8_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                            const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap tmap_out_tail,
                            const GemmArgs g, const __grid_constant__ EpiParams e)
@@ -396,85 +515,89 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
     if (threadIdx.x == 0)
     {
         const uint32_t sumw = (U8 && g.cplane) ? SUM_WARPS : 0; // the row-sum warps read every operand stage and publish with the accumulators
-        for (int s = 0; s < g.stages; s++) mbar_init(&ctl->full[s], 1), mbar_init(&ctl->empty[s], EPI_WARPS + sumw);
+        for (int s = 0; s < g.stages; s++) mbar_init(&ctl->full[s], 1), mbar_init(&ctl->empty[s], 1 + sumw);
         for (int s = 0; s < 2; s++) mbar_init(&ctl->sx_full[s], sumw ? sumw : 1), mbar_init(&ctl->sx_empty[s], EPI_WARPS);
         mbar_init(&ctl->b_full, 1);
+        mbar_init(&ctl->img_full, 4), mbar_init(&ctl->img_empty, EPI_WARPS);
         s_fixq.q = g.fixq ? g.fixq + (size_t)blockIdx.x * g.fixq_cap : nullptr, s_fixq.cap = (uint32_t)g.fixq_cap, s_fixq.count = 0;
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
 
-    if (warp == PRODUCER_WARP)
+    // the warpgroup index, broadcast from lane 0 so that the compiler sees the role branches as warp-uniform
+    const int wg = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0);
+    if (wg == 0)
     {
-        // ===================== TMA producer =====================
-        if (lane == 0)
+        setmaxnreg_dec<REG_WG0>();
+        if (warp == PRODUCER_WARP)
         {
-            asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_a)) : "memory");
-            asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_b)) : "memory");
-            int stage = 0;
-            uint32_t phase = 0;
-            if (g.b_res)
+            // ===================== TMA producer =====================
+            if (lane == 0)
             {
-                // the grid is a multiple of n_tiles, so this CTA only ever sees N tile blockIdx.x % n_tiles: load its
-                // weights (every k-block) once
-                const int nb = (blockIdx.x % g.n_tiles) * g.block_n;
-                mbar_expect_tx(&ctl->b_full, (uint32_t)g.k_blocks * b_bytes);
-                for (int kb = 0; kb < g.k_blocks; kb++)
+                asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_a)) : "memory");
+                asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_b)) : "memory");
+                int stage = 0;
+                uint32_t phase = 0;
+                if (g.b_res)
                 {
-                    const int kc = g.conv ? (kb / g.cblocks) * g.cp + (kb % g.cblocks) * g.block_k : kb * g.block_k;
-                    tma_load_2d(&tmap_b, &ctl->b_full, b_region + (size_t)kb * b_al, kc, nb);
-                }
-            }
-            for (int st = blockIdx.x; st < g.num_super; st += gridDim.x)
-            {
-                const int msup = st / g.n_tiles;
-                const int mt0 = msup * g.mt;
-                const int ntile = st - msup * g.n_tiles;
-                const int n0 = ntile * g.block_n; // row of this N tile in the packed weight matrix
-                for (int i = 0; i < g.mt && mt0 + i < g.m_tiles; i++)
-                {
-                    const int m0 = (mt0 + i) * BLOCK_M;
-                    int cn0 = 0, coh0 = 0, cow0 = 0;
-                    if (g.conv) tile_origin(g, mt0 + i, cn0, coh0, cow0);
+                    // the grid is a multiple of n_tiles, so this CTA only ever sees N tile blockIdx.x % n_tiles: load its
+                    // weights (every k-block) once
+                    const int nb = (blockIdx.x % g.n_tiles) * g.block_n;
+                    mbar_expect_tx(&ctl->b_full, (uint32_t)g.k_blocks * b_bytes);
                     for (int kb = 0; kb < g.k_blocks; kb++)
                     {
-                        mbar_wait(&ctl->empty[stage], phase ^ 1);
-                        uint8_t* sa = smem + (size_t)stage * stage_bytes;
-                        if (!g.conv)
+                        const int kc = g.conv ? (kb / g.cblocks) * g.cp + (kb % g.cblocks) * g.block_k : kb * g.block_k;
+                        tma_load_2d(&tmap_b, &ctl->b_full, b_region + (size_t)kb * b_al, kc, nb);
+                    }
+                }
+                for (int st = blockIdx.x; st < g.num_super; st += gridDim.x)
+                {
+                    const int msup = st / g.n_tiles;
+                    const int mt0 = msup * g.mt;
+                    const int ntile = st - msup * g.n_tiles;
+                    const int n0 = ntile * g.block_n; // row of this N tile in the packed weight matrix
+                    for (int i = 0; i < g.mt && mt0 + i < g.m_tiles; i++)
+                    {
+                        const int m0 = (mt0 + i) * BLOCK_M;
+                        int cn0 = 0, coh0 = 0, cow0 = 0;
+                        if (g.conv) tile_origin(g, mt0 + i, cn0, coh0, cow0);
+                        for (int kb = 0; kb < g.k_blocks; kb++)
                         {
-                            mbar_expect_tx(&ctl->full[stage], a_bytes + (g.b_res ? 0u : b_bytes));
-                            tma_load_2d(&tmap_a, &ctl->full[stage], sa, kb * g.block_k, m0);
-                            if (!g.b_res) tma_load_2d(&tmap_b, &ctl->full[stage], sa + a_bytes, kb * g.block_k, n0);
+                            mbar_wait(&ctl->empty[stage], phase ^ 1);
+                            uint8_t* sa = smem + (size_t)stage * stage_bytes;
+                            if (!g.conv)
+                            {
+                                mbar_expect_tx(&ctl->full[stage], a_bytes + (g.b_res ? 0u : b_bytes));
+                                tma_load_2d(&tmap_a, &ctl->full[stage], sa, kb * g.block_k, m0);
+                                if (!g.b_res) tma_load_2d(&tmap_b, &ctl->full[stage], sa + a_bytes, kb * g.block_k, n0);
+                            }
+                            else
+                            {
+                                // k-block = (filter tap, channel block): the A tile is the output patch shifted by the tap;
+                                // coordinates outside the image are zero-filled by the TMA unit = the convolution's padding
+                                const int tap = kb / g.cblocks, cb = kb - tap * g.cblocks;
+                                const int kh = tap / g.kw_n, kw = tap - kh * g.kw_n;
+                                mbar_expect_tx(&ctl->full[stage], g.a_tx_bytes + (g.b_res ? 0u : b_bytes));
+                                tma_load_4d(&tmap_a, &ctl->full[stage], sa, cb * g.block_k, cow0 * g.cstride - g.pad_w + kw,
+                                            coh0 * g.cstride - g.pad_h + kh, cn0);
+                                if (!g.b_res) tma_load_2d(&tmap_b, &ctl->full[stage], sa + a_bytes, tap * g.cp + cb * g.block_k, n0);
+                            }
+                            tlog(0, kb & 0xff);
+                            if (++stage == g.stages) stage = 0, phase ^= 1;
                         }
-                        else
-                        {
-                            // k-block = (filter tap, channel block): the A tile is the output patch shifted by the tap;
-                            // coordinates outside the image are zero-filled by the TMA unit = the convolution's padding
-                            const int tap = kb / g.cblocks, cb = kb - tap * g.cblocks;
-                            const int kh = tap / g.kw_n, kw = tap - kh * g.kw_n;
-                            mbar_expect_tx(&ctl->full[stage], g.a_tx_bytes + (g.b_res ? 0u : b_bytes));
-                            tma_load_4d(&tmap_a, &ctl->full[stage], sa, cb * g.block_k, cow0 * g.cstride - g.pad_w + kw,
-                                        coh0 * g.cstride - g.pad_h + kh, cn0);
-                            if (!g.b_res) tma_load_2d(&tmap_b, &ctl->full[stage], sa + a_bytes, tap * g.cp + cb * g.block_k, n0);
-                        }
-                        tlog(0, kb & 0xff);
-                        if (++stage == g.stages) stage = 0, phase ^= 1;
                     }
                 }
             }
         }
-    }
-    else if (U8 && warp >= SUM_WARP0)
-    {
-        // ===================== row sums (uint8, warps 18 and 19) =====================
-        // sum x*(w - zw) = sum x*(w - 128) [tensor cores, B signed] + (128 - zw) * sum(x).  sum(x) of output row r is the sum of ALL bytes
-        // of row r of every A tile of the m-tile (taps outside the image were zero-filled by the TMA unit, K tails too), and a sum
-        // does not care about the swizzle that permutes the 16-byte chunks inside a row.  Each of the two warps owns 64 rows (two per
-        // lane), reads them with 16-byte loads (chunk order rotated per lane so that a quarter-warp covers all banks), dp4a against
-        // 0x01010101, and publishes the sums through shared memory together with the accumulator stage.  This keeps the uint8 tiling
-        // identical to the int8 one: no extra B rows, no extra accumulator columns, no second MMA.
-        if (g.cplane)
+        else if (U8 && warp < SUM_WARP0 + SUM_WARPS && g.cplane)
         {
+            // ===================== row sums (uint8, warps 1 and 2) =====================
+            // sum x*(w - zw) = sum x*(w - 128) [tensor cores, B signed] + (128 - zw) * sum(x).  sum(x) of output row r is the sum of ALL bytes
+            // of row r of every A tile of the m-tile (taps outside the image were zero-filled by the TMA unit, K tails too), and a sum
+            // does not care about the swizzle that permutes the 16-byte chunks inside a row.  Each of the two warps owns 64 rows (two per
+            // lane), reads them with 16-byte loads (chunk order rotated per lane so that a quarter-warp covers all banks), dp4a against
+            // 0x01010101, and publishes the sums through shared memory together with the accumulator stage.  This keeps the uint8 tiling
+            // identical to the int8 one: no extra B rows, no extra accumulator columns, no second MMA.
             const int sw = warp - SUM_WARP0;
             const int cpr = g.block_k >> 4;                  // 16-byte chunks per row: 2, 4 or 8
             const int rot = (lane * g.block_k) >> 7;         // lanes whose rows start in the same 128-byte window get different chunks
@@ -517,27 +640,32 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
             }
         }
     }
+    else if (wg == 1)
+    {
+        // ===================== MMA (warps 4..7) =====================
+        setmaxnreg_inc<REG_MMA>();
+        const uint32_t b_res_base = smem_u32(b_region);
+        if (U8 && !g.b_signed) gemm_mma_dispatch<U8, true>(g, ctl, smem, stage_bytes, b_res_base, img_base, img_pitch, tlog);
+        else gemm_mma_dispatch<U8, false>(g, ctl, smem, stage_bytes, b_res_base, img_base, img_pitch, tlog);
+    }
     else
     {
-        // ===================== MMA + epilogue (warps 0..15) =====================
-        // Image quarter q (rows 32q..32q+31) is served by the four warps {q, q+4, q+8, q+12}.  The work of an accumulator
-        // stage is cut into store groups (m-tile i, columns [grp*16*cs, (grp+1)*16*cs)) of 32 rows each, dealt round-robin to
-        // the quarter's warps.  A warp requantises its group chunk by chunk (16 columns per load, the next chunk's load in
-        // flight), writes the bytes to its own swizzled staging buffer and hands the buffer to the TMA unit with one store.
+        // ===================== epilogue (warps 8..15) =====================
+        // Image quarter q (rows 32q..32q+31) is served by the two warps {8 + q, 12 + q}.  The work of an accumulator stage is cut
+        // into store groups (m-tile i, columns [grp*16*cs, (grp+1)*16*cs)) of 32 rows each, dealt round-robin to the quarter's
+        // warps.  A warp requantises its group chunk by chunk (16 columns per load, the next chunk's load in flight), writes the
+        // bytes to its own swizzled staging buffer and hands the buffer to the TMA unit with one store.  It releases the image to
+        // the MMA warpgroup (img_empty) as soon as it has issued its last load of the stage.
+        setmaxnreg_inc<REG_EPI>();
+        const int ew = warp - EPI_WARP0; // epilogue warp 0..7
         const int q = warp & 3;
-        const int sub = warp >> 2;
+        const int sub = ew >> 2;
+        const int et = (int)threadIdx.x - EPI_THREAD0;
         const int ngroups = g.ngroups;
-        // MMA share of this warpgroup (= sub): rows 64*mh.., chunks [c_lo, c_lo + c_n) of every B tile
-        const int mh = sub & 1, nch = g.block_n >> 4, chalf = (nch + 1) >> 1;
-        const int c_lo = (sub >> 1) ? chalf : 0, c_n = (sub >> 1) ? nch - chalf : chalf;
-        const uint32_t a_bytes_mma = BLOCK_M * g.block_k, b_al_mma = (g.block_n * g.block_k + 1023) & ~1023u;
-        int stage = 0;
-        uint32_t phase = 0;
-        if (g.b_res) mbar_wait(&ctl->b_full, 0);
         int qrows = g.rows_valid - q * 32; // rows of this quarter that are output pixels
         qrows = qrows < 0 ? 0 : (qrows > 32 ? 32 : qrows);
         const CUtensorMap* tm_out = (qrows == 32) ? &tmap_out : &tmap_out_tail;
-        const uint32_t buf0 = stg_base + (uint32_t)warp * 2u * buf_bytes;
+        const uint32_t buf0 = stg_base + (uint32_t)ew * 2u * buf_bytes;
         // swizzle of the staging buffer = the output map's swizzle: 16-byte chunk index ^= row bit 2 (Swizzle<1,4,3>, CS 2 only)
         const uint32_t xl = CS == 2 ? (uint32_t)((lane >> 2) & 1) << 4 : 0u;
         const uint32_t row_off = (uint32_t)lane * 16u * CS;
@@ -547,13 +675,13 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
         if (g.par_all)
         {
             // per-channel fast-path constants of every N tile, once; pad / overhanging channels get (0, 0)
-            for (int c = threadIdx.x; c < par_ch; c += EPI_THREADS)
+            for (int c = et; c < par_ch; c += EPI_THREADS)
                 sts_f2(par_base + c * 8, (c < g.ocp && (fast || U8)) ? __ldg(e.fast_par + c) : make_float2(0.f, 0.f));
             epilogue_bar_sync();
         }
         if (lane == 0 && qrows > 0) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tm_out)) : "memory");
         int as = 0;
-        uint32_t aphase = 0;
+        uint32_t aphase = 0, iphase = 0;
         for (int st = blockIdx.x; st < g.num_super; st += gridDim.x)
         {
             const int msup = st / g.n_tiles;
@@ -564,56 +692,21 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
             uint32_t par_s = par_base + (uint32_t)n0 * 8u;
             if (!g.par_all)
             {
-                epilogue_bar_sync(); // every warp is done with the previous tile's constants
-                for (int c = threadIdx.x; c < g.block_n; c += EPI_THREADS)
+                epilogue_bar_sync(); // every epilogue warp is done with the previous tile's constants
+                for (int c = et; c < g.block_n; c += EPI_THREADS)
                     sts_f2(par_base + c * 8, (n0 + c < g.ocp && (fast || U8)) ? __ldg(e.fast_par + n0 + c) : make_float2(0.f, 0.f));
                 epilogue_bar_sync();
                 par_s = par_base;
             }
-            // ---- MMA: every m-tile of the stage into the accumulator image ----
-            epilogue_bar_sync(); // every warp has read the previous stage's image
-            for (int i = 0; i < mtc; i++)
-            {
-                uint32_t acc[MMA_CHUNKS][8];
-#pragma unroll
-                for (int j = 0; j < MMA_CHUNKS; j++)
-#pragma unroll
-                    for (int r = 0; r < 8; r++) acc[j][r] = 0;
-                for (int kb = 0; kb < g.k_blocks; kb++)
-                {
-                    mbar_wait(&ctl->full[stage], phase); // TMA bytes have landed
-                    const uint32_t sa = smem_u32(smem + (size_t)stage * stage_bytes);
-                    const uint32_t sb = g.b_res ? smem_u32(b_region) + (uint32_t)kb * b_al_mma : sa + a_bytes_mma;
-                    const uint64_t da = make_smem_desc(sa + (uint32_t)(mh * 64 * g.swizzle), g.swizzle);
-                    const uint64_t db = make_smem_desc(sb + (uint32_t)(c_lo * 16 * g.swizzle), g.swizzle);
-                    wgmma_fence();
-                    for (int k = 0; k < g.block_k / 32; k++)
-#pragma unroll
-                        for (int j = 0; j < MMA_CHUNKS; j++)
-                            if (j < c_n)
-                            {
-                                // +32 bytes along K inside the swizzled rows: +2 in 16-byte units; +16 rows of B: +16*swizzle bytes
-                                const uint64_t a_d = da + (uint64_t)(k * 2), b_d = db + (uint64_t)(j * g.swizzle + k * 2);
-                                if (U8 && !g.b_signed) wgmma_n16<true, true>(acc[j], a_d, b_d, 1u);
-                                else wgmma_n16<U8, false>(acc[j], a_d, b_d, 1u);
-                            }
-                    wgmma_commit();
-                    wgmma_wait<0>();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&ctl->empty[stage]); // this warp's MMAs have read the stage
-                    if (++stage == g.stages) stage = 0, phase ^= 1;
-                }
-#pragma unroll
-                for (int j = 0; j < MMA_CHUNKS; j++)
-                    if (j < c_n) frag_to_image(acc[j], img_base, img_pitch, mh * 64, i * g.block_n + (c_lo + j) * 16);
-            }
-            epilogue_bar_sync(); // the image is complete
+            mbar_wait(&ctl->img_full, iphase); // the image holds this stage
+            iphase ^= 1;
             if (U8 && g.cplane) mbar_wait(&ctl->sx_full[as], aphase); // the row sums of this stage
             TLOG_E(0);
             const uint32_t tbase = img_base + (uint32_t)(q * 32 + lane) * img_pitch;
+            bool released = false; // this warp has arrived on img_empty for this stage
             if (qrows > 0)
             {
-                // groups of this warp: flattened index u = i * ngroups + grp, u = sub, sub + 4, ...
+                // groups of this warp: flattened index u = i * ngroups + grp, u = sub, sub + 2, ...
                 uint32_t v0[16], v1[16];
                 int i = 0, grp = sub;
                 while (grp >= ngroups) grp -= ngroups, i++;
@@ -621,7 +714,7 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
                     acc_ld16(tbase + 4u * (i * g.block_n + grp * (CS * 16)), reinterpret_cast<uint32_t(&)[16]>(v0));
                 while (i < mtc)
                 {
-                    int i2 = i, g2 = grp + 4; // the group after this one
+                    int i2 = i, g2 = grp + 2; // the group after this one
                     while (g2 >= ngroups) g2 -= ngroups, i2++;
                     const uint32_t buf = buf0 + (ucount & 1u) * buf_bytes;
                     // the store issued two groups ago has finished reading this buffer
@@ -651,9 +744,20 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
                         else if (MODE == 2) epilogue_unit_exact(v, dst, n0 + c, g.oc, e);
                         else epilogue_unit_fast<MODE == 1>(v, par_s + c * 8, dst, n0 + c, (uint32_t)(mt0 + i), e);
                     };
+                    // after the last image load of the stage: (release) the MMA warpgroup may overwrite the image
+                    auto release = [&]()
+                    {
+                        if (i2 >= mtc)
+                        {
+                            __syncwarp();
+                            if (lane == 0) mbar_arrive(&ctl->img_empty);
+                            released = true;
+                        }
+                    };
                     if (CS == 1)
                     {
                         acc_ld16(tg, reinterpret_cast<uint32_t(&)[16]>(v0));
+                        release();
                         unit(reinterpret_cast<const uint32_t(&)[16]>(v0), 0);
                     }
                     else
@@ -665,6 +769,7 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
                             // the next chunk's accumulators are in flight while this one is requantised
                             if (k + 1 < CS) acc_ld16(tg + (k + 1) * 64, reinterpret_cast<uint32_t(&)[16]>(*((k & 1) ? v0 : v1)));
                             else if (i2 < mtc) acc_ld16(tbase + 4u * (i2 * g.block_n + g2 * (CS * 16)), reinterpret_cast<uint32_t(&)[16]>(v0));
+                            if (k + 1 == CS) release();
                             unit(reinterpret_cast<const uint32_t(&)[16]>(*((k & 1) ? v1 : v0)), k);
                             TLOG_E(4);
                         }
@@ -693,7 +798,11 @@ __global__ void __launch_bounds__(U8 ? GEMM_THREADS_U8 : GEMM_THREADS, 1)
                 }
             }
             __syncwarp();
-            if (lane == 0) mbar_arrive(&ctl->sx_empty[as]); // stage drained: the row-sum warps may overwrite its sums
+            if (lane == 0)
+            {
+                if (!released) mbar_arrive(&ctl->img_empty); // a warp without a group in this stage
+                mbar_arrive(&ctl->sx_empty[as]);             // stage drained: the row-sum warps may overwrite its sums
+            }
             TLOG_E(2);
             if (++as == 2) as = 0, aphase ^= 1;
         }
@@ -861,7 +970,7 @@ static int plan_epilogue(GemmPlan* p, const void* out, uint64_t d1, uint64_t d2)
 static int epilogue_smem_bytes(const GemmPlan* p)
 {
     const int par_ch = p->n_tiles * p->block_n;
-    return EPI_WARPS * 2 * 512 * p->cs + (par_ch <= PAR_MAX ? par_ch : p->block_n) * 8 + (int)sizeof(GemmSmemCtl) + 2048 +
+    return PLAN_STG_WARPS * 2 * 512 * p->cs + (par_ch <= PAR_MAX ? par_ch : p->block_n) * 8 + (int)sizeof(GemmSmemCtl) + 2048 +
            128 * (int)acc_pitch(p->mt * p->block_n) + 16;
 }
 
@@ -979,7 +1088,7 @@ int gemm_plan_create_conv(GemmPlan* p, const void* in, const void* w, void* out,
 }
 
 // debug: event timeline of CTA 0 of the launch that just went out (needs a stream that is not being captured).
-// One line per event, sorted by time: cycles since the first event, role (P producer, M mma, E2/E17 epilogue warps), tag.
+// One line per event, sorted by time: cycles since the first event, role (P producer, M mma, E8/E15 epilogue warps), tag.
 static void gemm_trace_report(const GemmPlan& p, const GemmArgs& g, int grid, cudaStream_t st)
 {
     static unsigned long long h[4 * 1024];
@@ -990,9 +1099,9 @@ static void gemm_trace_report(const GemmPlan& p, const GemmArgs& g, int grid, cu
     unsigned long long t0 = ~0ull;
     for (int i = 0; i < 4 * 1024; i++)
         if (h[i] && (h[i] >> 8) < t0) t0 = h[i] >> 8;
-    static const char* role[4] = {"P", "M", "E0", "E15"};
-    static const char* tagM[3] = {"kblock mma issued", "got sx_empty", "commit sx_full"};
-    static const char* tagE[5] = {"got sx_full", "group stored", "arrive sx_empty", "tmem ld done", "unit done"};
+    static const char* role[4] = {"P", "M", "E8", "E15"};
+    static const char* tagM[3] = {"stage multiplied", "got img_empty", "arrive img_full"};
+    static const char* tagE[5] = {"got img_full", "group stored", "arrive sx_empty", "image ld issued", "unit done"};
     for (int r = 0; r < 4; r++)
         for (int i = 0; i < 1024 && h[r * 1024 + i]; i++)
         {
@@ -1061,7 +1170,7 @@ cudaError_t launch_gemm_i8(const GemmPlan& p, const EpiParams& e, const int32_t*
         if (launch_dbg)                                                                                                        \
             fprintf(stderr, "tengine_b200: launch gemm_i8_tcgen05_kernel<U8=%d,MODE=%d,CS=%d,BORDER=%d> out_mode=%d conv=%d n_tiles=%d b_res=%d fixq=%d mt=%d par_all=%d\n", \
                     (int)U, MD, C, (int)B, p.out_mode, p.conv, p.n_tiles, p.b_res, p.fixq != nullptr, p.mt, g.par_all);     \
-        gemm_i8_tcgen05_kernel<U, MD, C, B><<<grid, U ? GEMM_THREADS_U8 : GEMM_THREADS, smem, st>>>(ta, tb, to, tt, g, e);                           \
+        gemm_i8_tcgen05_kernel<U, MD, C, B><<<grid, GEMM_THREADS, smem, st>>>(ta, tb, to, tt, g, e);                                                \
         if (trace_on) gemm_trace_report(p, g, grid, st);                                                                       \
         err = cudaGetLastError();                                                                                              \
         if (launch_dbg || err != cudaSuccess) gemm_launch_debug((const void*)gemm_i8_tcgen05_kernel<U, MD, C, B>, "launch", err, grid, smem, st); \

@@ -87,6 +87,68 @@ __device__ __forceinline__ void wgmma_n16(uint32_t (&d)[8], uint64_t desc_a, uin
     else if (BU) wgmma_n16_su(d, desc_a, desc_b, accumulate);
     else wgmma_n16_ss(d, desc_a, desc_b, accumulate);
 }
+// m64nNk32 for N = 16, 32, .., 128: one instruction per 64 rows x N columns, so the A slice is read from shared memory once per
+// k-step whatever N is.  The s32 fragment is N/2 registers per thread = N/16 consecutive n16 fragments (above), column chunk c in
+// d[8c .. 8c+7].  The operand lists are spelled out per N because an asm string cannot be computed.
+#define TB200_WG_REGS_16 "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p"
+#define TB200_WG_PRED_16 "setp.ne.b32 p, %10, 0;"
+#define TB200_WG_OPS_16 "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7])
+#define TB200_WG_REGS_32 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p"
+#define TB200_WG_PRED_32 "setp.ne.b32 p, %18, 0;"
+#define TB200_WG_OPS_32 "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+#define TB200_WG_REGS_48 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, p"
+#define TB200_WG_PRED_48 "setp.ne.b32 p, %26, 0;"
+#define TB200_WG_OPS_48 "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23])
+#define TB200_WG_REGS_64 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p"
+#define TB200_WG_PRED_64 "setp.ne.b32 p, %34, 0;"
+#define TB200_WG_OPS_64 "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+#define TB200_WG_REGS_80 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, %40, %41, p"
+#define TB200_WG_PRED_80 "setp.ne.b32 p, %42, 0;"
+#define TB200_WG_OPS_80 "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39])
+#define TB200_WG_REGS_96 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p"
+#define TB200_WG_PRED_96 "setp.ne.b32 p, %50, 0;"
+#define TB200_WG_OPS_96 "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47])
+#define TB200_WG_REGS_112 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55}, %56, %57, p"
+#define TB200_WG_PRED_112 "setp.ne.b32 p, %58, 0;"
+#define TB200_WG_OPS_112 "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55])
+#define TB200_WG_REGS_128 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p"
+#define TB200_WG_PRED_128 "setp.ne.b32 p, %66, 0;"
+#define TB200_WG_OPS_128 "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+#define TB200_WGMMA_N(N, AT, BT)                                                                                                \
+    asm volatile("{\n\t.reg .pred p;\n\t" TB200_WG_PRED_##N "\n\t"                                                                    \
+                 "wgmma.mma_async.sync.aligned.m64n" #N "k32.s32." AT "." BT " " TB200_WG_REGS_##N ";\n\t}"                         \
+                 : TB200_WG_OPS_##N                                                                                             \
+                 : "l"(desc_a), "l"(desc_b), "r"(accumulate)                                                                    \
+                 : "memory")
+#define TB200_WGMMA_AB(N)                                                                                                      \
+    if constexpr (AU && BU) TB200_WGMMA_N(N, "u8", "u8");                                                                     \
+    else if constexpr (AU) TB200_WGMMA_N(N, "u8", "s8");                                                                      \
+    else if constexpr (BU) TB200_WGMMA_N(N, "s8", "u8");                                                                      \
+    else TB200_WGMMA_N(N, "s8", "s8")
+// AU / BU: A / B operand unsigned; accumulate = 0 overwrites d (the first k-step of a tile)
+template <int N, bool AU, bool BU>
+__device__ __forceinline__ void wgmma_m64(uint32_t (&d)[N / 2], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate)
+{
+    static_assert(N % 16 == 0 && N >= 16 && N <= 128, "m64nNk32: N = 16, 32, .., 128");
+    if constexpr (N == 16) { TB200_WGMMA_AB(16); }
+    else if constexpr (N == 32) { TB200_WGMMA_AB(32); }
+    else if constexpr (N == 48) { TB200_WGMMA_AB(48); }
+    else if constexpr (N == 64) { TB200_WGMMA_AB(64); }
+    else if constexpr (N == 80) { TB200_WGMMA_AB(80); }
+    else if constexpr (N == 96) { TB200_WGMMA_AB(96); }
+    else if constexpr (N == 112) { TB200_WGMMA_AB(112); }
+    else { TB200_WGMMA_AB(128); }
+}
+#undef TB200_WGMMA_AB
+#undef TB200_WGMMA_N
+// Pins a register between asm statements: reads of an accumulator stay after the wgmma.wait_group that completes it, and writes
+// before the wgmma.fence that orders them ahead of the next wgmma.
+__device__ __forceinline__ void reg_fence(uint32_t& r) { asm volatile("" : "+r"(r)::"memory"); }
+// Register budget of the executing warpgroup (all four warps execute it): a role gives registers back to the SM's pool or takes them
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 __device__ __forceinline__ void sts_u2(uint32_t addr, uint32_t a, uint32_t b)
 {
     asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(addr), "r"(a), "r"(b) : "memory");
