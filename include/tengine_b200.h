@@ -198,6 +198,29 @@ TB200_API int tb200_graph_prerun(tb200_context* ctx, const tb200_tensor_desc* te
  * NCHW->NHWC on device, launches the graph, converts back, copies D2H, waits. */
 TB200_API int tb200_graph_run(tb200_graph* g, const void* const* host_inputs, void* const* host_outputs);
 
+/* ---- partial batches --------------------------------------------------------------------------------------------------------
+ * Make images [0, n) the batch of every later call on g, 1 <= n <= the batch g was prepared for (dims[0] at prerun), without a
+ * new prerun: run, upload, download, launch, upload_images, upload_detect_images (and the geometry they return), topk,
+ * yolo_detect, yolov5_detect, read_tensor, profile, work and num_launches then cover n images.  Caller buffers need room for n
+ * images only; nothing is read or written beyond them (tb200_graph_run page-locks exactly n images of each buffer).  Images
+ * n.. of the device arena keep stale bytes that no output ever reaches.
+ * On a multi-GPU context shard r runs tb200_shard_range(n, shards, r), and tb200_graph_shard reports that split; a shard whose
+ * share is 0 images (n < shards) issues no copy, kernel or graph launch, and its rows of topk / detect outputs do not exist.
+ * Synchronous with respect to queued work: every stream of every shard is drained before any launch sequence or CUDA graph is
+ * replaced.  Setting the active batch again does nothing; returning to the prepared batch reuses the CUDA graphs captured at
+ * prerun (the state is that of prerun, bit for bit); another n builds the launch sequences for n -- the whole batch and the
+ * pipeline chunks of tb200_graph_run, cut by prerun's rule at n: two chunks for an even n >= 32, a quarter and three
+ * quarters from 64 -- and captures them once (TB200_PRERUN_NO_GRAPH: builds them only).  Those of the most recent such n are
+ * kept, so alternating between the prepared batch and one n costs nothing after the first switch.
+ * Unchanged: the weight arena, the pack cache, the fused-node plan, the kernel of each layer (tb200_graph_layer_kernel) and
+ * the activation arena.
+ * TB200_ERR_INVALID for a null graph, n < 1 or n above the prepared batch; TB200_ERR_UNSUPPORTED for n other than the
+ * prepared batch on a graph whose tensors differ in dim 0 (prerun runs such a graph unsharded, as a whole).  A failed call
+ * leaves the active batch, and everything that runs, as it was. */
+TB200_API int tb200_graph_set_batch(tb200_graph* g, int n);
+/* the active batch: the prepared one until tb200_graph_set_batch changes it (TB200_ERR_INVALID for a null graph) */
+TB200_API int tb200_graph_batch(tb200_graph* g);
+
 /* The same three stages separately, for callers that keep data resident or time the kernels alone. */
 TB200_API int tb200_graph_upload(tb200_graph* g, int input_index, const void* host_nchw);
 TB200_API int tb200_graph_launch(tb200_graph* g);                 /* asynchronous on the context stream */
@@ -300,7 +323,8 @@ TB200_API int tb200_shard_range(int n_images, int world, int rank, int* first_im
 
 /* multi-GPU contexts: re-send the arena (after a caller filled GPU 0's arena itself, TB200_PRERUN_NO_WEIGHTS) */
 TB200_API int tb200_graph_broadcast_weights(tb200_graph* g);
-/* how the batch was cut: shard `index` runs images [first_image, first_image + num_images) on CUDA device *cuda_device */
+/* how the active batch is cut: shard `index` runs images [first_image, first_image + num_images) on CUDA device *cuda_device
+ * (num_images may be 0 after tb200_graph_set_batch to fewer images than shards) */
 TB200_API int tb200_graph_num_shards(tb200_graph* g);
 TB200_API int tb200_graph_shard(tb200_graph* g, int index, int* cuda_device, int* first_image, int* num_images);
 /* bytes of the activation arena of GPU 0's shard, what it would be without slot reuse, and of the weight arena */

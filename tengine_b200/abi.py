@@ -57,7 +57,7 @@ class KConvShape(C.Structure):
 EXPORTS = [
     "tb200_abi_version", "tb200_last_error", "tb200_device_count", "tb200_context_create", "tb200_context_destroy",
     "tb200_context_stream", "tb200_context_create_multi", "tb200_context_num_gpus", "tb200_context_gpu", "tb200_context_stream_of",
-    "tb200_context_broadcast_kind", "tb200_shard_range", "tb200_graph_broadcast_weights", "tb200_graph_num_shards", "tb200_graph_shard", "tb200_graph_arena_bytes", "tb200_probe_int8_tops", "tb200_pack_cache_dir", "tb200_graph_pack_cache_state", "tb200_graph_yolo_detect", "tb200_graph_yolov5_detect", "tb200_graph_topk", "tb200k_conv_winograd43_f32_workspace", "tb200k_conv_winograd43_f32", "tb200k_conv_dw3x3_f32",
+    "tb200_context_broadcast_kind", "tb200_shard_range", "tb200_graph_broadcast_weights", "tb200_graph_num_shards", "tb200_graph_shard", "tb200_graph_arena_bytes", "tb200_probe_int8_tops", "tb200_pack_cache_dir", "tb200_graph_pack_cache_state", "tb200_graph_yolo_detect", "tb200_graph_yolov5_detect", "tb200_graph_topk", "tb200_graph_set_batch", "tb200_graph_batch", "tb200k_conv_winograd43_f32_workspace", "tb200k_conv_winograd43_f32", "tb200k_conv_dw3x3_f32",
     "tb200_host_alloc", "tb200_host_free", "tb200_graph_prerun", "tb200_graph_run",
     "tb200_graph_upload", "tb200_graph_upload_images", "tb200_graph_upload_detect_images", "tb200_detections_to_source", "tb200_graph_launch", "tb200_graph_download", "tb200_graph_sync", "tb200_graph_postrun",
     "tb200_graph_weight_arena", "tb200_graph_num_launches", "tb200_graph_layer_kernel", "tb200_graph_read_tensor",

@@ -192,6 +192,46 @@ struct TensorInfo
     int producer = -1;
 };
 
+struct WeightBlob
+{
+    size_t w_off, bias_off, scale_off, fast_off, btab_off, w_size;
+};
+
+// Everything the planner decides for one layer.  plan_kernels fills in the kernel choice and what follows from it once,
+// fuse_nodes and prove_fast_epilogues add their part; no later pass re-derives a decision from the descriptors.
+struct LayerPlan
+{
+    int kind = K_NONE;
+    WeightBlob blob{};       // where the layer's packed data sits in the weight arena
+    bool reads_nchw = false; // stem kinds: the layer reads the NCHW graph input itself (no NHWC copy)
+    int nhwc16 = 0;          // K_GATHER_TC over a 16- / 32-channel NHWC tensor
+    bool u8_tc = false;      // uint8 K_GEMM / K_IGEMM / K_GATHER_TC: epilogue constants in the tensor-core layout
+    int gemm_zp = 0;         // zero-point argument of the GEMM planners: 1 + weight zero point for uint8, else 0
+    size_t k = 0;            // conv / FC: real K extent per output channel
+    int fuse_bias = 0;       // the int8 fast epilogue folds the bias into its FMA (an int: the pack-cache key hashes it so)
+    bool fast_ok = true;     // conv / FC: the fast epilogue is proven exact (fast-int proof and uint8 tensor-core proof)
+    int post_relu = 0;       // eltwise: the folded ReLU that follows it
+    int pool_relu = -1;      // max pooling: the folded (leaky) ReLU layer before it
+    int silu_sig = -1;       // Eltwise-PROD turned byte table: the folded Sigmoid layer
+    int silu_operand = 0;    // which operand of the product the sigmoid was (operand scales differ)
+    size_t scratch_off = 0;  // K_RESHAPE: NCHW staging in the activation arena
+};
+
+// The launch sequences of one shard for one active batch: images [0, n) of the shard's arena as a whole and as pipeline chunks,
+// and their CUDA graphs.  n == 0 (a shard left without images) has no steps at all.
+struct BatchPlan
+{
+    int n = -1;
+    std::vector<Step> steps;
+    int chunks = 1;
+    std::vector<int> chunk_first, chunk_count; // images of pipeline chunk k: [first, first + count)
+    std::vector<std::vector<Step>> chunk_steps;
+    std::vector<cudaGraph_t> cu_graphs; // [0] = whole slice, [1..K] = the pipeline chunks
+    std::vector<cudaGraphExec_t> cu_execs;
+    double work_ops = 0, work_bytes = 0, work_wbytes = 0;
+    int num_launches = 0;
+};
+
 struct tb200_graph
 {
     tb200_context* ctx;
@@ -199,26 +239,25 @@ struct tb200_graph
     std::vector<TensorInfo> tensors;
     std::vector<tb200_layer_desc> layers;
     std::vector<const char*> layer_kernel;
-    std::vector<Step> steps;
+    std::vector<LayerPlan> plan;
     std::vector<int> input_ids, output_ids;
     std::vector<uint8_t*> in_nchw_dev, out_nchw_dev;
     uint8_t* act_arena = nullptr;
     size_t act_bytes = 0;
     uint8_t* w_arena = nullptr;
     size_t w_bytes = 0;
-    int chunks = 1;
-    std::vector<int> chunk_first, chunk_count; // images of pipeline chunk k: [first, first + count)
-    std::vector<std::vector<Step>> chunk_steps;
-    std::vector<cudaGraph_t> cu_graphs;
-    std::vector<cudaGraphExec_t> cu_execs;
+    // tb200_graph_set_batch: `prepared` covers the batch of prerun, `other` the most recent smaller one; `cur` is the active one
+    BatchPlan prepared, other;
+    BatchPlan* cur = &prepared;
+    int other_batch = 0; // the active batch `other` was built for (root; 0: none)
     cudaStream_t copy_stream = nullptr, d2h_stream = nullptr;
     std::vector<cudaEvent_t> ev_in, ev_out;
     cudaEvent_t ev_done = nullptr;
-    double work_ops = 0, work_bytes = 0, work_wbytes = 0;
-    int num_launches = 0;
-    // batch sharding over the GPUs of a multi-GPU context: this graph is the shard of GPU 0 and owns the others
+    // batch sharding over the GPUs of a multi-GPU context: this graph is the shard of GPU 0 and owns the others.
+    // first_image / num_images: the shard's part of the active batch (num_images may be 0); prep_images: its part of the batch
+    // of prerun, the dim 0 of its tensors; total_images: that batch; batch: the active one (root)
     std::vector<tb200_graph*> shards;
-    int first_image = 0, num_images = 0, total_images = 0;
+    int first_image = 0, num_images = 0, prep_images = 0, total_images = 0, batch = 0;
     size_t act_unshared_bytes = 0; // what the arena would need without slot reuse (introspection)
     int pack_cache_state = 0;      // 0 no cache directory, 1 packed and written, 2 read from the cache
     // tb200_graph_upload_images: device copy of this shard's pixel span, its image descriptors (staged through page-locked host
@@ -405,6 +444,26 @@ int tb200k_cpad(int channels) { return cpad(channels); }
 
 } // extern "C"
 
+// cudaMemcpyAsync between the device and pageable host memory: the caller's buffers and the library's own (the packed weight image, the
+// detection tables).  host_pin keeps a caller buffer registered until postrun; once the caller frees it, a later allocation at that
+// address -- a caller buffer of another size (a batch changed with tb200_graph_set_batch), or a vector of this library -- can start
+// inside the stale registration and run past it, and CUDA refuses the copy (invalid argument).  Then every GPU of the group finishes
+// its queued work, all of this context's registrations are dropped and the copy is issued once more; registrations come back as
+// buffers are seen again.
+static cudaError_t host_copy(tb200_context* root, void* dst, const void* src, size_t bytes, cudaMemcpyKind kind, cudaStream_t st)
+{
+    cudaError_t e = cudaMemcpyAsync(dst, src, bytes, kind, st);
+    if (e != cudaErrorInvalidValue || root->host_regs.empty()) return e;
+    cudaGetLastError();
+    int dev = 0;
+    cudaGetDevice(&dev);
+    for (int k = 0; k <= (int)root->peers.size(); k++)
+        if (cudaSetDevice(context_of(root, k)->device) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) cudaGetLastError();
+    cudaSetDevice(dev);
+    host_unregister_all(root);
+    return cudaMemcpyAsync(dst, src, bytes, kind, st);
+}
+
 // ---- planner ------------------------------------------------------------------------------------------------
 static EpiParams make_epi(const tb200_layer_desc& L, const tb200_tensor_desc& tin, const tb200_tensor_desc& tout, bool fc)
 {
@@ -473,11 +532,6 @@ static size_t gemm_weight_bytes(int ocp, int k)
     return (size_t)nt * bn * k;
 }
 
-struct WeightBlob
-{
-    size_t w_off, bias_off, scale_off, fast_off, btab_off, w_size;
-};
-
 static int run_step(tb200_graph* g, const Step& s, cudaStream_t st)
 {
     cudaError_t err = cudaSuccess;
@@ -519,14 +573,22 @@ static int run_step(tb200_graph* g, const Step& s, cudaStream_t st)
     return 0;
 }
 
+// the CUDA graphs of `bp` (on the current device) and its steps; bp is then empty
+static void destroy_batch_plan(BatchPlan& bp)
+{
+    for (auto e : bp.cu_execs) if (e) cudaGraphExecDestroy(e);
+    for (auto c : bp.cu_graphs) if (c) cudaGraphDestroy(c);
+    bp = BatchPlan();
+}
+
 static void destroy_graph(tb200_graph* g)
 {
     if (!g) return;
     for (tb200_graph* sh : g->shards) destroy_graph(sh);
     g->shards.clear();
     cudaSetDevice(g->ctx->device);
-    for (auto e : g->cu_execs) if (e) cudaGraphExecDestroy(e);
-    for (auto c : g->cu_graphs) if (c) cudaGraphDestroy(c);
+    destroy_batch_plan(g->prepared);
+    destroy_batch_plan(g->other);
     for (auto e : g->ev_in) cudaEventDestroy(e);
     for (auto e : g->ev_out) cudaEventDestroy(e);
     if (g->ev_done) cudaEventDestroy(g->ev_done);
@@ -623,26 +685,6 @@ static void build_relu_lut(bool u8, const tb200_tensor_desc& tin, const tb200_te
 
 // ---- graph prerun: planning passes -----------------------------------------------------------------------------
 // prerun_one runs them in order; each pass reads the layer plans the earlier ones filled in.
-
-// Everything the planner decides for one layer.  plan_kernels fills in the kernel choice and what follows from it once,
-// fuse_nodes and prove_fast_epilogues add their part; no later pass re-derives a decision from the descriptors.
-struct LayerPlan
-{
-    int kind = K_NONE;
-    WeightBlob blob{};       // where the layer's packed data sits in the weight arena
-    bool reads_nchw = false; // stem kinds: the layer reads the NCHW graph input itself (no NHWC copy)
-    int nhwc16 = 0;          // K_GATHER_TC over a 16- / 32-channel NHWC tensor
-    bool u8_tc = false;      // uint8 K_GEMM / K_IGEMM / K_GATHER_TC: epilogue constants in the tensor-core layout
-    int gemm_zp = 0;         // zero-point argument of the GEMM planners: 1 + weight zero point for uint8, else 0
-    size_t k = 0;            // conv / FC: real K extent per output channel
-    int fuse_bias = 0;       // the int8 fast epilogue folds the bias into its FMA (an int: the pack-cache key hashes it so)
-    bool fast_ok = true;     // conv / FC: the fast epilogue is proven exact (fast-int proof and uint8 tensor-core proof)
-    int post_relu = 0;       // eltwise: the folded ReLU that follows it
-    int pool_relu = -1;      // max pooling: the folded (leaky) ReLU layer before it
-    int silu_sig = -1;       // Eltwise-PROD turned byte table: the folded Sigmoid layer
-    int silu_operand = 0;    // which operand of the product the sigmoid was (operand scales differ)
-    size_t scratch_off = 0;  // K_RESHAPE: NCHW staging in the activation arena
-};
 
 // ---- node fusion (SURVEY.md 8(f)-1), decided from the descriptors alone ----
 // [tensor] the one layer that reads it, or -1 when it has no reader, several, or is a graph output: a node may be folded into
@@ -1378,18 +1420,17 @@ static int upload_weights(tb200_graph* g, const std::vector<LayerPlan>& plan)
     if (!cache_hit) pack_arena_image(g, plan, img.data());
     if (getenv("TB200_DEBUG_HASH") && atoi(getenv("TB200_DEBUG_HASH")) >= 2) debug_print_pack(g, plan, img.data());
     if (!cache_path.empty() && !cache_hit) pack_cache_store(cache_path, key, img);
-    CUDA_OK(cudaMemcpyAsync(g->w_arena, img.data(), g->w_bytes, cudaMemcpyHostToDevice, g->ctx->stream));
+    CUDA_OK(host_copy(g->ctx, g->w_arena, img.data(), g->w_bytes, cudaMemcpyHostToDevice, g->ctx->stream));
     CUDA_OK(cudaStreamSynchronize(g->ctx->stream));
     return 0;
 }
 
 // ---- pipeline chunks: an even batch of 32 or more is cut into two chunks (images are independent units) so that `run` can
 //      overlap the H2D copy of the second with the kernels of the first; each chunk owns a slice of every tensor ----
-static void plan_chunks(tb200_graph* g)
+static void plan_chunks(const tb200_graph* g, int Ntot, BatchPlan& bp)
 {
-    const int Ntot = g->tensors[0].d.dims[0];
     bool same_batch = true;
-    for (auto& t : g->tensors) same_batch &= (t.d.dims[0] == Ntot);
+    for (auto& t : g->tensors) same_batch &= (t.d.dims[0] == g->tensors[0].d.dims[0]);
     int K = 1;
     std::vector<int> cfirst{0}, ccount{Ntot};
     if (same_batch && !(g->flags & TB200_PRERUN_NO_GRAPH) && Ntot >= 32 && Ntot % 2 == 0)
@@ -1400,9 +1441,9 @@ static void plan_chunks(tb200_graph* g)
         const int a = Ntot >= 64 ? ((Ntot / 4 + 7) / 8) * 8 : Ntot / 2;
         cfirst = {0, a}, ccount = {a, Ntot - a};
     }
-    g->chunks = K;
-    g->chunk_first = cfirst, g->chunk_count = ccount;
-    g->chunk_steps.resize(K > 1 ? K : 0);
+    bp.chunks = K;
+    bp.chunk_first = cfirst, bp.chunk_count = ccount;
+    bp.chunk_steps.resize(K > 1 ? K : 0);
 }
 
 // ---- step building ----
@@ -1415,7 +1456,7 @@ struct Slice
     long long bytes(const TensorInfo& t) const { return (long long)(t.nhwc_bytes / (size_t)ntot * (size_t)nb); }
 };
 
-static int fill_conv_step(tb200_graph* g, int li, const LayerPlan& P, const Slice& sl, bool count_work, Step& s)
+static int fill_conv_step(tb200_graph* g, int li, const LayerPlan& P, const Slice& sl, BatchPlan* work, Step& s)
 {
     const tb200_layer_desc& L = g->layers[li];
     const TensorInfo& tin = g->tensors[L.inputs[0]];
@@ -1444,12 +1485,14 @@ static int fill_conv_step(tb200_graph* g, int li, const LayerPlan& P, const Slic
         cs.dh = L.dilation_h, cs.dw = L.dilation_w, cs.group = L.group;
         cs.cg = C / L.group, cs.cgp = (L.group == 1) ? tin.cp : cs.cg;
     }
-    if (count_work)
+    if (work)
     {
-        const double k = (double)P.k, outputs = fc ? (double)sl.ntot * OC : (double)tout.nchw_bytes; // an FC has one output pixel
-        g->work_ops += 2.0 * outputs * k;
-        g->work_bytes += (double)tin.nchw_bytes + tout.nchw_bytes + (double)OC * k + (L.bias ? 4.0 * OC : 0);
-        g->work_wbytes += (double)OC * k + (L.bias ? 4.0 * OC : 0);
+        auto part = [&](size_t b) { return sl.nb == sl.ntot ? b : b / sl.ntot * sl.nb; }; // the slice's share of a tensor
+        const size_t in_bytes = part(tin.nchw_bytes), out_bytes = part(tout.nchw_bytes);
+        const double k = (double)P.k, outputs = fc ? (double)sl.nb * OC : (double)out_bytes; // an FC has one output pixel
+        work->work_ops += 2.0 * outputs * k;
+        work->work_bytes += (double)in_bytes + out_bytes + (double)OC * k + (L.bias ? 4.0 * OC : 0);
+        work->work_wbytes += (double)OC * k + (L.bias ? 4.0 * OC : 0);
     }
     if (P.reads_nchw) s.in = g->in_nchw_dev[tin.input_index] + sl.off(tin.nchw_bytes);
     s.nhwc16 = P.nhwc16;
@@ -1582,9 +1625,11 @@ static int fill_data_step(const tb200_graph* g, int li, const LayerPlan& P, cons
     return 0;
 }
 
-// The launch sequence of images [first, first + nb) (the whole batch, or one pipeline chunk) into `steps`.
-static int build_steps(tb200_graph* g, const std::vector<LayerPlan>& plan, int first, int nb, std::vector<Step>& steps, bool count_work)
+// The launch sequence of images [first, first + nb) (the active batch, or one pipeline chunk of it) into `steps`; the work of its
+// convolutions is added to *work when given.
+static int build_steps(tb200_graph* g, int first, int nb, std::vector<Step>& steps, BatchPlan* work)
 {
+    const std::vector<LayerPlan>& plan = g->plan;
     const Slice sl{first, nb, g->tensors[0].d.dims[0]};
     auto layout_step = [&](int kind, const void* in, void* out, const TensorInfo& t)
     {
@@ -1608,7 +1653,7 @@ static int build_steps(tb200_graph* g, const std::vector<LayerPlan>& plan, int f
         s.kind = P.kind, s.layer = li, s.u8 = tin.d.data_type == TB200_DT_UINT8;
         s.in = sl.dev(tin), s.out = sl.dev(g->tensors[L.output]);
         int rc;
-        if (L.op == TB200_OP_CONV || L.op == TB200_OP_FC) rc = fill_conv_step(g, li, P, sl, count_work, s);
+        if (L.op == TB200_OP_CONV || L.op == TB200_OP_FC) rc = fill_conv_step(g, li, P, sl, work, s);
         else if (P.kind == K_POOL) rc = fill_pool_step(g, li, P, sl, s);
         else if (P.kind == K_POINTWISE) rc = fill_pointwise_step(g, li, P, sl, s);
         else if (P.kind == K_CONCAT_PART) rc = fill_concat_steps(g, li, P, sl, s, steps);
@@ -1625,28 +1670,29 @@ static int build_steps(tb200_graph* g, const std::vector<LayerPlan>& plan, int f
     return 0;
 }
 
-// ---- capture the launch sequences into CUDA graphs: [0] = whole batch, [1..K] = the pipeline chunks ----
-static int capture_graphs(tb200_graph* g)
+// ---- capture the launch sequences of `bp` into CUDA graphs: [0] = whole slice, [1..K] = the pipeline chunks ----
+static int capture_graphs(tb200_graph* g, BatchPlan& bp)
 {
     cudaStream_t st = g->ctx->stream;
-    const int ngraphs = 1 + (int)g->chunk_steps.size();
-    g->cu_graphs.assign(ngraphs, nullptr);
-    g->cu_execs.assign(ngraphs, nullptr);
+    const int ngraphs = 1 + (int)bp.chunk_steps.size();
+    bp.cu_graphs.assign(ngraphs, nullptr);
+    bp.cu_execs.assign(ngraphs, nullptr);
     for (int gi = 0; gi < ngraphs; gi++)
     {
-        const std::vector<Step>& seq = gi == 0 ? g->steps : g->chunk_steps[gi - 1];
+        const std::vector<Step>& seq = gi == 0 ? bp.steps : bp.chunk_steps[gi - 1];
         CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
         int rc = 0;
         for (const Step& s : seq)
             if ((rc = run_step(g, s, st)) != 0) break;
-        cudaError_t ce = cudaStreamEndCapture(st, &g->cu_graphs[gi]);
+        cudaError_t ce = cudaStreamEndCapture(st, &bp.cu_graphs[gi]);
         if (rc) return rc;
         if (ce != cudaSuccess) return fail(TB200_ERR_CUDA, "graph capture failed: %s", cudaGetErrorString(ce));
-        ce = cudaGraphInstantiate(&g->cu_execs[gi], g->cu_graphs[gi], 0);
+        ce = cudaGraphInstantiate(&bp.cu_execs[gi], bp.cu_graphs[gi], 0);
         if (ce != cudaSuccess) return fail(TB200_ERR_CUDA, "graph instantiate failed: %s", cudaGetErrorString(ce));
     }
-    const int K = g->chunks;
-    if (K > 1)
+    // the pipeline's streams and events: made by the first plan with chunks, shared by every later one
+    const int K = bp.chunks;
+    if (K > 1 && !g->copy_stream)
     {
         CUDA_OK(cudaStreamCreateWithFlags(&g->copy_stream, cudaStreamNonBlocking));
         CUDA_OK(cudaStreamCreateWithFlags(&g->d2h_stream, cudaStreamNonBlocking));
@@ -1661,6 +1707,38 @@ static int capture_graphs(tb200_graph* g)
     return 0;
 }
 
+// A capture a failed CUDA call may have left open on `st` is ended and its graph dropped.
+static void end_open_capture(cudaStream_t st)
+{
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    if (cudaStreamIsCapturing(st, &cs) == cudaSuccess && cs != cudaStreamCaptureStatusNone)
+    {
+        cudaGraph_t junk = nullptr;
+        cudaStreamEndCapture(st, &junk);
+        if (junk) cudaGraphDestroy(junk);
+    }
+    cudaGetLastError();
+}
+
+// The launch sequences of images [0, nb) of this shard into bp: the whole slice, the pipeline chunks at nb (plan_chunks) and,
+// unless TB200_PRERUN_NO_GRAPH, their CUDA graphs.  nb == 0 leaves bp without steps: nothing is encoded or captured.
+static int build_batch_plan(tb200_graph* g, int nb, BatchPlan& bp)
+{
+    bp.n = nb;
+    if (nb == 0) return 0;
+    // the whole-slice plan serves tb200_graph_launch / profile (device-resident use); the chunk plans serve the pipelined
+    // tb200_graph_run.  They address the same tensors (a chunk is a slice of dim 0), so either may run at any time.
+    plan_chunks(g, nb, bp);
+    int rc;
+    if ((rc = build_steps(g, 0, nb, bp.steps, &bp)) != 0) return rc;
+    for (int ck = 0; ck < (int)bp.chunk_steps.size(); ck++)
+        if ((rc = build_steps(g, bp.chunk_first[ck], bp.chunk_count[ck], bp.chunk_steps[ck], nullptr)) != 0) return rc;
+    bp.num_launches = (int)bp.steps.size();
+    for (const Step& st : bp.steps) bp.num_launches += st.kind == K_RESHAPE ? 1 : 0; // two layout kernels
+    if (!(g->flags & TB200_PRERUN_NO_GRAPH) && (rc = capture_graphs(g, bp)) != 0) return rc;
+    return 0;
+}
+
 // Plans one graph on one GPU.  On failure the caller destroys g (arenas, tensor maps, CUDA graphs, an open capture).
 static int prerun_one(tb200_context* ctx, const tb200_tensor_desc* tensors, int num_tensors, const tb200_layer_desc* layers, int num_layers,
                       const int32_t* input_ids, int num_inputs, const int32_t* output_ids, int num_outputs, int flags, tb200_graph* g)
@@ -1668,7 +1746,8 @@ static int prerun_one(tb200_context* ctx, const tb200_tensor_desc* tensors, int 
     CUDA_OK(cudaSetDevice(ctx->device));
     g->layers.assign(layers, layers + num_layers);
     g->layer_kernel.assign(num_layers, kStepName[K_NONE]); // build_steps names every layer that was not folded away
-    std::vector<LayerPlan> plan(num_layers);
+    g->plan.assign(num_layers, LayerPlan());
+    std::vector<LayerPlan>& plan = g->plan;
     if (!(flags & TB200_PRERUN_NO_GRAPH)) fuse_nodes(layers, tensors, num_tensors, output_ids, num_outputs, g->layers, plan);
     int rc;
     if ((rc = setup_tensors(g, tensors, num_tensors, input_ids, num_inputs, output_ids, num_outputs)) != 0) return rc;
@@ -1677,17 +1756,9 @@ static int prerun_one(tb200_context* ctx, const tb200_tensor_desc* tensors, int 
     if ((rc = alloc_device_buffers(g)) != 0) return rc;
     prove_fast_epilogues(g, plan);
     if (!(flags & TB200_PRERUN_NO_WEIGHTS) && (rc = upload_weights(g, plan)) != 0) return rc;
-    // the whole-batch plan serves tb200_graph_launch / profile (device-resident use); the chunk plans serve the pipelined
-    // tb200_graph_run.  They address the same tensors (a chunk is a slice of dim 0), so either may run at any time.
-    plan_chunks(g);
-    if ((rc = build_steps(g, plan, 0, g->tensors[0].d.dims[0], g->steps, true)) != 0) return rc;
-    for (int ck = 0; ck < (int)g->chunk_steps.size(); ck++)
-        if ((rc = build_steps(g, plan, g->chunk_first[ck], g->chunk_count[ck], g->chunk_steps[ck], false)) != 0) return rc;
-    g->num_launches = (int)g->steps.size();
-    for (const Step& st : g->steps) g->num_launches += st.kind == K_RESHAPE ? 1 : 0; // two layout kernels
     CUDA_OK(cudaStreamSynchronize(ctx->stream));
-    if (!(flags & TB200_PRERUN_NO_GRAPH) && (rc = capture_graphs(g)) != 0) return rc;
-    return 0;
+    g->cur = &g->prepared;
+    return build_batch_plan(g, g->tensors[0].d.dims[0], g->prepared);
 }
 
 // ---- page-locking of the caller's buffers ---------------------------------------------------------------------------------
@@ -1738,6 +1809,7 @@ static bool host_pin(tb200_context* root, const void* ptr, size_t bytes)
     return true;
 }
 
+
 // every shard of a graph, the root's own first
 template <typename F>
 static int for_each_shard(tb200_graph* g, F f)
@@ -1746,7 +1818,21 @@ static int for_each_shard(tb200_graph* g, F f)
     for (size_t i = 0; rc == 0 && i < g->shards.size(); i++) rc = f(g->shards[i], (int)i + 1);
     return rc;
 }
-static inline size_t image_bytes(const tb200_graph* g, int tensor_id) { return g->tensors[tensor_id].nchw_bytes / (size_t)g->num_images; }
+// the shards that hold images of the active batch: a shard left without any issues no copy, kernel or graph launch
+template <typename F>
+static int for_each_busy_shard(tb200_graph* g, F f)
+{
+    return for_each_shard(g, [&](tb200_graph* sh, int r) { return sh->num_images ? f(sh, r) : 0; });
+}
+// NCHW bytes of one image of a tensor (from the batch of prerun, which sized the tensor)
+static inline size_t image_bytes(const tb200_graph* g, int tensor_id) { return g->tensors[tensor_id].nchw_bytes / (size_t)g->prep_images; }
+// dim 0 and NCHW bytes of the shard's active images of a tensor: all of it at the batch of prerun (also when its dim 0 is not the
+// batch), else num_images images
+static inline int active_dim0(const tb200_graph* g, const TensorInfo& t) { return g->num_images == g->prep_images ? t.d.dims[0] : g->num_images; }
+static inline size_t active_nchw_bytes(const tb200_graph* g, const TensorInfo& t)
+{
+    return g->num_images == g->prep_images ? t.nchw_bytes : t.nchw_bytes / (size_t)t.d.dims[0] * (size_t)g->num_images;
+}
 
 // One ncclBroadcast of the packed arena from GPU 0 to every other GPU of the group (grouped: one call per device from this
 // single thread), or peer copies when NCCL is not in use.
@@ -1801,19 +1887,11 @@ static int prerun_guarded(tb200_context* ctx, const tb200_tensor_desc* tensors, 
     const int rc = prerun_one(ctx, tensors, num_tensors, layers, num_layers, input_ids, num_inputs, output_ids, num_outputs, flags, g);
     if (rc)
     {
-        // a failed CUDA call may have left a capture open on the context stream
-        cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-        if (cudaStreamIsCapturing(ctx->stream, &cs) == cudaSuccess && cs != cudaStreamCaptureStatusNone)
-        {
-            cudaGraph_t junk = nullptr;
-            cudaStreamEndCapture(ctx->stream, &junk);
-            if (junk) cudaGraphDestroy(junk);
-        }
-        cudaGetLastError();
+        end_open_capture(ctx->stream);
         destroy_graph(g);
         return rc;
     }
-    g->num_images = g->total_images = tensors[0].dims[0];
+    g->num_images = g->prep_images = g->total_images = g->batch = tensors[0].dims[0];
     *out = g;
     return 0;
 }
@@ -1852,7 +1930,7 @@ int tb200_graph_prerun(tb200_context* ctx, const tb200_tensor_desc* tensors, int
             cudaSetDevice(ctx->device);
             return rc;
         }
-        sh->first_image = first, sh->num_images = count, sh->total_images = N;
+        sh->first_image = first, sh->num_images = sh->prep_images = count, sh->total_images = sh->batch = N;
         first += count;
         if (r == 0) root = sh;
         else root->shards.push_back(sh);
@@ -1916,6 +1994,69 @@ int tb200_graph_shard(tb200_graph* g, int index, int* cuda_device, int* first_im
     return 0;
 }
 
+// Drains every stream of every shard, then makes images [0, n) the batch of every later call.  The steps and CUDA graphs of a
+// batch other than the prepared one are built once and kept until another such batch replaces them.
+int tb200_graph_set_batch(tb200_graph* g, int n)
+{
+    if (!g) return fail(TB200_ERR_INVALID, "null graph");
+    if (n < 1 || n > g->total_images) return fail(TB200_ERR_INVALID, "set_batch: %d images; the graph was prepared for 1..%d", n, g->total_images);
+    if (n == g->batch) return 0;
+    for (const TensorInfo& t : g->tensors)
+        if (t.d.dims[0] != g->tensors[0].d.dims[0])
+            return fail(TB200_ERR_UNSUPPORTED, "set_batch: the graph's tensors differ in dim 0, so it runs only at the batch of %d it was prepared for",
+                        g->total_images);
+    int rc = for_each_shard(g, [&](tb200_graph* sh, int) -> int {
+        CUDA_OK(cudaSetDevice(sh->ctx->device));
+        if (sh->copy_stream) CUDA_OK(cudaStreamSynchronize(sh->copy_stream));
+        if (sh->d2h_stream) CUDA_OK(cudaStreamSynchronize(sh->d2h_stream));
+        CUDA_OK(cudaStreamSynchronize(sh->ctx->stream));
+        return 0;
+    });
+    const int R = 1 + (int)g->shards.size();
+    auto shard = [&](int r) { return r == 0 ? g : g->shards[r - 1]; };
+    const bool prepared = n == g->total_images;
+    if (rc == 0 && !prepared && n != g->other_batch)
+    {
+        // build every shard's plan before replacing any: a failure leaves the graph as it was
+        std::vector<BatchPlan> fresh(R);
+        for (int r = 0; r < R && rc == 0; r++)
+        {
+            tb200_graph* sh = shard(r);
+            int count = 0;
+            tb200_shard_range(n, R, r, nullptr, &count);
+            const std::vector<const char*> names = sh->layer_kernel; // the kernel names stay those of prerun
+            cudaSetDevice(sh->ctx->device);
+            rc = build_batch_plan(sh, count, fresh[r]);
+            sh->layer_kernel = names;
+            if (rc) end_open_capture(sh->ctx->stream);
+        }
+        for (int r = 0; r < R; r++)
+        {
+            tb200_graph* sh = shard(r);
+            cudaSetDevice(sh->ctx->device);
+            destroy_batch_plan(rc ? fresh[r] : sh->other);
+            if (!rc) sh->other = std::move(fresh[r]);
+        }
+        if (!rc) g->other_batch = n;
+    }
+    if (rc == 0)
+        for (int r = 0; r < R; r++)
+        {
+            tb200_graph* sh = shard(r);
+            sh->cur = prepared ? &sh->prepared : &sh->other;
+            tb200_shard_range(n, R, r, &sh->first_image, &sh->num_images);
+            sh->batch = n;
+        }
+    cudaSetDevice(g->ctx->device);
+    return rc;
+}
+
+int tb200_graph_batch(tb200_graph* g)
+{
+    if (!g) return fail(TB200_ERR_INVALID, "null graph");
+    return g->batch;
+}
+
 int tb200_graph_arena_bytes(tb200_graph* g, size_t* activation_bytes, size_t* unshared_bytes, size_t* weight_bytes)
 {
     if (!g) return fail(TB200_ERR_INVALID, "null graph");
@@ -1928,11 +2069,11 @@ int tb200_graph_arena_bytes(tb200_graph* g, size_t* activation_bytes, size_t* un
 int tb200_graph_upload(tb200_graph* g, int input_index, const void* host_nchw)
 {
     if (!g || input_index < 0 || input_index >= (int)g->input_ids.size() || !host_nchw) return fail(TB200_ERR_INVALID, "bad upload arguments");
-    const int rc = for_each_shard(g, [&](tb200_graph* sh, int) -> int {
+    const int rc = for_each_busy_shard(g, [&](tb200_graph* sh, int) -> int {
         CUDA_OK(cudaSetDevice(sh->ctx->device));
         const int id = sh->input_ids[input_index];
-        CUDA_OK(cudaMemcpyAsync(sh->in_nchw_dev[input_index], (const uint8_t*)host_nchw + (size_t)sh->first_image * image_bytes(sh, id),
-                                sh->tensors[id].nchw_bytes, cudaMemcpyHostToDevice, sh->ctx->stream));
+        CUDA_OK(host_copy(g->ctx, sh->in_nchw_dev[input_index], (const uint8_t*)host_nchw + (size_t)sh->first_image * image_bytes(sh, id),
+                                active_nchw_bytes(sh, sh->tensors[id]), cudaMemcpyHostToDevice, sh->ctx->stream));
         return 0;
     });
     cudaSetDevice(g->ctx->device);
@@ -1945,7 +2086,7 @@ static int check_images(const tb200_graph* g, const char* what, size_t pixel_byt
 {
     for (int k = 0; k < 3; k++)
         if (!std::isfinite(mean[k]) || !std::isfinite(scale[k])) return fail(TB200_ERR_INVALID, "%s: mean / scale %d is not finite", what, k);
-    for (int i = 0; i < g->total_images; i++)
+    for (int i = 0; i < g->batch; i++)
     {
         const tb200_image& im = images[i];
         if (im.c != 3 && im.c != 4) return fail(TB200_ERR_UNSUPPORTED, "%s: image %d has %d channels (3 or 4 supported)", what, i, im.c);
@@ -1968,7 +2109,7 @@ static int upload_staged_images(tb200_graph* g, const char* what, const void* pi
 {
     CUDA_OK(cudaSetDevice(g->ctx->device));
     host_pin(g->ctx, pixels, pixel_bytes);
-    const int rc = for_each_shard(g, [&](tb200_graph* sh, int) -> int {
+    const int rc = for_each_busy_shard(g, [&](tb200_graph* sh, int) -> int {
         CUDA_OK(cudaSetDevice(sh->ctx->device));
         cudaGetLastError(); // the launch below reports cudaGetLastError(): a non-sticky error an earlier call left behind is not its own
         const int n = sh->num_images;
@@ -1998,7 +2139,7 @@ static int upload_staged_images(tb200_graph* g, const char* what, const void* pi
             sh->img_desc_host[i] = gm ? ImageDesc{im[i].offset - lo, im[i].w, im[i].h, im[i].c, gm[i].resize_w, gm[i].resize_h, gm[i].left, gm[i].top}
                                       : ImageDesc{im[i].offset - lo, im[i].w, im[i].h, im[i].c, 0, 0, 0, 0};
         cudaStream_t st = sh->ctx->stream;
-        CUDA_OK(cudaMemcpyAsync(sh->img_stage, (const uint8_t*)pixels + lo, hi - lo, cudaMemcpyHostToDevice, st));
+        CUDA_OK(host_copy(g->ctx, sh->img_stage, (const uint8_t*)pixels + lo, hi - lo, cudaMemcpyHostToDevice, st));
         CUDA_OK(cudaMemcpyAsync(sh->img_desc, sh->img_desc_host, sizeof(ImageDesc) * n, cudaMemcpyHostToDevice, st));
         CUDA_OK(cudaEventRecord(sh->img_ev, st));
         const cudaError_t e = launch(sh, sh->img_stage, sh->img_desc, n, st);
@@ -2062,8 +2203,8 @@ int tb200_graph_upload_detect_images(tb200_graph* g, int input_index, const void
     // the laid-out image: the input's own H x W, or twice it with Focus
     const int H = focus ? td.dims[2] * 2 : td.dims[2], W = focus ? td.dims[3] * 2 : td.dims[3];
     if (const int rc = check_images(g, "upload_detect_images", pixel_bytes, images, pre->mean, pre->scale)) return rc;
-    std::vector<tb200_detect_geometry> geo(g->total_images);
-    for (int i = 0; i < g->total_images; i++)
+    std::vector<tb200_detect_geometry> geo(g->batch);
+    for (int i = 0; i < g->batch; i++)
     {
         geo[i] = detect_geometry(pre->mode, images[i].w, images[i].h, W, H);
         if (geo[i].resize_w < 1 || geo[i].resize_h < 1 || geo[i].resize_w > W || geo[i].resize_h > H)
@@ -2131,7 +2272,7 @@ static int launch_one(tb200_graph* g)
         host.resize(g->w_bytes);
         CUDA_OK(cudaMemcpy(host.data(), g->w_arena, g->w_bytes, cudaMemcpyDeviceToHost));
         fprintf(stderr, "[tb200 dbg] weight arena %zu bytes hash %016llx\n", g->w_bytes, (unsigned long long)fnv1a(host.data(), g->w_bytes));
-        for (const Step& s : g->steps)
+        for (const Step& s : g->cur->steps)
         {
             int rc = run_step(g, s, g->ctx->stream);
             if (rc) return rc;
@@ -2145,12 +2286,12 @@ static int launch_one(tb200_graph* g)
         }
         return 0;
     }
-    if (!g->cu_execs.empty())
+    if (!g->cur->cu_execs.empty())
     {
-        CUDA_OK(cudaGraphLaunch(g->cu_execs[0], g->ctx->stream)); // the whole-batch graph
+        CUDA_OK(cudaGraphLaunch(g->cur->cu_execs[0], g->ctx->stream)); // the whole-batch graph
         return 0;
     }
-    for (const Step& s : g->steps)
+    for (const Step& s : g->cur->steps)
     {
         int rc = run_step(g, s, g->ctx->stream);
         if (rc) return rc;
@@ -2161,7 +2302,7 @@ static int launch_one(tb200_graph* g)
 int tb200_graph_launch(tb200_graph* g)
 {
     if (!g) return fail(TB200_ERR_INVALID, "null graph");
-    const int rc = for_each_shard(g, [&](tb200_graph* sh, int) { return launch_one(sh); });
+    const int rc = for_each_busy_shard(g, [&](tb200_graph* sh, int) { return launch_one(sh); });
     cudaSetDevice(g->ctx->device);
     return rc;
 }
@@ -2169,11 +2310,11 @@ int tb200_graph_launch(tb200_graph* g)
 int tb200_graph_download(tb200_graph* g, int output_index, void* host_nchw)
 {
     if (!g || output_index < 0 || output_index >= (int)g->output_ids.size() || !host_nchw) return fail(TB200_ERR_INVALID, "bad download arguments");
-    const int rc = for_each_shard(g, [&](tb200_graph* sh, int) -> int {
+    const int rc = for_each_busy_shard(g, [&](tb200_graph* sh, int) -> int {
         CUDA_OK(cudaSetDevice(sh->ctx->device));
         const int id = sh->output_ids[output_index];
-        CUDA_OK(cudaMemcpyAsync((uint8_t*)host_nchw + (size_t)sh->first_image * image_bytes(sh, id), sh->out_nchw_dev[output_index],
-                                sh->tensors[id].nchw_bytes, cudaMemcpyDeviceToHost, sh->ctx->stream));
+        CUDA_OK(host_copy(g->ctx, (uint8_t*)host_nchw + (size_t)sh->first_image * image_bytes(sh, id), sh->out_nchw_dev[output_index],
+                                active_nchw_bytes(sh, sh->tensors[id]), cudaMemcpyDeviceToHost, sh->ctx->stream));
         return 0;
     });
     cudaSetDevice(g->ctx->device);
@@ -2194,22 +2335,22 @@ int tb200_graph_sync(tb200_graph* g)
 
 // ---- run: three phases over the shards so that every GPU's copy engine starts before any GPU's kernels are queued ----
 // (1) queue the H2D copies of all chunks on the shard's copy stream
-static int run_enqueue_h2d(tb200_graph* g, const void* const* host_inputs)
+static int run_enqueue_h2d(tb200_context* root, tb200_graph* g, const void* const* host_inputs)
 {
     CUDA_OK(cudaSetDevice(g->ctx->device));
-    if (g->chunks <= 1 || g->cu_execs.empty())
+    if (g->cur->chunks <= 1 || g->cur->cu_execs.empty())
     {
         for (size_t i = 0; i < g->input_ids.size(); i++)
         {
             const int id = g->input_ids[i];
-            CUDA_OK(cudaMemcpyAsync(g->in_nchw_dev[i], (const uint8_t*)host_inputs[i] + (size_t)g->first_image * image_bytes(g, id),
-                                    g->tensors[id].nchw_bytes, cudaMemcpyHostToDevice, g->ctx->stream));
+            CUDA_OK(host_copy(root, g->in_nchw_dev[i], (const uint8_t*)host_inputs[i] + (size_t)g->first_image * image_bytes(g, id),
+                                    active_nchw_bytes(g, g->tensors[id]), cudaMemcpyHostToDevice, g->ctx->stream));
         }
         return 0;
     }
     // Pipelined: the H2D copies of all chunks are queued back to back on the copy stream (the link stays busy), chunk k's
     // kernels start as soon as ITS slice has landed, and its outputs leave on a third stream while chunk k+1 computes.
-    const int K = g->chunks;
+    const int K = g->cur->chunks;
     CUDA_OK(cudaEventRecord(g->ev_done, g->ctx->stream)); // order after whatever the caller queued on the context stream
     CUDA_OK(cudaStreamWaitEvent(g->copy_stream, g->ev_done, 0));
     for (int ck = 0; ck < K; ck++)
@@ -2217,8 +2358,8 @@ static int run_enqueue_h2d(tb200_graph* g, const void* const* host_inputs)
         for (size_t i = 0; i < g->input_ids.size(); i++)
         {
             const int id = g->input_ids[i];
-            const size_t ib = image_bytes(g, id), off = ib * (size_t)g->chunk_first[ck], bytes = ib * (size_t)g->chunk_count[ck];
-            CUDA_OK(cudaMemcpyAsync(g->in_nchw_dev[i] + off, (const uint8_t*)host_inputs[i] + (size_t)g->first_image * ib + off, bytes, cudaMemcpyHostToDevice,
+            const size_t ib = image_bytes(g, id), off = ib * (size_t)g->cur->chunk_first[ck], bytes = ib * (size_t)g->cur->chunk_count[ck];
+            CUDA_OK(host_copy(root, g->in_nchw_dev[i] + off, (const uint8_t*)host_inputs[i] + (size_t)g->first_image * ib + off, bytes, cudaMemcpyHostToDevice,
                                     g->copy_stream));
         }
         CUDA_OK(cudaEventRecord(g->ev_in[ck], g->copy_stream));
@@ -2226,35 +2367,35 @@ static int run_enqueue_h2d(tb200_graph* g, const void* const* host_inputs)
     return 0;
 }
 // (2) kernels + D2H
-static int run_enqueue_compute(tb200_graph* g, void* const* host_outputs)
+static int run_enqueue_compute(tb200_context* root, tb200_graph* g, void* const* host_outputs)
 {
     CUDA_OK(cudaSetDevice(g->ctx->device));
     cudaStream_t cs = g->ctx->stream;
     static const int dbg2 = getenv("TB200_DEBUG_HASH") ? atoi(getenv("TB200_DEBUG_HASH")) : 0;
-    if (g->chunks <= 1 || g->cu_execs.empty() || dbg2 >= 2)
+    if (g->cur->chunks <= 1 || g->cur->cu_execs.empty() || dbg2 >= 2)
     {
         int rc = launch_one(g);
         if (rc) return rc;
         for (size_t i = 0; i < g->output_ids.size(); i++)
         {
             const int id = g->output_ids[i];
-            CUDA_OK(cudaMemcpyAsync((uint8_t*)host_outputs[i] + (size_t)g->first_image * image_bytes(g, id), g->out_nchw_dev[i], g->tensors[id].nchw_bytes,
+            CUDA_OK(host_copy(root, (uint8_t*)host_outputs[i] + (size_t)g->first_image * image_bytes(g, id), g->out_nchw_dev[i], active_nchw_bytes(g, g->tensors[id]),
                                     cudaMemcpyDeviceToHost, cs));
         }
         return 0;
     }
-    const int K = g->chunks;
+    const int K = g->cur->chunks;
     for (int ck = 0; ck < K; ck++)
     {
         CUDA_OK(cudaStreamWaitEvent(cs, g->ev_in[ck], 0));
-        CUDA_OK(cudaGraphLaunch(g->cu_execs[1 + ck], cs));
+        CUDA_OK(cudaGraphLaunch(g->cur->cu_execs[1 + ck], cs));
         CUDA_OK(cudaEventRecord(g->ev_out[ck], cs));
         CUDA_OK(cudaStreamWaitEvent(g->d2h_stream, g->ev_out[ck], 0));
         for (size_t i = 0; i < g->output_ids.size(); i++)
         {
             const int id = g->output_ids[i];
-            const size_t ib = image_bytes(g, id), off = ib * (size_t)g->chunk_first[ck], bytes = ib * (size_t)g->chunk_count[ck];
-            CUDA_OK(cudaMemcpyAsync((uint8_t*)host_outputs[i] + (size_t)g->first_image * ib + off, g->out_nchw_dev[i] + off, bytes, cudaMemcpyDeviceToHost,
+            const size_t ib = image_bytes(g, id), off = ib * (size_t)g->cur->chunk_first[ck], bytes = ib * (size_t)g->cur->chunk_count[ck];
+            CUDA_OK(host_copy(root, (uint8_t*)host_outputs[i] + (size_t)g->first_image * ib + off, g->out_nchw_dev[i] + off, bytes, cudaMemcpyDeviceToHost,
                                     g->d2h_stream));
         }
     }
@@ -2264,7 +2405,7 @@ static int run_enqueue_compute(tb200_graph* g, void* const* host_outputs)
 static int run_wait(tb200_graph* g)
 {
     CUDA_OK(cudaSetDevice(g->ctx->device));
-    if (g->d2h_stream && g->chunks > 1 && !g->cu_execs.empty()) CUDA_OK(cudaStreamSynchronize(g->d2h_stream));
+    if (g->d2h_stream && g->cur->chunks > 1 && !g->cur->cu_execs.empty()) CUDA_OK(cudaStreamSynchronize(g->d2h_stream));
     CUDA_OK(cudaStreamSynchronize(g->ctx->stream));
     return 0;
 }
@@ -2278,22 +2419,22 @@ int tb200_graph_run(tb200_graph* g, const void* const* host_inputs, void* const*
         if (!host_outputs[i]) return fail(TB200_ERR_INVALID, "run: output %d has no host buffer (the graph has %d outputs)", (int)i, (int)g->output_ids.size());
     // page-lock the caller's buffers (whole batch) on first sight
     CUDA_OK(cudaSetDevice(g->ctx->device));
-    for (size_t i = 0; i < g->input_ids.size(); i++) host_pin(g->ctx, host_inputs[i], image_bytes(g, g->input_ids[i]) * (size_t)g->total_images);
-    for (size_t i = 0; i < g->output_ids.size(); i++) host_pin(g->ctx, host_outputs[i], image_bytes(g, g->output_ids[i]) * (size_t)g->total_images);
-    int rc = for_each_shard(g, [&](tb200_graph* sh, int) { return run_enqueue_h2d(sh, host_inputs); });
-    if (!rc) rc = for_each_shard(g, [&](tb200_graph* sh, int) { return run_enqueue_compute(sh, host_outputs); });
+    for (size_t i = 0; i < g->input_ids.size(); i++) host_pin(g->ctx, host_inputs[i], image_bytes(g, g->input_ids[i]) * (size_t)g->batch);
+    for (size_t i = 0; i < g->output_ids.size(); i++) host_pin(g->ctx, host_outputs[i], image_bytes(g, g->output_ids[i]) * (size_t)g->batch);
+    int rc = for_each_busy_shard(g, [&](tb200_graph* sh, int) { return run_enqueue_h2d(g->ctx, sh, host_inputs); });
+    if (!rc) rc = for_each_busy_shard(g, [&](tb200_graph* sh, int) { return run_enqueue_compute(g->ctx, sh, host_outputs); });
     const int rc2 = for_each_shard(g, [&](tb200_graph* sh, int) { return run_wait(sh); }); // always drain what was queued
     cudaSetDevice(g->ctx->device);
     static const bool dbg = getenv("TB200_DEBUG_HASH") != nullptr;
     if (dbg)
     {
         for (size_t i = 0; i < g->input_ids.size(); i++)
-            fprintf(stderr, "[tb200 run] input %zu: %zu bytes, hash %016llx\n", i, image_bytes(g, g->input_ids[i]) * (size_t)g->total_images,
-                    (unsigned long long)fnv1a(host_inputs[i], image_bytes(g, g->input_ids[i]) * (size_t)g->total_images));
+            fprintf(stderr, "[tb200 run] input %zu: %zu bytes, hash %016llx\n", i, image_bytes(g, g->input_ids[i]) * (size_t)g->batch,
+                    (unsigned long long)fnv1a(host_inputs[i], image_bytes(g, g->input_ids[i]) * (size_t)g->batch));
         for (size_t i = 0; i < g->output_ids.size(); i++)
-            fprintf(stderr, "[tb200 run] output %zu (tensor %d): %zu bytes, hash %016llx\n", i, g->output_ids[i], image_bytes(g, g->output_ids[i]) * (size_t)g->total_images,
-                    (unsigned long long)fnv1a(host_outputs[i], image_bytes(g, g->output_ids[i]) * (size_t)g->total_images));
-        fprintf(stderr, "[tb200 run] %zu layers, %d launches, chunks %d, shards %zu, flags %d\n", g->layers.size(), g->num_launches, g->chunks, g->shards.size() + 1, g->flags);
+            fprintf(stderr, "[tb200 run] output %zu (tensor %d): %zu bytes, hash %016llx\n", i, g->output_ids[i], image_bytes(g, g->output_ids[i]) * (size_t)g->batch,
+                    (unsigned long long)fnv1a(host_outputs[i], image_bytes(g, g->output_ids[i]) * (size_t)g->batch));
+        fprintf(stderr, "[tb200 run] %zu layers, %d launches, chunks %d, shards %zu, flags %d\n", g->layers.size(), g->cur->num_launches, g->cur->chunks, g->shards.size() + 1, g->flags);
     }
     return rc ? rc : rc2;
 }
@@ -2323,8 +2464,8 @@ int tb200_graph_weight_arena(tb200_graph* g, void** device_ptr, size_t* bytes)
 int tb200_graph_num_launches(tb200_graph* g)
 {
     if (!g) return 0;
-    int n = g->num_launches;
-    for (tb200_graph* sh : g->shards) n += sh->num_launches;
+    int n = g->cur->num_launches;
+    for (tb200_graph* sh : g->shards) n += sh->cur->num_launches;
     return n;
 }
 
@@ -2337,14 +2478,15 @@ const char* tb200_graph_layer_kernel(tb200_graph* g, int layer)
 int tb200_graph_read_tensor(tb200_graph* g, int tensor_id, void* host_nchw)
 {
     if (!g || tensor_id < 0 || tensor_id >= (int)g->tensors.size() || !host_nchw) return fail(TB200_ERR_INVALID, "bad arguments");
-    const int rc = for_each_shard(g, [&](tb200_graph* sh, int) -> int {
+    const int rc = for_each_busy_shard(g, [&](tb200_graph* sh, int) -> int {
         CUDA_OK(cudaSetDevice(sh->ctx->device));
         const TensorInfo& t = sh->tensors[tensor_id];
         uint8_t* tmp = nullptr;
-        CUDA_OK(cudaMalloc(&tmp, t.nchw_bytes));
-        cudaError_t e = launch_nhwc_to_nchw(t.dev, tmp, t.d.dims[0], t.d.dims[1], t.d.dims[2], t.d.dims[3], sh->ctx->stream);
+        const size_t bytes = active_nchw_bytes(sh, t);
+        CUDA_OK(cudaMalloc(&tmp, bytes));
+        cudaError_t e = launch_nhwc_to_nchw(t.dev, tmp, active_dim0(sh, t), t.d.dims[1], t.d.dims[2], t.d.dims[3], sh->ctx->stream);
         if (e == cudaSuccess)
-            e = cudaMemcpyAsync((uint8_t*)host_nchw + (size_t)sh->first_image * image_bytes(sh, tensor_id), tmp, t.nchw_bytes, cudaMemcpyDeviceToHost, sh->ctx->stream);
+            e = host_copy(g->ctx, (uint8_t*)host_nchw + (size_t)sh->first_image * image_bytes(sh, tensor_id), tmp, bytes, cudaMemcpyDeviceToHost, sh->ctx->stream);
         if (e == cudaSuccess) e = cudaStreamSynchronize(sh->ctx->stream);
         cudaFree(tmp);
         if (e != cudaSuccess) return fail(TB200_ERR_CUDA, "read_tensor: %s", cudaGetErrorString(e));
@@ -2363,7 +2505,7 @@ int tb200_graph_profile(tb200_graph* g, float* layer_ms, int num_layers)
     CUDA_OK(cudaEventCreate(&a));
     CUDA_OK(cudaEventCreate(&b));
     int rc = 0;
-    for (const Step& s : g->steps)
+    for (const Step& s : g->cur->steps)
     {
         cudaEventRecord(a, g->ctx->stream);
         rc = run_step(g, s, g->ctx->stream);
@@ -2409,7 +2551,7 @@ static int yolo_detect(tb200_graph* g, const tb200_yolo_params* p, tb200_detecti
     if (!g || !p || !out || !counts || max_per_image < 1 || p->num_heads < 1 || p->num_heads > 3) return fail(TB200_ERR_INVALID, "bad arguments");
     const int max_cand = p->max_candidates > 0 ? p->max_candidates : 4096;
     static_assert(sizeof(YoloDet) == sizeof(tb200_detection), "detection record layout");
-    const int rc = for_each_shard(g, [&](tb200_graph* sh, int) -> int {
+    const int rc = for_each_busy_shard(g, [&](tb200_graph* sh, int) -> int {
         const TensorInfo* heads[3] = {};
         for (int hd = 0; hd < p->num_heads; hd++)
         {
@@ -2443,7 +2585,7 @@ static int yolo_detect(tb200_graph* g, const tb200_yolo_params* p, tb200_detecti
         if (e == cudaSuccess) e = cudaMalloc(&ocnt, sizeof(int) * n_img);
         if (e == cudaSuccess) e = cudaMalloc(&dtab, sizeof tab);
         if (e == cudaSuccess) e = cudaMemsetAsync(cnt, 0, sizeof(int) * n_img, st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(dtab, &tab, sizeof tab, cudaMemcpyHostToDevice, st);
+        if (e == cudaSuccess) e = host_copy(g->ctx, dtab, &tab, sizeof tab, cudaMemcpyHostToDevice, st);
         const double* ex = (const double*)dtab;
         const float* sig = (const float*)(dtab + offsetof(YoloTables, sig));
         unsigned key_base = 0;
@@ -2457,8 +2599,8 @@ static int yolo_detect(tb200_graph* g, const tb200_yolo_params* p, tb200_detecti
         }
         if (e == cudaSuccess) e = launch_yolo_nms(cand, cnt, n_img, max_cand, p->nms_threshold, sorted, det, max_per_image, ocnt, st);
         if (e == cudaSuccess)
-            e = cudaMemcpyAsync(out + (size_t)sh->first_image * max_per_image, det, sizeof(YoloDet) * (size_t)n_img * max_per_image, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(counts + sh->first_image, ocnt, sizeof(int) * n_img, cudaMemcpyDeviceToHost, st);
+            e = host_copy(g->ctx, out + (size_t)sh->first_image * max_per_image, det, sizeof(YoloDet) * (size_t)n_img * max_per_image, cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess) e = host_copy(g->ctx, counts + sh->first_image, ocnt, sizeof(int) * n_img, cudaMemcpyDeviceToHost, st);
         if (e == cudaSuccess) e = cudaStreamSynchronize(st);
         cleanup();
         if (e != cudaSuccess) return fail(TB200_ERR_CUDA, "yolo_detect: %s", cudaGetErrorString(e));
@@ -2500,7 +2642,7 @@ int tb200_graph_topk(tb200_graph* g, int output_index, int k, tb200_class_score*
         const tb200_tensor_desc& d = g->tensors[g->output_ids[output_index]].d;
         if (const int rc = class_topk_check(d.data_type, d.scale, (long long)d.dims[1] * d.dims[2] * d.dims[3], k)) return rc;
     }
-    const int rc = for_each_shard(g, [&](tb200_graph* sh, int) -> int {
+    const int rc = for_each_busy_shard(g, [&](tb200_graph* sh, int) -> int {
         const TensorInfo& t = sh->tensors[sh->output_ids[output_index]];
         CUDA_OK(cudaSetDevice(sh->ctx->device));
         cudaGetLastError(); // the launch below reports cudaGetLastError(): a non-sticky error an earlier call left behind is not its own
@@ -2510,7 +2652,7 @@ int tb200_graph_topk(tb200_graph* g, int output_index, int k, tb200_class_score*
         cudaError_t e = cudaMalloc(&dev, bytes);
         if (e == cudaSuccess)
             e = launch_class_topk(t.dev, sh->num_images, t.d.dims[1], t.d.dims[2], t.d.dims[3], t.d.data_type == TB200_DT_UINT8, t.d.scale, t.d.zero_point, k, dev, st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(out + (size_t)sh->first_image * k, dev, bytes, cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess) e = host_copy(g->ctx, out + (size_t)sh->first_image * k, dev, bytes, cudaMemcpyDeviceToHost, st);
         if (e == cudaSuccess) e = cudaStreamSynchronize(st);
         cudaFree(dev);
         if (e != cudaSuccess) return fail(TB200_ERR_CUDA, "topk: %s", cudaGetErrorString(e));
@@ -2523,8 +2665,8 @@ int tb200_graph_topk(tb200_graph* g, int output_index, int k, tb200_class_score*
 int tb200_graph_work(tb200_graph* g, double* ops, double* bytes)
 {
     if (!g) return fail(TB200_ERR_INVALID, "null graph");
-    double o = g->work_ops, b = g->work_bytes;
-    for (tb200_graph* sh : g->shards) o += sh->work_ops, b += sh->work_bytes - sh->work_wbytes; // weights count once per launch
+    double o = g->cur->work_ops, b = g->cur->work_bytes;
+    for (tb200_graph* sh : g->shards) o += sh->cur->work_ops, b += sh->cur->work_bytes - sh->cur->work_wbytes; // weights count once per launch
     if (ops) *ops = o;
     if (bytes) *bytes = b;
     return 0;

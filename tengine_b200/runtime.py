@@ -46,7 +46,7 @@ def lib():
         for name in ("tb200_graph_run", "tb200_graph_upload", "tb200_graph_launch", "tb200_graph_download",
                      "tb200_graph_sync", "tb200_graph_postrun", "tb200_graph_weight_arena",
                      "tb200_graph_num_launches", "tb200_graph_read_tensor", "tb200_graph_profile",
-                     "tb200_graph_work", "tb200_context_destroy"):
+                     "tb200_graph_work", "tb200_context_destroy", "tb200_graph_set_batch", "tb200_graph_batch"):
             getattr(L, name).restype = C.c_int
         L.tb200_graph_upload.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         L.tb200_graph_upload_images.restype = C.c_int
@@ -80,6 +80,8 @@ def lib():
         L.tb200_graph_broadcast_weights.argtypes = [C.c_void_p]
         L.tb200_pack_cache_dir.argtypes = [C.c_char_p]
         L.tb200_graph_pack_cache_state.argtypes = [C.c_void_p]
+        L.tb200_graph_set_batch.argtypes = [C.c_void_p, C.c_int]
+        L.tb200_graph_batch.argtypes = [C.c_void_p]
         L.tb200_graph_topk.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
         L.tb200k_class_topk.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int32, C.c_int, C.c_void_p, C.c_void_p]
         _lib = L
@@ -233,13 +235,32 @@ class Graph:
                                         len(gdef.inputs), gdef.id_array(gdef.outputs), len(gdef.outputs), int(flags),
                                         C.byref(self.h)))
 
+    def set_batch(self, n):
+        """Make images [0, n) the batch of every later call, 1 <= n <= the batch the graph was prepared for
+        (tb200_graph_set_batch): host arrays then hold n images."""
+        _check(lib().tb200_graph_set_batch(self.h, int(n)))
+
+    @property
+    def batch(self):
+        """The active batch: the prepared one until set_batch changes it."""
+        n = lib().tb200_graph_batch(self.h)
+        if n < 0:
+            _check(n)
+        return n
+
+    def dims(self, t):
+        """Dims of tensor t at the active batch: the GraphDef's own at the prepared batch, else dim 0 is the active batch."""
+        d = tuple(self.gdef.dims(t))
+        n = self.batch
+        return d if n == self.gdef.dims(0)[0] else (n,) + d[1:]  # prerun's batch is dim 0 of tensor 0
+
     def run(self, inputs, outputs=None):
         g = self.gdef
         ins = [np.ascontiguousarray(x) for x in inputs]
         for x, t in zip(ins, g.inputs):
-            assert x.shape == g.dims(t) and x.dtype == g.np_dtype, (x.shape, g.dims(t), x.dtype)
+            assert x.shape == self.dims(t) and x.dtype == g.np_dtype, (x.shape, self.dims(t), x.dtype)
         if outputs is None:
-            outputs = [np.empty(g.dims(t), dtype=g.np_dtype) for t in g.outputs]
+            outputs = [np.empty(self.dims(t), dtype=g.np_dtype) for t in g.outputs]
         assert len(ins) == len(g.inputs) and len(outputs) == len(g.outputs), "one host buffer per graph input / output"
         ip = (C.c_void_p * len(ins))(*[a.ctypes.data for a in ins])
         op = (C.c_void_p * len(outputs))(*[a.ctypes.data for a in outputs])
@@ -253,8 +274,8 @@ class Graph:
         """The images packed into a page-locked buffer kept on the graph (waiting first for the graph's queued work, which may still
         read it) and their descriptors."""
         imgs = [np.ascontiguousarray(a) for a in images]
-        if len(imgs) != self.gdef.dims(self.gdef.inputs[i])[0]:
-            raise ValueError(f"{len(imgs)} images for a batch of {self.gdef.dims(self.gdef.inputs[i])[0]}")
+        if len(imgs) != self.dims(self.gdef.inputs[i])[0]:
+            raise ValueError(f"{len(imgs)} images for a batch of {self.dims(self.gdef.inputs[i])[0]}")
         descs = (abi.Image * len(imgs))()
         off = 0
         for d, a in zip(descs, imgs):
@@ -306,7 +327,7 @@ class Graph:
         _check(lib().tb200_graph_sync(self.h))
 
     def read_tensor(self, t):
-        out = np.empty(self.gdef.dims(t), dtype=self.gdef.np_dtype)
+        out = np.empty(self.dims(t), dtype=self.gdef.np_dtype)
         _check(lib().tb200_graph_read_tensor(self.h, t, out.ctypes.data))
         return out
 
@@ -362,7 +383,7 @@ class Graph:
             for k in range(6):
                 p.heads[i].anchors[k] = float(anchors[k])
         p.num_classes, p.prob_threshold, p.nms_threshold, p.max_candidates = int(num_classes), float(prob_threshold), float(nms_threshold), int(max_candidates)
-        n = self.gdef.dims(self.gdef.outputs[0])[0]
+        n = self.dims(self.gdef.outputs[0])[0]
         out = (abi.Detection * (n * max_per_image))()
         counts = (C.c_int32 * n)()
         fn = lib().tb200_graph_yolo_detect if version == 3 else lib().tb200_graph_yolov5_detect
@@ -383,7 +404,7 @@ class Graph:
         """What the classification examples print for every image of the last run (tb200_graph_topk): graph output `output_index`
         dequantised and ranked on the device in print_topk's order, its tie order included.  Returns (scores [N, k] float32,
         ids [N, k] int32); an id is the class's position among the image's elements in NCHW order."""
-        n = self.gdef.dims(self.gdef.outputs[output_index])[0]
+        n = self.dims(self.gdef.outputs[output_index])[0]
         out = np.zeros((n, max(int(k), 0)), np.dtype([("score", np.float32), ("id", np.int32)]))
         assert out.dtype.itemsize == C.sizeof(abi.ClassScore)
         _check(lib().tb200_graph_topk(self.h, int(output_index), int(k), out.ctypes.data))
