@@ -135,7 +135,7 @@ typedef struct tb200_layer_desc
     float bias_scale;
 } tb200_layer_desc;
 
-typedef struct tb200_context tb200_context; /* one GPU -- or a group of GPUs driven by this process -- : streams, NCCL communicators */
+typedef struct tb200_context tb200_context; /* one GPU -- or a group of GPUs driven by this process -- : streams */
 typedef struct tb200_graph tb200_graph;     /* one per Tengine subgraph (subgraph->device_graph) */
 
 /* ---- library / device ---------------------------------------------------------------------------- */
@@ -153,15 +153,14 @@ TB200_API void* tb200_context_stream(tb200_context* ctx);
 /* Several GPUs behind ONE device (SURVEY.md 8(e); the option-blob precedent is trt_option,
  * source/device/tensorrt/trt_define.h:36-42).  Every tb200_graph_* call on such a context shards dim 0 of the batch
  * contiguously over the GPUs: prerun plans one shard per GPU, packs the weights once (GPU 0) and moves the arena to
- * the others with ONE grouped ncclBroadcast (communicators from ncclCommInitAll; NCCL is dlopen'ed); run copies each
- * GPU's slice of the caller's NCHW buffers straight to that GPU and joins all streams before it returns.  There is no
- * collective in the steady state.  Listing a device twice (single-GPU test boxes) keeps every mechanism except NCCL
- * itself, which refuses duplicate devices: the arena is then copied with cudaMemcpyPeerAsync. */
+ * the others with one cudaMemcpyPeerAsync per GPU; run copies each GPU's slice of the caller's NCHW buffers straight
+ * to that GPU and joins all streams before it returns.  There is no collective in the steady state.  A device may be
+ * listed more than once (single-GPU test boxes): every mechanism stays the same. */
 TB200_API int tb200_context_create_multi(const int* cuda_devices, int num_devices, tb200_context** out);
 TB200_API int tb200_context_num_gpus(tb200_context* ctx);
 TB200_API int tb200_context_gpu(tb200_context* ctx, int index);        /* CUDA ordinal of GPU `index` of the group */
 TB200_API void* tb200_context_stream_of(tb200_context* ctx, int index); /* its stream (cudaStream_t) */
-TB200_API const char* tb200_context_broadcast_kind(tb200_context* ctx); /* "none" | "nccl" | "memcpy_peer" */
+TB200_API const char* tb200_context_broadcast_kind(tb200_context* ctx); /* "none" (one GPU) | "memcpy_peer" (a group) */
 
 /* What set_context_device(ctx, "B200", &opt, sizeof opt) carries (source/api/c_api.c:207-211 memcpy's it; the first field
  * must be the device name because sched_prerun dereferences *(char**)options, scheduler.c:49).  Zero = default. */
@@ -300,7 +299,7 @@ TB200_API int tb200_graph_upload_detect_images(tb200_graph* g, int input_index, 
 /* interface->post_run (device.h:53) */
 TB200_API int tb200_graph_postrun(tb200_graph* g);
 
-/* Packed-weight arena (device pointer + size): the object of the single NCCL broadcast at prerun when the
+/* Packed-weight arena (device pointer + size): what prerun copies from GPU 0 to the other GPUs when the
  * batch is sharded over several GPUs (SURVEY.md 8(e)); identical layout on every rank for identical graphs. */
 TB200_API int tb200_graph_weight_arena(tb200_graph* g, void** device_ptr, size_t* bytes);
 

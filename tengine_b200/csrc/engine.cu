@@ -5,7 +5,6 @@
 // cpu_device.c:62-95) and of conv_hcl_prerun's weight packing (conv_kernel_x86.c:2137-2209); run = the
 // analogue of cpu_device.c:97-221 with every node executing on the GPU.  No CPU compute path exists here.
 #include <cuda_runtime.h>
-#include <dlfcn.h>
 #include <unistd.h>
 
 #include <algorithm>
@@ -66,64 +65,18 @@ struct HostReg
 };
 
 // One context per GPU.  A multi-GPU context (tb200_context_create_multi, SURVEY.md 8(e)) is the context of GPU 0 plus `peers`
-// (GPUs 1..R-1), all driven by the calling thread; `comms` are the ncclComm_t of ncclCommInitAll over the group.
+// (GPUs 1..R-1), all driven by the calling thread.
 struct tb200_context
 {
     int device;
     int num_sms;
     cudaStream_t stream;
     std::vector<tb200_context*> peers;
-    std::vector<void*> comms; // [R] when NCCL is in use
-    const char* bcast_kind = "none";
     std::vector<HostReg> host_regs;
     std::vector<const void*> host_reg_failed;
     void* fixq = nullptr; // scratch of the GEMM kernels' deferred rare path: FIXQ_CAP entries per SM (gemm_tcgen05.cu)
 };
 static constexpr int FIXQ_CAP = 4096;
-// TB200_DEBUG_STAGES=1: progress lines of the multi-GPU set-up on stderr (which call a hang or an error sits in)
-#define STAGE(...)                                                                  \
-    do                                                                              \
-    {                                                                               \
-        static const bool on_ = getenv("TB200_DEBUG_STAGES") != nullptr;             \
-        if (on_) fprintf(stderr, "tengine_b200 stage: " __VA_ARGS__), fputc('\n', stderr), fflush(stderr); \
-    } while (0)
-
-// ---- NCCL, loaded at run time (libnccl.so.2: the copy torch already mapped when running under Python, the system one
-//      otherwise) so that single-GPU users never need it.  Only what the one broadcast at prerun needs. ----
-struct NcclApi
-{
-    void* handle = nullptr;
-    int (*CommInitAll)(void**, int, const int*) = nullptr;
-    int (*CommDestroy)(void*) = nullptr;
-    int (*GroupStart)() = nullptr;
-    int (*GroupEnd)() = nullptr;
-    int (*Broadcast)(const void*, void*, size_t, int, int, void*, cudaStream_t) = nullptr;
-    const char* (*GetErrorString)(int) = nullptr;
-    bool ok = false;
-};
-static NcclApi* nccl_api()
-{
-    static NcclApi api;
-    static bool tried = false;
-    if (tried) return api.ok ? &api : nullptr;
-    tried = true;
-    if (getenv("TB200_NO_NCCL")) return nullptr;
-    // TB200_NCCL_LIB names the copy to use; else whatever "libnccl.so.2" resolves to -- a copy the process has already mapped (the one
-    // torch bundles, when running under Python: tengine_b200/runtime.py maps it first on purpose) or the system one
-    const char* forced = getenv("TB200_NCCL_LIB");
-    if (forced && *forced) api.handle = dlopen(forced, RTLD_NOW | RTLD_GLOBAL);
-    for (const char* name : {"libnccl.so.2", "libnccl.so"})
-        if (!api.handle) api.handle = dlopen(name, RTLD_NOW | RTLD_GLOBAL);
-    if (!api.handle) return nullptr;
-    api.CommInitAll = (int (*)(void**, int, const int*))dlsym(api.handle, "ncclCommInitAll");
-    api.CommDestroy = (int (*)(void*))dlsym(api.handle, "ncclCommDestroy");
-    api.GroupStart = (int (*)())dlsym(api.handle, "ncclGroupStart");
-    api.GroupEnd = (int (*)())dlsym(api.handle, "ncclGroupEnd");
-    api.Broadcast = (int (*)(const void*, void*, size_t, int, int, void*, cudaStream_t))dlsym(api.handle, "ncclBroadcast");
-    api.GetErrorString = (const char* (*)(int))dlsym(api.handle, "ncclGetErrorString");
-    api.ok = api.CommInitAll && api.CommDestroy && api.GroupStart && api.GroupEnd && api.Broadcast && api.GetErrorString;
-    return api.ok ? &api : nullptr;
-}
 
 enum StepKind
 {
@@ -346,16 +299,14 @@ int tb200_context_create(int cuda_device, tb200_context** out)
 }
 
 // SURVEY.md 8(e): one process drives R GPUs; the batch of every run is cut into R contiguous slices of dim 0.  The packed
-// weight arena is built once (GPU 0) and reaches the other GPUs by ONE grouped ncclBroadcast at prerun (communicators from
-// ncclCommInitAll); there is no collective in the steady state.  A device listed twice (tests on a one-GPU box) rules NCCL
-// out (it refuses duplicate devices): the arena then travels by cudaMemcpyPeerAsync, everything else is identical.
+// weight arena is built once (GPU 0) and reaches the other GPUs by one cudaMemcpyPeerAsync per GPU at prerun; there is no
+// collective in the steady state.  A device may be listed more than once (tests on a one-GPU box).
 int tb200_context_create_multi(const int* cuda_devices, int num_devices, tb200_context** out)
 {
     if (!out || !cuda_devices || num_devices < 1 || num_devices > 64) return fail(TB200_ERR_INVALID, "bad device list");
     tb200_context* root = nullptr;
     int rc = context_create_one(cuda_devices[0], &root);
     if (rc) return rc;
-    bool distinct = true;
     for (int i = 1; i < num_devices; i++)
     {
         tb200_context* p = nullptr;
@@ -365,27 +316,8 @@ int tb200_context_create_multi(const int* cuda_devices, int num_devices, tb200_c
             return rc;
         }
         root->peers.push_back(p);
-        for (int j = 0; j < i; j++) distinct &= cuda_devices[j] != cuda_devices[i];
     }
-    if (num_devices > 1)
-    {
-        root->bcast_kind = "memcpy_peer";
-        NcclApi* nc = distinct ? nccl_api() : nullptr;
-        if (nc)
-        {
-            std::vector<void*> comms(num_devices, nullptr);
-            STAGE("ncclCommInitAll over %d devices ...", num_devices);
-            const int r = nc->CommInitAll(comms.data(), num_devices, cuda_devices);
-            STAGE("ncclCommInitAll -> %d", r);
-            if (r == 0)
-                root->comms = comms, root->bcast_kind = "nccl";
-            else
-                fprintf(stderr, "tengine_b200: ncclCommInitAll failed (%s); the weight arena will be broadcast with cudaMemcpyPeer\n", nc->GetErrorString(r));
-        }
-        else if (distinct && !getenv("TB200_NO_NCCL"))
-            fprintf(stderr, "tengine_b200: libnccl.so.2 not found; the weight arena will be broadcast with cudaMemcpyPeer\n");
-        cudaSetDevice(cuda_devices[0]);
-    }
+    cudaSetDevice(cuda_devices[0]);
     *out = root;
     return 0;
 }
@@ -394,10 +326,6 @@ int tb200_context_destroy(tb200_context* ctx)
 {
     if (!ctx) return 0;
     host_unregister_all(ctx);
-    if (!ctx->comms.empty())
-        if (NcclApi* nc = nccl_api())
-            for (void* c : ctx->comms)
-                if (c) nc->CommDestroy(c);
     for (tb200_context* p : ctx->peers) tb200_context_destroy(p);
     cudaSetDevice(ctx->device);
     cudaStreamDestroy(ctx->stream);
@@ -423,7 +351,7 @@ void* tb200_context_stream_of(tb200_context* ctx, int index)
     tb200_context* c = context_of(ctx, index);
     return c ? (void*)c->stream : nullptr;
 }
-const char* tb200_context_broadcast_kind(tb200_context* ctx) { return ctx ? ctx->bcast_kind : "none"; }
+const char* tb200_context_broadcast_kind(tb200_context* ctx) { return ctx && !ctx->peers.empty() ? "memcpy_peer" : "none"; }
 
 void* tb200_host_alloc(size_t bytes)
 {
@@ -1834,42 +1762,20 @@ static inline size_t active_nchw_bytes(const tb200_graph* g, const TensorInfo& t
     return g->num_images == g->prep_images ? t.nchw_bytes : t.nchw_bytes / (size_t)t.d.dims[0] * (size_t)g->num_images;
 }
 
-// One ncclBroadcast of the packed arena from GPU 0 to every other GPU of the group (grouped: one call per device from this
-// single thread), or peer copies when NCCL is not in use.
+// The packed arena from GPU 0 to every other GPU of the group: one peer copy per shard, all on the root's stream.
 static int broadcast_arena(tb200_graph* g)
 {
     tb200_context* root = g->ctx;
     if (g->shards.empty()) return 0;
     CUDA_OK(cudaSetDevice(root->device));
     CUDA_OK(cudaStreamSynchronize(root->stream));
-    NcclApi* nc = root->comms.empty() ? nullptr : nccl_api();
-    if (nc)
+    for (size_t i = 0; i < g->shards.size(); i++)
     {
-        STAGE("grouped ncclBroadcast of %zu bytes ...", g->w_bytes);
-        int r = nc->GroupStart();
-        if (r == 0) r = nc->Broadcast(g->w_arena, g->w_arena, g->w_bytes, /*ncclUint8*/ 1, 0, root->comms[0], root->stream);
-        for (size_t i = 0; r == 0 && i < g->shards.size(); i++)
-        {
-            tb200_graph* sh = g->shards[i];
-            if (sh->w_bytes != g->w_bytes) return fail(TB200_ERR_INVALID, "shard %d planned a different weight arena (%zu vs %zu bytes)", (int)i + 1, sh->w_bytes, g->w_bytes);
-            r = nc->Broadcast(sh->w_arena, sh->w_arena, sh->w_bytes, 1, 0, root->comms[i + 1], sh->ctx->stream);
-        }
-        const int r2 = nc->GroupEnd();
-        STAGE("ncclGroupEnd -> %d / %d", r, r2);
-        if (r || r2) return fail(TB200_ERR_CUDA, "ncclBroadcast of the weight arena failed: %s", nc->GetErrorString(r ? r : r2));
+        tb200_graph* sh = g->shards[i];
+        if (sh->w_bytes != g->w_bytes) return fail(TB200_ERR_INVALID, "shard %d planned a different weight arena (%zu vs %zu bytes)", (int)i + 1, sh->w_bytes, g->w_bytes);
+        CUDA_OK(cudaMemcpyPeerAsync(sh->w_arena, sh->ctx->device, g->w_arena, root->device, g->w_bytes, root->stream));
     }
-    else
-    {
-        for (size_t i = 0; i < g->shards.size(); i++)
-        {
-            tb200_graph* sh = g->shards[i];
-            if (sh->w_bytes != g->w_bytes) return fail(TB200_ERR_INVALID, "shard %d planned a different weight arena", (int)i + 1);
-            CUDA_OK(cudaMemcpyPeerAsync(sh->w_arena, sh->ctx->device, g->w_arena, root->device, g->w_bytes, root->stream));
-        }
-    }
-    CUDA_OK(cudaSetDevice(root->device));
     CUDA_OK(cudaStreamSynchronize(root->stream));
-    STAGE("broadcast: root stream drained");
     for (tb200_graph* sh : g->shards)
     {
         CUDA_OK(cudaSetDevice(sh->ctx->device));

@@ -131,38 +131,6 @@ def device_count():
     return lib().tb200_device_count()
 
 
-_nccl_preloaded = False
-
-
-def _preload_bundled_nccl():
-    """The library dlopen()s "libnccl.so.2" when a context spans distinct GPUs.  In a Python process that imports torch LATER, that
-    must be the NCCL build torch was linked against (its wheel bundles one): with the system copy mapped first, `import torch` fails
-    on a missing symbol (seen on a 2-GPU box: torch 2.11 wants ncclDevCommCreate of NCCL 2.28, /usr/lib has 2.27).  So map the
-    bundled copy first, when there is one; dlopen by soname then returns it.  TB200_NCCL_LIB=<path> overrides."""
-    global _nccl_preloaded
-    if _nccl_preloaded:
-        return
-    _nccl_preloaded = True
-    path = os.environ.get("TB200_NCCL_LIB")
-    if not path:
-        try:
-            import importlib.util
-
-            spec = importlib.util.find_spec("nvidia")
-            for base in (spec.submodule_search_locations if spec else []):
-                cand = os.path.join(base, "nccl", "lib", "libnccl.so.2")
-                if os.path.exists(cand):
-                    path = cand
-                    break
-        except Exception:
-            path = None
-    if path:
-        try:
-            C.CDLL(path, mode=C.RTLD_GLOBAL)
-        except OSError:
-            pass
-
-
 class Context:
     """interface->init / release_device: binds one GPU, or (devices=[...]) a group of GPUs driven by this process over
     which every graph shards its batch (tb200_context_create_multi)."""
@@ -173,8 +141,6 @@ class Context:
             _check(lib().tb200_context_create(int(device), C.byref(self.h)))
             self.devices = [int(device)]
         else:
-            if len(set(int(d) for d in devices)) > 1:
-                _preload_bundled_nccl()
             arr = (C.c_int * len(devices))(*[int(d) for d in devices])
             _check(lib().tb200_context_create_multi(arr, len(devices), C.byref(self.h)))
             self.devices = [int(d) for d in devices]

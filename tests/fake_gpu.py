@@ -12,7 +12,7 @@ class FakeContext:
     def __init__(self, device=0, devices=None):
         self.devices = [int(device)] if devices is None else [int(d) for d in devices]
         self.device = self.devices[0]
-        self.broadcast_kind = "nccl" if len(self.devices) > 1 else "none"
+        self.broadcast_kind = "memcpy_peer" if len(self.devices) > 1 else "none"
 
     def stream_of(self, i):
         return 1000 + i
