@@ -13,8 +13,9 @@
 //   WG1, warps 4-7: MMA.  One accumulator stage (mt m-tiles x block_n columns) in registers: per m-tile and k-step two
 //                   m64n<block_n>k32, rows 0-63 and 64-127; one commit group in flight, a ring stage is released when the
 //                   group after it has been committed and the one reading it has completed.  At the end of the stage the
-//                   fragments go into the accumulator image ([128 rows][mt * block_n] s32 in shared memory) as soon as the
-//                   epilogue has read the previous stage out of it (mbarriers img_empty / img_full).
+//                   fragments go into the accumulator image ([128 rows][mt * block_n] s32 in shared memory) quarter by quarter:
+//                   32-row quarter q is written by two MMA warps as soon as its two epilogue warps have read the previous stage
+//                   out of it (mbarriers img_empty[q] / img_full[q]), so no warp waits for the whole CTA at the hand-over.
 //   WG2-3, warps 8-15: epilogue.  Two warps per 32-row quarter of the image; a warp owns whole "store groups" = 32 rows x
 //                   16/32 channels: image -> registers -> requant_fast4_i8 -> bytes -> its own swizzled smem buffer -> ONE
 //                   TMA store per group (cp.async.bulk.tensor, double-buffered).  No address arithmetic for the stores,
@@ -125,7 +126,9 @@ struct __align__(16) GemmSmemCtl
     uint64_t full[MAX_STAGES], empty[MAX_STAGES];
     uint64_t b_full; // resident-B mode: all k-blocks of the N tile's weights have landed
     uint64_t sx_full[2], sx_empty[2]; // uint8 row sums of stage s published by the row-sum warps / read by the epilogue
-    uint64_t img_full, img_empty;     // the accumulator image holds a complete stage (MMA -> epilogue) / has been read (epilogue -> MMA)
+    // per 32-row quarter q of the accumulator image: its rows of the stage are written (the two MMA warps of q -> epilogue) /
+    // have been read (the two epilogue warps of q -> MMA)
+    uint64_t img_full[4], img_empty[4];
 };
 
 // named barrier 1 over the epilogue warps only (the MMA warpgroup never joins it)
@@ -374,9 +377,10 @@ __device__ __forceinline__ uint32_t padding_taps(const GemmArgs& g, int mt, int 
 // m64nBNk32, rows 0-63 and 64-127, into MT * BN s32 registers per thread.  One commit group per k-block stays in flight: after
 // committing k-block kb the warpgroup waits for the group of kb - 1 and releases the ring stage that group read; the pipe is
 // drained (wait_group 0) only at the end of the stage.  The registers are the second accumulator buffer: while this stage is
-// multiplied the epilogue drains the previous one from the image; the fragments are then written into the image once every
-// epilogue warp has read it (img_empty) and published with img_full.  BN, MT and the operand signs are template parameters so
-// that the accumulators are indexed statically and no wgmma sits in a branch the compiler cannot prove uniform.
+// multiplied the epilogue drains the previous one from the image; the fragments are then written into each 32-row quarter of the
+// image once that quarter's two epilogue warps have read it (img_empty[q]) and published with img_full[q].  BN, MT and the operand
+// signs are template parameters so that the accumulators are indexed statically and no wgmma sits in a branch the compiler cannot
+// prove uniform.
 template <bool AU, bool BU, int BN, int MT, typename Log>
 __device__ __forceinline__ void gemm_mma(const GemmArgs& g, GemmSmemCtl* ctl, uint8_t* smem, uint32_t stage_bytes, uint32_t b_res_base,
                                          uint32_t img_base, uint32_t img_pitch, Log&& tlog)
@@ -435,22 +439,33 @@ __device__ __forceinline__ void gemm_mma(const GemmArgs& g, GemmSmemCtl* ctl, ui
 #pragma unroll
                 for (int r = 0; r < NR; r++) reg_fence(acc[i][h][r]);
         tlog(1, 0);
-        mbar_wait(&ctl->img_empty, iphase ^ 1); // every epilogue warp has read the previous stage out of the image
-        tlog(1, 1);
+        // Hand the stage over per 32-row image quarter.  Warp w of the warpgroup holds rows 16w..16w+15 of each half h, i.e. half of
+        // quarter q = 2h + w/2; warp w ^ 1 holds the other half, and only epilogue warps 8 + q and 12 + q read it.  So each quarter
+        // waits for its own two readers only, not for the slowest of all eight.
+        const int wq = (threadIdx.x >> 6) & 1; // w / 2
 #pragma unroll
-        for (int i = 0; i < MT; i++)
+        for (int h = 0; h < 2; h++)
         {
-            if (i >= mtc) break;
+            const int q = 2 * h + wq;
+            mbar_wait(&ctl->img_empty[q], iphase ^ 1); // both epilogue warps of quarter q have read the previous stage out of it
+            if (h == 0) tlog(1, 1);
 #pragma unroll
-            for (int h = 0; h < 2; h++)
+            for (int i = 0; i < MT; i++)
+            {
+                if (i >= mtc) break;
 #pragma unroll
                 for (int c = 0; c < BN / 16; c++)
                     frag_to_image(*reinterpret_cast<const uint32_t(*)[8]>(&acc[i][h][8 * c]), img_base, img_pitch, h * 64, i * BN + c * 16);
+            }
+            __syncwarp();
+            if ((threadIdx.x & 31) == 0) mbar_arrive(&ctl->img_full[q]); // (release) this warp's rows of quarter q are in the image
         }
-        __syncwarp();
-        if ((threadIdx.x & 31) == 0) mbar_arrive(&ctl->img_full); // (release) this warp's rows of the stage are in the image
         tlog(1, 2);
         iphase ^= 1;
+        // The four warps leave these waits at different times and need no barrier among themselves before the next stage's
+        // wgmma_fence: wgmma.fence / mma_async / commit / wait are .sync.aligned warpgroup-collective instructions that the
+        // hardware synchronises across the four warps, just as after the ring's full-barrier waits, which each warp leaves on
+        // its own too.
     }
 }
 
@@ -518,7 +533,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
         for (int s = 0; s < g.stages; s++) mbar_init(&ctl->full[s], 1), mbar_init(&ctl->empty[s], 1 + sumw);
         for (int s = 0; s < 2; s++) mbar_init(&ctl->sx_full[s], sumw ? sumw : 1), mbar_init(&ctl->sx_empty[s], EPI_WARPS);
         mbar_init(&ctl->b_full, 1);
-        mbar_init(&ctl->img_full, 4), mbar_init(&ctl->img_empty, EPI_WARPS);
+        for (int q = 0; q < 4; q++) mbar_init(&ctl->img_full[q], 2), mbar_init(&ctl->img_empty[q], 2);
         s_fixq.q = g.fixq ? g.fixq + (size_t)blockIdx.x * g.fixq_cap : nullptr, s_fixq.cap = (uint32_t)g.fixq_cap, s_fixq.count = 0;
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
@@ -654,8 +669,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
         // Image quarter q (rows 32q..32q+31) is served by the two warps {8 + q, 12 + q}.  The work of an accumulator stage is cut
         // into store groups (m-tile i, columns [grp*16*cs, (grp+1)*16*cs)) of 32 rows each, dealt round-robin to the quarter's
         // warps.  A warp requantises its group chunk by chunk (16 columns per load, the next chunk's load in flight), writes the
-        // bytes to its own swizzled staging buffer and hands the buffer to the TMA unit with one store.  It releases the image to
-        // the MMA warpgroup (img_empty) as soon as it has issued its last load of the stage.
+        // bytes to its own swizzled staging buffer and hands the buffer to the TMA unit with one store.  It releases its quarter
+        // of the image to the MMA warpgroup (img_empty[q]) as soon as it has issued its last load of the stage; a warp with no group
+        // in the stage, or whose quarter has no valid rows, arrives at the end of the stage, so each warp arrives once per stage.
         setmaxnreg_inc<REG_EPI>();
         const int ew = warp - EPI_WARP0; // epilogue warp 0..7
         const int q = warp & 3;
@@ -698,7 +714,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
                 epilogue_bar_sync();
                 par_s = par_base;
             }
-            mbar_wait(&ctl->img_full, iphase); // the image holds this stage
+            mbar_wait(&ctl->img_full[q], iphase); // this warp's quarter of the image holds this stage
             iphase ^= 1;
             if (U8 && g.cplane) mbar_wait(&ctl->sx_full[as], aphase); // the row sums of this stage
             TLOG_E(0);
@@ -750,7 +766,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
                         if (i2 >= mtc)
                         {
                             __syncwarp();
-                            if (lane == 0) mbar_arrive(&ctl->img_empty);
+                            if (lane == 0) mbar_arrive(&ctl->img_empty[q]);
                             released = true;
                         }
                     };
@@ -800,7 +816,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
             __syncwarp();
             if (lane == 0)
             {
-                if (!released) mbar_arrive(&ctl->img_empty); // a warp without a group in this stage
+                if (!released) mbar_arrive(&ctl->img_empty[q]); // a warp without a group in this stage (or a quarter without valid rows)
                 mbar_arrive(&ctl->sx_empty[as]);             // stage drained: the row-sum warps may overwrite its sums
             }
             TLOG_E(2);

@@ -6,9 +6,10 @@
 # must fail every tie-dense case of a fast epilogue (exact-epilogue, LUT and tb200k_* cases still pass).  Never shipped.
 set -e
 cd "$(dirname "$0")/../tengine_b200/csrc"
-mkdir -p ../../build/nofix
+rm -rf ../../build/nofix && mkdir -p ../../build/nofix
 FLAGS="-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-fvisibility=hidden --expt-relaxed-constexpr -DTB200_TIE_EPS=-1.0f"
-for f in engine kernels_direct gemm_tcgen05 dw_tma conv_window yolo_detect conv_fp32; do nvcc $FLAGS -c $f.cu -o ../../build/nofix/$f.o & done
-wait
-nvcc -gencode arch=compute_90a,code=sm_90a -shared -o ../../build/nofix/libtengine_b200_nofix.so ../../build/nofix/*.o -ldl
+SRCS=$(sed -n 's/^SRCS := //p' Makefile) # every source of the product library, so that the build links completely
+for f in $SRCS; do nvcc $FLAGS -c $f -o ../../build/nofix/${f%.cu}.o & done
+for j in $(jobs -p); do wait $j; done # (set -e: a failed compile stops the script)
+nvcc -gencode arch=compute_90a,code=sm_90a -shared -o ../../build/nofix/libtengine_b200_nofix.so ../../build/nofix/*.o -ldl -Xlinker --no-undefined
 echo built build/nofix/libtengine_b200_nofix.so
