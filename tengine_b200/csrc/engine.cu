@@ -64,19 +64,24 @@ struct HostReg
     bool ours; // false: the range was already page-locked by the application (cudaHostAlloc / its own registration)
 };
 
-// One context per GPU.  A multi-GPU context (tb200_context_create_multi, SURVEY.md 8(e)) is the context of GPU 0 plus `peers`
-// (GPUs 1..R-1), all driven by the calling thread.
-struct tb200_context
+// One GPU of a context.
+struct Gpu
 {
     int device;
     int num_sms;
     cudaStream_t stream;
-    std::vector<tb200_context*> peers;
-    std::vector<HostReg> host_regs;
-    std::vector<const void*> host_reg_failed;
     void* fixq = nullptr; // scratch of the GEMM kernels' deferred rare path: FIXQ_CAP entries per SM (gemm_tcgen05.cu)
 };
 static constexpr int FIXQ_CAP = 4096;
+
+// A group of GPUs driven by the calling thread (tb200_context_create_multi, SURVEY.md 8(e)); tb200_context_create makes a group
+// of one.  gpus[0] is GPU 0.  The registrations of caller memory serve every GPU of the group.
+struct tb200_context
+{
+    std::vector<Gpu> gpus;
+    std::vector<HostReg> host_regs;
+    std::vector<const void*> host_reg_failed;
+};
 
 enum StepKind
 {
@@ -185,13 +190,13 @@ struct BatchPlan
     int num_launches = 0;
 };
 
-struct tb200_graph
+// One GPU's part of a graph: the plan of its slice of the batch, planned from its own descriptors, and what runs it there.
+struct Shard
 {
-    tb200_context* ctx;
-    int flags;
+    const Gpu* gpu;
+    int flags; // those of prerun
     std::vector<TensorInfo> tensors;
     std::vector<tb200_layer_desc> layers;
-    std::vector<const char*> layer_kernel;
     std::vector<LayerPlan> plan;
     std::vector<int> input_ids, output_ids;
     std::vector<uint8_t*> in_nchw_dev, out_nchw_dev;
@@ -199,20 +204,16 @@ struct tb200_graph
     size_t act_bytes = 0;
     uint8_t* w_arena = nullptr;
     size_t w_bytes = 0;
+    size_t act_unshared_bytes = 0; // what the arena would need without slot reuse (introspection)
     // tb200_graph_set_batch: `prepared` covers the batch of prerun, `other` the most recent smaller one; `cur` is the active one
     BatchPlan prepared, other;
     BatchPlan* cur = &prepared;
-    int other_batch = 0; // the active batch `other` was built for (root; 0: none)
     cudaStream_t copy_stream = nullptr, d2h_stream = nullptr;
     std::vector<cudaEvent_t> ev_in, ev_out;
     cudaEvent_t ev_done = nullptr;
-    // batch sharding over the GPUs of a multi-GPU context: this graph is the shard of GPU 0 and owns the others.
     // first_image / num_images: the shard's part of the active batch (num_images may be 0); prep_images: its part of the batch
-    // of prerun, the dim 0 of its tensors; total_images: that batch; batch: the active one (root)
-    std::vector<tb200_graph*> shards;
-    int first_image = 0, num_images = 0, prep_images = 0, total_images = 0, batch = 0;
-    size_t act_unshared_bytes = 0; // what the arena would need without slot reuse (introspection)
-    int pack_cache_state = 0;      // 0 no cache directory, 1 packed and written, 2 read from the cache
+    // of prerun, the dim 0 of its tensors
+    int first_image = 0, num_images = 0, prep_images = 0;
     // tb200_graph_upload_images: device copy of this shard's pixel span, its image descriptors (staged through page-locked host
     // memory that is rewritten only after img_ev, the previous descriptor copy, has completed); grown on demand
     uint8_t* img_stage = nullptr;
@@ -220,6 +221,17 @@ struct tb200_graph
     ImageDesc *img_desc = nullptr, *img_desc_host = nullptr;
     int img_desc_cap = 0;
     cudaEvent_t img_ev = nullptr;
+};
+
+// The batch is cut over the GPUs of the context: shard r runs on ctx->gpus[r].
+struct tb200_graph
+{
+    tb200_context* ctx;
+    std::vector<Shard> shards; // sized once at prerun: a shard's `cur` points into the shard
+    std::vector<const char*> layer_kernel; // decided by prerun from shard 0's launch sequence at the prepared batch
+    int batch = 0, prepared_batch = 0; // the active batch and that of prerun
+    int other_batch = 0;               // the active batch the shards' `other` plans were built for (0: none)
+    int pack_cache_state = 0;          // 0 no cache directory, 1 packed and written, 2 read from the cache
 };
 
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
@@ -258,7 +270,8 @@ int tb200_device_count(void)
     return good;
 }
 
-static int context_create_one(int cuda_device, tb200_context** out)
+// Adds GPU cuda_device to the group; it is current afterwards.
+static int add_gpu(tb200_context* ctx, int cuda_device)
 {
     int n = 0;
     if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0)
@@ -273,14 +286,10 @@ static int context_create_one(int cuda_device, tb200_context** out)
     CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, cuda_device));
     if (major != 9 || minor != 0) return fail(TB200_ERR_NO_DEVICE, "device %d is sm_%d%d; this backend is built for sm_90a only", cuda_device, major, minor);
     CUDA_OK(cudaSetDevice(cuda_device));
-    cudaStream_t st;
-    CUDA_OK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-    tb200_context* c = new tb200_context();
-    c->device = cuda_device;
-    c->num_sms = sms;
-    c->stream = st;
-    CUDA_OK(cudaMalloc(&c->fixq, (size_t)sms * FIXQ_CAP * 16));
-    *out = c;
+    Gpu gpu{cuda_device, sms, nullptr};
+    CUDA_OK(cudaStreamCreateWithFlags(&gpu.stream, cudaStreamNonBlocking));
+    ctx->gpus.push_back(gpu);
+    CUDA_OK(cudaMalloc(&ctx->gpus.back().fixq, (size_t)sms * FIXQ_CAP * 16));
     return 0;
 }
 
@@ -295,7 +304,7 @@ static void host_unregister_all(tb200_context* ctx)
 int tb200_context_create(int cuda_device, tb200_context** out)
 {
     if (!out) return fail(TB200_ERR_INVALID, "null out");
-    return context_create_one(cuda_device, out);
+    return tb200_context_create_multi(&cuda_device, 1, out);
 }
 
 // SURVEY.md 8(e): one process drives R GPUs; the batch of every run is cut into R contiguous slices of dim 0.  The packed
@@ -304,21 +313,15 @@ int tb200_context_create(int cuda_device, tb200_context** out)
 int tb200_context_create_multi(const int* cuda_devices, int num_devices, tb200_context** out)
 {
     if (!out || !cuda_devices || num_devices < 1 || num_devices > 64) return fail(TB200_ERR_INVALID, "bad device list");
-    tb200_context* root = nullptr;
-    int rc = context_create_one(cuda_devices[0], &root);
-    if (rc) return rc;
-    for (int i = 1; i < num_devices; i++)
-    {
-        tb200_context* p = nullptr;
-        if ((rc = context_create_one(cuda_devices[i], &p)) != 0)
+    tb200_context* ctx = new tb200_context();
+    for (int i = 0; i < num_devices; i++)
+        if (const int rc = add_gpu(ctx, cuda_devices[i]))
         {
-            tb200_context_destroy(root);
+            tb200_context_destroy(ctx);
             return rc;
         }
-        root->peers.push_back(p);
-    }
     cudaSetDevice(cuda_devices[0]);
-    *out = root;
+    *out = ctx;
     return 0;
 }
 
@@ -326,32 +329,27 @@ int tb200_context_destroy(tb200_context* ctx)
 {
     if (!ctx) return 0;
     host_unregister_all(ctx);
-    for (tb200_context* p : ctx->peers) tb200_context_destroy(p);
-    cudaSetDevice(ctx->device);
-    cudaStreamDestroy(ctx->stream);
-    if (ctx->fixq) cudaFree(ctx->fixq);
+    for (size_t i = ctx->gpus.size(); i-- > 0;) // GPU 0 last: it is current afterwards
+    {
+        cudaSetDevice(ctx->gpus[i].device);
+        cudaStreamDestroy(ctx->gpus[i].stream);
+        if (ctx->gpus[i].fixq) cudaFree(ctx->gpus[i].fixq);
+    }
     delete ctx;
     return 0;
 }
 
-void* tb200_context_stream(tb200_context* ctx) { return ctx ? (void*)ctx->stream : nullptr; }
-int tb200_context_num_gpus(tb200_context* ctx) { return ctx ? 1 + (int)ctx->peers.size() : 0; }
-static tb200_context* context_of(tb200_context* ctx, int index)
-{
-    if (!ctx || index < 0 || index > (int)ctx->peers.size()) return nullptr;
-    return index == 0 ? ctx : ctx->peers[index - 1];
-}
+void* tb200_context_stream(tb200_context* ctx) { return ctx ? (void*)ctx->gpus[0].stream : nullptr; }
+int tb200_context_num_gpus(tb200_context* ctx) { return ctx ? (int)ctx->gpus.size() : 0; }
 int tb200_context_gpu(tb200_context* ctx, int index)
 {
-    tb200_context* c = context_of(ctx, index);
-    return c ? c->device : -1;
+    return ctx && index >= 0 && index < (int)ctx->gpus.size() ? ctx->gpus[index].device : -1;
 }
 void* tb200_context_stream_of(tb200_context* ctx, int index)
 {
-    tb200_context* c = context_of(ctx, index);
-    return c ? (void*)c->stream : nullptr;
+    return ctx && index >= 0 && index < (int)ctx->gpus.size() ? (void*)ctx->gpus[index].stream : nullptr;
 }
-const char* tb200_context_broadcast_kind(tb200_context* ctx) { return ctx && !ctx->peers.empty() ? "memcpy_peer" : "none"; }
+const char* tb200_context_broadcast_kind(tb200_context* ctx) { return ctx && ctx->gpus.size() > 1 ? "memcpy_peer" : "none"; }
 
 void* tb200_host_alloc(size_t bytes)
 {
@@ -378,17 +376,17 @@ int tb200k_cpad(int channels) { return cpad(channels); }
 // inside the stale registration and run past it, and CUDA refuses the copy (invalid argument).  Then every GPU of the group finishes
 // its queued work, all of this context's registrations are dropped and the copy is issued once more; registrations come back as
 // buffers are seen again.
-static cudaError_t host_copy(tb200_context* root, void* dst, const void* src, size_t bytes, cudaMemcpyKind kind, cudaStream_t st)
+static cudaError_t host_copy(tb200_context* ctx, void* dst, const void* src, size_t bytes, cudaMemcpyKind kind, cudaStream_t st)
 {
     cudaError_t e = cudaMemcpyAsync(dst, src, bytes, kind, st);
-    if (e != cudaErrorInvalidValue || root->host_regs.empty()) return e;
+    if (e != cudaErrorInvalidValue || ctx->host_regs.empty()) return e;
     cudaGetLastError();
     int dev = 0;
     cudaGetDevice(&dev);
-    for (int k = 0; k <= (int)root->peers.size(); k++)
-        if (cudaSetDevice(context_of(root, k)->device) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) cudaGetLastError();
+    for (const Gpu& gpu : ctx->gpus)
+        if (cudaSetDevice(gpu.device) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) cudaGetLastError();
     cudaSetDevice(dev);
-    host_unregister_all(root);
+    host_unregister_all(ctx);
     return cudaMemcpyAsync(dst, src, bytes, kind, st);
 }
 
@@ -460,7 +458,7 @@ static size_t gemm_weight_bytes(int ocp, int k)
     return (size_t)nt * bn * k;
 }
 
-static int run_step(tb200_graph* g, const Step& s, cudaStream_t st)
+static int run_step(const Shard* g, const Step& s, cudaStream_t st)
 {
     cudaError_t err = cudaSuccess;
     switch (s.kind)
@@ -469,15 +467,15 @@ static int run_step(tb200_graph* g, const Step& s, cudaStream_t st)
     case K_NHWC2NCHW: err = launch_nhwc_to_nchw(s.in, s.out, s.n, s.c, s.h, s.w_, st); break;
     case K_CONV_STEM: err = launch_conv_stem(s.in, s.w, s.out, s.cs, s.epi, st); break;
     case K_GATHER_TC:
-        err = s.wp.valid ? launch_conv_window(s.wp, s.w, s.out, s.cs, s.epi, g->ctx->num_sms, st)
-                         : launch_conv_gather_tc(s.in, s.w, s.out, s.cs, s.epi, s.nhwc16, g->ctx->num_sms, st);
+        err = s.wp.valid ? launch_conv_window(s.wp, s.w, s.out, s.cs, s.epi, g->gpu->num_sms, st)
+                         : launch_conv_gather_tc(s.in, s.w, s.out, s.cs, s.epi, s.nhwc16, g->gpu->num_sms, st);
         break;
     case K_CONV_DW:
         err = s.dwp.valid ? launch_conv_dw_tma(s.dwp, s.w, s.out, s.cs, s.epi, st) : launch_conv_dw(s.in, s.w, s.out, s.cs, s.epi, st);
         break;
     case K_CONV_DIRECT: err = launch_conv_direct(s.in, s.w, s.out, s.cs, s.epi, st); break;
     case K_GEMM:
-    case K_IGEMM: err = launch_gemm_i8(s.gemm, s.epi, s.btab, g->ctx->num_sms, st); break;
+    case K_IGEMM: err = launch_gemm_i8(s.gemm, s.epi, s.btab, g->gpu->num_sms, st); break;
     case K_POOL: err = launch_pool(s.in, s.out, s.ps, s.u8, st); break;
     case K_POINTWISE: err = launch_pointwise(s.in, s.in2, s.out, s.bytes, s.pp, s.u8, st); break;
     case K_CONCAT_PART:
@@ -509,27 +507,30 @@ static void destroy_batch_plan(BatchPlan& bp)
     bp = BatchPlan();
 }
 
+// Drains and frees every shard on its own GPU, past any failure, then the graph; GPU 0 is current afterwards.
 static void destroy_graph(tb200_graph* g)
 {
-    if (!g) return;
-    for (tb200_graph* sh : g->shards) destroy_graph(sh);
-    g->shards.clear();
-    cudaSetDevice(g->ctx->device);
-    destroy_batch_plan(g->prepared);
-    destroy_batch_plan(g->other);
-    for (auto e : g->ev_in) cudaEventDestroy(e);
-    for (auto e : g->ev_out) cudaEventDestroy(e);
-    if (g->ev_done) cudaEventDestroy(g->ev_done);
-    if (g->copy_stream) cudaStreamDestroy(g->copy_stream);
-    if (g->d2h_stream) cudaStreamDestroy(g->d2h_stream);
-    for (auto p : g->in_nchw_dev) cudaFree(p);
-    for (auto p : g->out_nchw_dev) cudaFree(p);
-    cudaFree(g->act_arena);
-    cudaFree(g->w_arena);
-    cudaFree(g->img_stage);
-    cudaFree(g->img_desc);
-    cudaFreeHost(g->img_desc_host);
-    if (g->img_ev) cudaEventDestroy(g->img_ev);
+    for (Shard& sh : g->shards)
+    {
+        cudaSetDevice(sh.gpu->device);
+        cudaStreamSynchronize(sh.gpu->stream);
+        destroy_batch_plan(sh.prepared);
+        destroy_batch_plan(sh.other);
+        for (auto e : sh.ev_in) cudaEventDestroy(e);
+        for (auto e : sh.ev_out) cudaEventDestroy(e);
+        if (sh.ev_done) cudaEventDestroy(sh.ev_done);
+        if (sh.copy_stream) cudaStreamDestroy(sh.copy_stream);
+        if (sh.d2h_stream) cudaStreamDestroy(sh.d2h_stream);
+        for (auto p : sh.in_nchw_dev) cudaFree(p);
+        for (auto p : sh.out_nchw_dev) cudaFree(p);
+        cudaFree(sh.act_arena);
+        cudaFree(sh.w_arena);
+        cudaFree(sh.img_stage);
+        cudaFree(sh.img_desc);
+        cudaFreeHost(sh.img_desc_host);
+        if (sh.img_ev) cudaEventDestroy(sh.img_ev);
+    }
+    cudaSetDevice(g->ctx->gpus[0].device);
     delete g;
 }
 
@@ -699,7 +700,7 @@ static void fuse_nodes(const tb200_layer_desc* layers, const tb200_tensor_desc* 
 }
 
 // ---- tensors ----
-static int setup_tensors(tb200_graph* g, const tb200_tensor_desc* tensors, int num_tensors, const int32_t* input_ids, int num_inputs, const int32_t* output_ids,
+static int setup_tensors(Shard* g, const tb200_tensor_desc* tensors, int num_tensors, const int32_t* input_ids, int num_inputs, const int32_t* output_ids,
                          int num_outputs)
 {
     g->tensors.resize(num_tensors);
@@ -777,7 +778,7 @@ static int plan_conv(int li, const tb200_layer_desc& L, const TensorInfo& tin, c
 }
 
 // Validates every layer, chooses its kernel and lays out the weight arena (g->w_bytes).
-static int plan_kernels(tb200_graph* g, std::vector<LayerPlan>& plan)
+static int plan_kernels(Shard* g, std::vector<LayerPlan>& plan)
 {
     const int num_layers = (int)g->layers.size(), num_tensors = (int)g->tensors.size();
     const bool no_tc = (g->flags & TB200_PRERUN_NO_TENSORCORE) != 0;
@@ -882,7 +883,7 @@ static int plan_kernels(tb200_graph* g, std::vector<LayerPlan>& plan)
 // ---- activation arena: one 1 KiB-aligned slot per tensor; a slot is handed on once the tensor's last consumer has run
 //      (first-fit over a coalescing free list, the role of source/device/cpu/cpu_pool.c:253-439).  Graph inputs and outputs
 //      keep their slots; with TB200_PRERUN_NO_GRAPH (debug: every intermediate stays readable) nothing is reused. ----
-static void plan_activation_arena(tb200_graph* g, std::vector<LayerPlan>& plan)
+static void plan_activation_arena(Shard* g, std::vector<LayerPlan>& plan)
 {
     const int num_layers = (int)g->layers.size(), num_tensors = (int)g->tensors.size();
     const bool reuse = !(g->flags & TB200_PRERUN_NO_GRAPH);
@@ -963,12 +964,12 @@ static void plan_activation_arena(tb200_graph* g, std::vector<LayerPlan>& plan)
 }
 
 // The arenas and the NCHW staging buffers of the graph's inputs and outputs.
-static int alloc_device_buffers(tb200_graph* g)
+static int alloc_device_buffers(Shard* g)
 {
     const size_t act = g->act_bytes;
     CUDA_OK(cudaMalloc(&g->act_arena, act ? act : 1024));
     // pad lanes of every tensor are (re)written by its producer; the initial fill only matters for debugging reads
-    CUDA_OK(cudaMemsetAsync(g->act_arena, (g->flags & TB200_PRERUN_POISON_ARENA) ? 0xA5 : 0, act ? act : 1024, g->ctx->stream));
+    CUDA_OK(cudaMemsetAsync(g->act_arena, (g->flags & TB200_PRERUN_POISON_ARENA) ? 0xA5 : 0, act ? act : 1024, g->gpu->stream));
     for (auto& t : g->tensors) t.dev = g->act_arena + t.off;
     CUDA_OK(cudaMalloc(&g->w_arena, g->w_bytes));
     for (int id : g->input_ids)
@@ -988,7 +989,7 @@ static int alloc_device_buffers(tb200_graph* g)
 
 // ---- the fast-epilogue proofs, per conv / FC layer.  Decided from the descriptors alone so that every rank of a sharded job
 //      reaches the same arena format. ----
-static void prove_fast_epilogues(const tb200_graph* g, std::vector<LayerPlan>& plan)
+static void prove_fast_epilogues(const Shard* g, std::vector<LayerPlan>& plan)
 {
     for (size_t li = 0; li < g->layers.size(); li++)
     {
@@ -1043,7 +1044,7 @@ static void prove_fast_epilogues(const tb200_graph* g, std::vector<LayerPlan>& p
 // Per-input requantisation of concat_kernel_ref_int8.c:70-80 (roundf(q * (s_in / s_out)), including its clamp of values below
 // -127 to +127) and concat_kernel_ref_uint8.c:82 (roundf((q - zp_in) * (s_in / s_out) + zp_out), the zero point inside the
 // rounding, clamp) as byte tables, 256 bytes per input.
-static void pack_concat_tables(const tb200_graph* g, const tb200_layer_desc& L, uint8_t* dst)
+static void pack_concat_tables(const Shard* g, const tb200_layer_desc& L, uint8_t* dst)
 {
     const tb200_tensor_desc& to = g->tensors[L.output].d;
     for (int k = 0; k < L.num_inputs && k < 4; k++)
@@ -1075,7 +1076,7 @@ static void pack_concat_tables(const tb200_graph* g, const tb200_layer_desc& L, 
 
 // x -> sigmoid(x) (its own requantisation, the Sigmoid node's output tensor) -> eltwise product with x.  L is the fused
 // product (it reads x), S the folded Sigmoid, `operand` the product's operand that S was.
-static void pack_silu_table(const tb200_graph* g, const tb200_layer_desc& L, const tb200_layer_desc& S, int operand, uint8_t* lut)
+static void pack_silu_table(const Shard* g, const tb200_layer_desc& L, const tb200_layer_desc& S, int operand, uint8_t* lut)
 {
     const tb200_tensor_desc &tx = g->tensors[L.inputs[0]].d, &ts = g->tensors[S.output].d, &to = g->tensors[L.output].d;
     const bool u8 = tx.data_type == TB200_DT_UINT8;
@@ -1219,7 +1220,7 @@ static void pack_epilogue_consts(const tb200_layer_desc& L, const LayerPlan& P, 
 }
 
 // Every layer's part of the arena image `img` (zero-filled, g->w_bytes).
-static void pack_arena_image(const tb200_graph* g, const std::vector<LayerPlan>& plan, uint8_t* img)
+static void pack_arena_image(const Shard* g, const std::vector<LayerPlan>& plan, uint8_t* img)
 {
     for (size_t li = 0; li < g->layers.size(); li++)
     {
@@ -1247,7 +1248,7 @@ static void pack_arena_image(const tb200_graph* g, const std::vector<LayerPlan>&
 }
 
 // TB200_DEBUG_HASH >= 2: the packed constants and hashes of every conv / FC layer's part of the arena image.
-static void debug_print_pack(const tb200_graph* g, const std::vector<LayerPlan>& plan, const uint8_t* img)
+static void debug_print_pack(const Shard* g, const std::vector<LayerPlan>& plan, const uint8_t* img)
 {
     for (size_t li = 0; li < g->layers.size(); li++)
     {
@@ -1274,7 +1275,7 @@ static void debug_print_pack(const tb200_graph* g, const std::vector<LayerPlan>&
 //      conv_kernel_x86.c:2137-2209, next to the tmfile).  What is hashed, and in which order, is part of the cache format. ----
 static const uint64_t kPackMagic = 0x3032424b43415054ull + TB200_PACK_FORMAT;
 
-static uint64_t pack_cache_key(const tb200_graph* g, const std::vector<LayerPlan>& plan)
+static uint64_t pack_cache_key(const Shard* g, const std::vector<LayerPlan>& plan)
 {
     uint64_t h = kFnvBasis;
     auto mix = [&](const void* p, size_t n) { h = fnv1a(p, n, h); };
@@ -1328,9 +1329,11 @@ static void pack_cache_store(const std::string& path, uint64_t key, const std::v
     }
 }
 
-// Fills the weight arena: from the pack cache when it holds this model, else by packing (and then storing it there).
-static int upload_weights(tb200_graph* g, const std::vector<LayerPlan>& plan)
+// Fills the weight arena of GPU 0: from the pack cache when it holds this model, else by packing (and then storing it there).
+static int upload_weights(tb200_graph* graph)
 {
+    const Shard* g = &graph->shards[0];
+    const std::vector<LayerPlan>& plan = g->plan;
     std::vector<uint8_t> img(g->w_bytes, 0);
     const std::string dir = pack_cache_dir();
     std::string cache_path;
@@ -1344,18 +1347,18 @@ static int upload_weights(tb200_graph* g, const std::vector<LayerPlan>& plan)
         cache_path = dir + name;
         cache_hit = pack_cache_load(cache_path, key, img);
     }
-    g->pack_cache_state = cache_path.empty() ? 0 : (cache_hit ? 2 : 1);
+    graph->pack_cache_state = cache_path.empty() ? 0 : (cache_hit ? 2 : 1);
     if (!cache_hit) pack_arena_image(g, plan, img.data());
     if (getenv("TB200_DEBUG_HASH") && atoi(getenv("TB200_DEBUG_HASH")) >= 2) debug_print_pack(g, plan, img.data());
     if (!cache_path.empty() && !cache_hit) pack_cache_store(cache_path, key, img);
-    CUDA_OK(host_copy(g->ctx, g->w_arena, img.data(), g->w_bytes, cudaMemcpyHostToDevice, g->ctx->stream));
-    CUDA_OK(cudaStreamSynchronize(g->ctx->stream));
+    CUDA_OK(host_copy(graph->ctx, g->w_arena, img.data(), g->w_bytes, cudaMemcpyHostToDevice, g->gpu->stream));
+    CUDA_OK(cudaStreamSynchronize(g->gpu->stream));
     return 0;
 }
 
 // ---- pipeline chunks: an even batch of 32 or more is cut into two chunks (images are independent units) so that `run` can
 //      overlap the H2D copy of the second with the kernels of the first; each chunk owns a slice of every tensor ----
-static void plan_chunks(const tb200_graph* g, int Ntot, BatchPlan& bp)
+static void plan_chunks(const Shard* g, int Ntot, BatchPlan& bp)
 {
     bool same_batch = true;
     for (auto& t : g->tensors) same_batch &= (t.d.dims[0] == g->tensors[0].d.dims[0]);
@@ -1384,7 +1387,7 @@ struct Slice
     long long bytes(const TensorInfo& t) const { return (long long)(t.nhwc_bytes / (size_t)ntot * (size_t)nb); }
 };
 
-static int fill_conv_step(tb200_graph* g, int li, const LayerPlan& P, const Slice& sl, BatchPlan* work, Step& s)
+static int fill_conv_step(Shard* g, int li, const LayerPlan& P, const Slice& sl, BatchPlan* work, Step& s)
 {
     const tb200_layer_desc& L = g->layers[li];
     const TensorInfo& tin = g->tensors[L.inputs[0]];
@@ -1434,7 +1437,7 @@ static int fill_conv_step(tb200_graph* g, int li, const LayerPlan& P, const Slic
     {
         int rc = gemm_plan_create_conv(&s.gemm, s.in, s.w, s.out, s.cs, P.gemm_zp);
         if (rc) return fail(rc, "layer %d: implicit-GEMM plan failed", li);
-        s.gemm.fixq = g->ctx->fixq, s.gemm.fixq_cap = FIXQ_CAP;
+        s.gemm.fixq = g->gpu->fixq, s.gemm.fixq_cap = FIXQ_CAP;
     }
     if (s.kind == K_GEMM)
     {
@@ -1442,12 +1445,12 @@ static int fill_conv_step(tb200_graph* g, int li, const LayerPlan& P, const Slic
         const int kdim = fc ? H * W * tin.cp : tin.cp;
         int rc = gemm_plan_create(&s.gemm, s.in, kdim, s.w, s.out, m, kdim, OC, tout.cp, tout.cp, P.gemm_zp);
         if (rc) return fail(rc, "layer %d: TMA descriptor creation failed (m=%lld k=%d oc=%d)", li, m, kdim, OC);
-        s.gemm.fixq = g->ctx->fixq, s.gemm.fixq_cap = FIXQ_CAP;
+        s.gemm.fixq = g->gpu->fixq, s.gemm.fixq_cap = FIXQ_CAP;
     }
     return 0;
 }
 
-static int fill_pool_step(const tb200_graph* g, int li, const LayerPlan& P, const Slice& sl, Step& s)
+static int fill_pool_step(const Shard* g, int li, const LayerPlan& P, const Slice& sl, Step& s)
 {
     const tb200_layer_desc& L = g->layers[li];
     const TensorInfo& tin = g->tensors[L.inputs[0]];
@@ -1465,7 +1468,7 @@ static int fill_pool_step(const tb200_graph* g, int li, const LayerPlan& P, cons
 }
 
 // ReLU and eltwise
-static int fill_pointwise_step(const tb200_graph* g, int li, const LayerPlan& P, const Slice& sl, Step& s)
+static int fill_pointwise_step(const Shard* g, int li, const LayerPlan& P, const Slice& sl, Step& s)
 {
     const tb200_layer_desc& L = g->layers[li];
     const TensorInfo& tin = g->tensors[L.inputs[0]];
@@ -1491,7 +1494,7 @@ static int fill_pointwise_step(const tb200_graph* g, int li, const LayerPlan& P,
 }
 
 // One step per input; all but the last are pushed here, the last is left in `s`.
-static int fill_concat_steps(const tb200_graph* g, int li, const LayerPlan& P, const Slice& sl, Step& s, std::vector<Step>& steps)
+static int fill_concat_steps(const Shard* g, int li, const LayerPlan& P, const Slice& sl, Step& s, std::vector<Step>& steps)
 {
     const tb200_layer_desc& L = g->layers[li];
     const TensorInfo& tin = g->tensors[L.inputs[0]];
@@ -1517,7 +1520,7 @@ static int fill_concat_steps(const tb200_graph* g, int li, const LayerPlan& P, c
 }
 
 // Upsample, byte table, softmax, reshape, copy.
-static int fill_data_step(const tb200_graph* g, int li, const LayerPlan& P, const Slice& sl, Step& s)
+static int fill_data_step(const Shard* g, int li, const LayerPlan& P, const Slice& sl, Step& s)
 {
     const tb200_layer_desc& L = g->layers[li];
     const TensorInfo& tin = g->tensors[L.inputs[0]];
@@ -1555,7 +1558,7 @@ static int fill_data_step(const tb200_graph* g, int li, const LayerPlan& P, cons
 
 // The launch sequence of images [first, first + nb) (the active batch, or one pipeline chunk of it) into `steps`; the work of its
 // convolutions is added to *work when given.
-static int build_steps(tb200_graph* g, int first, int nb, std::vector<Step>& steps, BatchPlan* work)
+static int build_steps(Shard* g, int first, int nb, std::vector<Step>& steps, BatchPlan* work)
 {
     const std::vector<LayerPlan>& plan = g->plan;
     const Slice sl{first, nb, g->tensors[0].d.dims[0]};
@@ -1575,7 +1578,7 @@ static int build_steps(tb200_graph* g, int first, int nb, std::vector<Step>& ste
     {
         const tb200_layer_desc& L = g->layers[li];
         const LayerPlan& P = plan[li];
-        if (P.kind == K_NONE) continue; // keeps the name prerun_one gave it
+        if (P.kind == K_NONE) continue;
         const TensorInfo& tin = g->tensors[L.inputs[0]];
         Step s;
         s.kind = P.kind, s.layer = li, s.u8 = tin.d.data_type == TB200_DT_UINT8;
@@ -1587,7 +1590,6 @@ static int build_steps(tb200_graph* g, int first, int nb, std::vector<Step>& ste
         else if (P.kind == K_CONCAT_PART) rc = fill_concat_steps(g, li, P, sl, s, steps);
         else rc = fill_data_step(g, li, P, sl, s);
         if (rc) return rc;
-        g->layer_kernel[li] = (s.kind == K_CONV_DW && s.dwp.valid) ? "conv_dw3x3_tma_dp4a" : ((s.kind == K_GATHER_TC && s.wp.valid) ? "conv_window_tcgen05" : kStepName[s.kind]);
         steps.push_back(s);
     }
     for (size_t i = 0; i < g->output_ids.size(); i++)
@@ -1599,9 +1601,9 @@ static int build_steps(tb200_graph* g, int first, int nb, std::vector<Step>& ste
 }
 
 // ---- capture the launch sequences of `bp` into CUDA graphs: [0] = whole slice, [1..K] = the pipeline chunks ----
-static int capture_graphs(tb200_graph* g, BatchPlan& bp)
+static int capture_graphs(Shard* g, BatchPlan& bp)
 {
-    cudaStream_t st = g->ctx->stream;
+    cudaStream_t st = g->gpu->stream;
     const int ngraphs = 1 + (int)bp.chunk_steps.size();
     bp.cu_graphs.assign(ngraphs, nullptr);
     bp.cu_execs.assign(ngraphs, nullptr);
@@ -1650,7 +1652,7 @@ static void end_open_capture(cudaStream_t st)
 
 // The launch sequences of images [0, nb) of this shard into bp: the whole slice, the pipeline chunks at nb (plan_chunks) and,
 // unless TB200_PRERUN_NO_GRAPH, their CUDA graphs.  nb == 0 leaves bp without steps: nothing is encoded or captured.
-static int build_batch_plan(tb200_graph* g, int nb, BatchPlan& bp)
+static int build_batch_plan(Shard* g, int nb, BatchPlan& bp)
 {
     bp.n = nb;
     if (nb == 0) return 0;
@@ -1667,25 +1669,22 @@ static int build_batch_plan(tb200_graph* g, int nb, BatchPlan& bp)
     return 0;
 }
 
-// Plans one graph on one GPU.  On failure the caller destroys g (arenas, tensor maps, CUDA graphs, an open capture).
-static int prerun_one(tb200_context* ctx, const tb200_tensor_desc* tensors, int num_tensors, const tb200_layer_desc* layers, int num_layers,
-                      const int32_t* input_ids, int num_inputs, const int32_t* output_ids, int num_outputs, int flags, tb200_graph* g)
+// Plans shard g on its GPU, which is current, for the batch of its descriptors; all but the weights.  On failure the caller
+// destroys the graph (arenas, tensor maps, CUDA graphs, an open capture).
+static int prerun_one(Shard* g, const tb200_tensor_desc* tensors, int num_tensors, const tb200_layer_desc* layers, int num_layers,
+                      const int32_t* input_ids, int num_inputs, const int32_t* output_ids, int num_outputs)
 {
-    CUDA_OK(cudaSetDevice(ctx->device));
     g->layers.assign(layers, layers + num_layers);
-    g->layer_kernel.assign(num_layers, kStepName[K_NONE]); // build_steps names every layer that was not folded away
     g->plan.assign(num_layers, LayerPlan());
     std::vector<LayerPlan>& plan = g->plan;
-    if (!(flags & TB200_PRERUN_NO_GRAPH)) fuse_nodes(layers, tensors, num_tensors, output_ids, num_outputs, g->layers, plan);
+    if (!(g->flags & TB200_PRERUN_NO_GRAPH)) fuse_nodes(layers, tensors, num_tensors, output_ids, num_outputs, g->layers, plan);
     int rc;
     if ((rc = setup_tensors(g, tensors, num_tensors, input_ids, num_inputs, output_ids, num_outputs)) != 0) return rc;
     if ((rc = plan_kernels(g, plan)) != 0) return rc;
     plan_activation_arena(g, plan);
     if ((rc = alloc_device_buffers(g)) != 0) return rc;
     prove_fast_epilogues(g, plan);
-    if (!(flags & TB200_PRERUN_NO_WEIGHTS) && (rc = upload_weights(g, plan)) != 0) return rc;
-    CUDA_OK(cudaStreamSynchronize(ctx->stream));
-    g->cur = &g->prepared;
+    CUDA_OK(cudaStreamSynchronize(g->gpu->stream));
     return build_batch_plan(g, g->tensors[0].d.dims[0], g->prepared);
 }
 
@@ -1695,29 +1694,29 @@ static int prerun_one(tb200_context* ctx, const tb200_tensor_desc* tensors, int 
 // chunks of the copy/compute pipeline.  So a buffer is registered (cudaHostRegisterPortable) the first time it is seen and the
 // registration is cached (up to 16 ranges, oldest dropped; everything is unregistered at postrun / context destruction).
 // Returns true when [p, p+bytes) is page-locked.  Failure is not an error: the copy then takes the driver's pageable path.
-static bool host_pin(tb200_context* root, const void* ptr, size_t bytes)
+static bool host_pin(tb200_context* ctx, const void* ptr, size_t bytes)
 {
     if (!ptr || !bytes) return false;
     const uint8_t* p = (const uint8_t*)ptr;
-    for (const HostReg& r : root->host_regs)
+    for (const HostReg& r : ctx->host_regs)
         if (p >= r.p && p + bytes <= r.p + r.bytes) return true;
-    for (const void* f : root->host_reg_failed)
+    for (const void* f : ctx->host_reg_failed)
         if (f == ptr) return false;
     cudaPointerAttributes at;
     if (cudaPointerGetAttributes(&at, ptr) == cudaSuccess && at.type == cudaMemoryTypeHost)
     {
-        root->host_regs.push_back(HostReg{p, bytes, false}); // already page-locked by its owner
+        ctx->host_regs.push_back(HostReg{p, bytes, false}); // already page-locked by its owner
         return true;
     }
     cudaGetLastError();
     // an older, smaller registration of the same buffer would make the new one fail: drop overlapping ranges of ours first
-    for (size_t i = 0; i < root->host_regs.size();)
+    for (size_t i = 0; i < ctx->host_regs.size();)
     {
-        const HostReg& r = root->host_regs[i];
+        const HostReg& r = ctx->host_regs[i];
         if (r.ours && p < r.p + r.bytes && r.p < p + bytes)
         {
             if (cudaHostUnregister((void*)r.p) != cudaSuccess) cudaGetLastError();
-            root->host_regs.erase(root->host_regs.begin() + i);
+            ctx->host_regs.erase(ctx->host_regs.begin() + i);
         }
         else
             i++;
@@ -1725,81 +1724,66 @@ static bool host_pin(tb200_context* root, const void* ptr, size_t bytes)
     if (cudaHostRegister((void*)ptr, bytes, cudaHostRegisterPortable) != cudaSuccess)
     {
         cudaGetLastError();
-        if (root->host_reg_failed.size() < 64) root->host_reg_failed.push_back(ptr);
+        if (ctx->host_reg_failed.size() < 64) ctx->host_reg_failed.push_back(ptr);
         return false;
     }
-    root->host_regs.push_back(HostReg{p, bytes, true});
-    if (root->host_regs.size() > 16)
+    ctx->host_regs.push_back(HostReg{p, bytes, true});
+    if (ctx->host_regs.size() > 16)
     {
-        if (root->host_regs[0].ours && cudaHostUnregister((void*)root->host_regs[0].p) != cudaSuccess) cudaGetLastError();
-        root->host_regs.erase(root->host_regs.begin());
+        if (ctx->host_regs[0].ours && cudaHostUnregister((void*)ctx->host_regs[0].p) != cudaSuccess) cudaGetLastError();
+        ctx->host_regs.erase(ctx->host_regs.begin());
     }
     return true;
 }
 
 
-// every shard of a graph, the root's own first
+// f(shard, index) for every shard in order, with the shard's GPU current, up to the first failure; GPU 0 is current afterwards
 template <typename F>
 static int for_each_shard(tb200_graph* g, F f)
 {
-    int rc = f(g, 0);
-    for (size_t i = 0; rc == 0 && i < g->shards.size(); i++) rc = f(g->shards[i], (int)i + 1);
+    int rc = 0;
+    for (size_t r = 0; rc == 0 && r < g->shards.size(); r++)
+    {
+        const cudaError_t e = cudaSetDevice(g->shards[r].gpu->device);
+        rc = e == cudaSuccess ? f(&g->shards[r], (int)r) : fail(TB200_ERR_CUDA, "cudaSetDevice(%d) failed: %s", g->shards[r].gpu->device, cudaGetErrorString(e));
+    }
+    cudaSetDevice(g->shards[0].gpu->device);
     return rc;
 }
 // the shards that hold images of the active batch: a shard left without any issues no copy, kernel or graph launch
 template <typename F>
 static int for_each_busy_shard(tb200_graph* g, F f)
 {
-    return for_each_shard(g, [&](tb200_graph* sh, int r) { return sh->num_images ? f(sh, r) : 0; });
+    return for_each_shard(g, [&](Shard* sh, int r) { return sh->num_images ? f(sh, r) : 0; });
 }
 // NCHW bytes of one image of a tensor (from the batch of prerun, which sized the tensor)
-static inline size_t image_bytes(const tb200_graph* g, int tensor_id) { return g->tensors[tensor_id].nchw_bytes / (size_t)g->prep_images; }
+static inline size_t image_bytes(const Shard* g, int tensor_id) { return g->tensors[tensor_id].nchw_bytes / (size_t)g->prep_images; }
 // dim 0 and NCHW bytes of the shard's active images of a tensor: all of it at the batch of prerun (also when its dim 0 is not the
 // batch), else num_images images
-static inline int active_dim0(const tb200_graph* g, const TensorInfo& t) { return g->num_images == g->prep_images ? t.d.dims[0] : g->num_images; }
-static inline size_t active_nchw_bytes(const tb200_graph* g, const TensorInfo& t)
+static inline int active_dim0(const Shard* g, const TensorInfo& t) { return g->num_images == g->prep_images ? t.d.dims[0] : g->num_images; }
+static inline size_t active_nchw_bytes(const Shard* g, const TensorInfo& t)
 {
     return g->num_images == g->prep_images ? t.nchw_bytes : t.nchw_bytes / (size_t)t.d.dims[0] * (size_t)g->num_images;
 }
 
-// The packed arena from GPU 0 to every other GPU of the group: one peer copy per shard, all on the root's stream.
+// The packed arena from GPU 0 to every other GPU of the group: one peer copy per shard, all on GPU 0's stream.
 static int broadcast_arena(tb200_graph* g)
 {
-    tb200_context* root = g->ctx;
-    if (g->shards.empty()) return 0;
-    CUDA_OK(cudaSetDevice(root->device));
-    CUDA_OK(cudaStreamSynchronize(root->stream));
-    for (size_t i = 0; i < g->shards.size(); i++)
+    const Shard& s0 = g->shards[0];
+    if (g->shards.size() == 1) return 0;
+    CUDA_OK(cudaSetDevice(s0.gpu->device));
+    CUDA_OK(cudaStreamSynchronize(s0.gpu->stream));
+    for (size_t r = 1; r < g->shards.size(); r++)
     {
-        tb200_graph* sh = g->shards[i];
-        if (sh->w_bytes != g->w_bytes) return fail(TB200_ERR_INVALID, "shard %d planned a different weight arena (%zu vs %zu bytes)", (int)i + 1, sh->w_bytes, g->w_bytes);
-        CUDA_OK(cudaMemcpyPeerAsync(sh->w_arena, sh->ctx->device, g->w_arena, root->device, g->w_bytes, root->stream));
+        const Shard& sh = g->shards[r];
+        if (sh.w_bytes != s0.w_bytes) return fail(TB200_ERR_INVALID, "shard %d planned a different weight arena (%zu vs %zu bytes)", (int)r, sh.w_bytes, s0.w_bytes);
+        CUDA_OK(cudaMemcpyPeerAsync(sh.w_arena, sh.gpu->device, s0.w_arena, s0.gpu->device, s0.w_bytes, s0.gpu->stream));
     }
-    CUDA_OK(cudaStreamSynchronize(root->stream));
-    for (tb200_graph* sh : g->shards)
-    {
-        CUDA_OK(cudaSetDevice(sh->ctx->device));
-        CUDA_OK(cudaStreamSynchronize(sh->ctx->stream));
-    }
-    CUDA_OK(cudaSetDevice(root->device));
-    return 0;
-}
-
-static int prerun_guarded(tb200_context* ctx, const tb200_tensor_desc* tensors, int num_tensors, const tb200_layer_desc* layers, int num_layers,
-                          const int32_t* input_ids, int num_inputs, const int32_t* output_ids, int num_outputs, int flags, tb200_graph** out)
-{
-    tb200_graph* g = new tb200_graph();
-    g->ctx = ctx, g->flags = flags;
-    const int rc = prerun_one(ctx, tensors, num_tensors, layers, num_layers, input_ids, num_inputs, output_ids, num_outputs, flags, g);
-    if (rc)
-    {
-        end_open_capture(ctx->stream);
-        destroy_graph(g);
-        return rc;
-    }
-    g->num_images = g->prep_images = g->total_images = g->batch = tensors[0].dims[0];
-    *out = g;
-    return 0;
+    CUDA_OK(cudaStreamSynchronize(s0.gpu->stream));
+    return for_each_shard(g, [](Shard* sh, int) -> int {
+        CUDA_OK(cudaStreamSynchronize(sh->gpu->stream));
+        return 0;
+    });
 }
 
 extern "C" {
@@ -1810,48 +1794,41 @@ int tb200_graph_prerun(tb200_context* ctx, const tb200_tensor_desc* tensors, int
     if (!ctx || !tensors || !layers || !out || num_tensors <= 0 || num_layers <= 0) return fail(TB200_ERR_INVALID, "bad arguments");
     if ((num_inputs > 0 && !input_ids) || (num_outputs > 0 && !output_ids)) return fail(TB200_ERR_INVALID, "null id table");
     // ---- how many GPUs take part: the batch (dim 0, the same for every tensor) is cut into contiguous slices ----
-    int R = 1 + (int)ctx->peers.size();
+    int R = (int)ctx->gpus.size();
     const int N = tensors[0].dims[0];
     for (int i = 0; i < num_tensors; i++)
         if (tensors[i].dims[0] != N) R = 1; // not a plain batch dimension: GPU 0 runs the whole subgraph
     if (R > N) R = N > 0 ? N : 1;
-    if (R == 1) return prerun_guarded(ctx, tensors, num_tensors, layers, num_layers, input_ids, num_inputs, output_ids, num_outputs, flags, out);
 
+    tb200_graph* g = new tb200_graph();
+    g->ctx = ctx, g->batch = g->prepared_batch = N;
+    g->shards.resize(R);
+    for (int r = 0; r < R; r++) g->shards[r].gpu = &ctx->gpus[r], g->shards[r].flags = flags;
     std::vector<tb200_tensor_desc> td(tensors, tensors + num_tensors);
-    tb200_graph* root = nullptr;
-    int first = 0;
-    for (int r = 0; r < R; r++)
+    int rc = for_each_shard(g, [&](Shard* sh, int r) -> int {
+        tb200_shard_range(N, R, r, &sh->first_image, &sh->num_images);
+        sh->prep_images = sh->num_images;
+        if (R > 1)
+            for (auto& t : td) t.dims[0] = sh->num_images;
+        // every shard allocates a weight arena of the same layout (it depends on the descriptors alone); GPU 0's is packed below
+        const int e = prerun_one(sh, td.data(), num_tensors, layers, num_layers, input_ids, num_inputs, output_ids, num_outputs);
+        if (e) end_open_capture(sh->gpu->stream);
+        return e;
+    });
+    if (rc == 0)
     {
-        int count = 0;
-        tb200_shard_range(N, R, r, nullptr, &count);
-        for (auto& t : td) t.dims[0] = count;
-        tb200_graph* sh = nullptr;
-        tb200_context* c = r == 0 ? ctx : ctx->peers[r - 1];
-        // GPU 0 packs the weights; the others only allocate the arena (same layout: it depends on the descriptors alone)
-        const int rc = prerun_guarded(c, td.data(), num_tensors, layers, num_layers, input_ids, num_inputs, output_ids, num_outputs,
-                                      flags | (r ? TB200_PRERUN_NO_WEIGHTS : 0), &sh);
-        if (rc)
-        {
-            if (root) destroy_graph(root);
-            cudaSetDevice(ctx->device);
-            return rc;
-        }
-        sh->first_image = first, sh->num_images = sh->prep_images = count, sh->total_images = sh->batch = N;
-        first += count;
-        if (r == 0) root = sh;
-        else root->shards.push_back(sh);
+        g->layer_kernel.assign(num_layers, kStepName[K_NONE]);
+        for (const Step& s : g->shards[0].prepared.steps)
+            if (s.layer >= 0)
+                g->layer_kernel[s.layer] = (s.kind == K_CONV_DW && s.dwp.valid) ? "conv_dw3x3_tma_dp4a" : ((s.kind == K_GATHER_TC && s.wp.valid) ? "conv_window_tcgen05" : kStepName[s.kind]);
+        if (!(flags & TB200_PRERUN_NO_WEIGHTS) && (rc = upload_weights(g)) == 0) rc = broadcast_arena(g);
     }
-    if (!(flags & TB200_PRERUN_NO_WEIGHTS))
+    if (rc)
     {
-        const int rc = broadcast_arena(root);
-        if (rc)
-        {
-            destroy_graph(root);
-            return rc;
-        }
+        destroy_graph(g);
+        return rc;
     }
-    cudaSetDevice(ctx->device);
-    *out = root;
+    *out = g;
     return 0;
 }
 
@@ -1874,8 +1851,9 @@ int tb200_graph_broadcast_weights(tb200_graph* g)
 int tb200_probe_int8_tops(tb200_context* ctx, double* tops)
 {
     if (!ctx || !tops) return fail(TB200_ERR_INVALID, "bad arguments");
-    CUDA_OK(cudaSetDevice(ctx->device));
-    const cudaError_t e = probe_int8_mma_peak(ctx->num_sms, tops, ctx->stream);
+    const Gpu& gpu = ctx->gpus[0];
+    CUDA_OK(cudaSetDevice(gpu.device));
+    const cudaError_t e = probe_int8_mma_peak(gpu.num_sms, tops, gpu.stream);
     if (e != cudaSuccess) return fail(TB200_ERR_CUDA, "int8 MMA probe: %s", cudaGetErrorString(e));
     return 0;
 }
@@ -1888,15 +1866,15 @@ int tb200_pack_cache_dir(const char* dir)
 }
 int tb200_graph_pack_cache_state(tb200_graph* g) { return g ? g->pack_cache_state : 0; }
 
-int tb200_graph_num_shards(tb200_graph* g) { return g ? 1 + (int)g->shards.size() : 0; }
+int tb200_graph_num_shards(tb200_graph* g) { return g ? (int)g->shards.size() : 0; }
 
 int tb200_graph_shard(tb200_graph* g, int index, int* cuda_device, int* first_image, int* num_images)
 {
-    if (!g || index < 0 || index > (int)g->shards.size()) return fail(TB200_ERR_INVALID, "shard index out of range");
-    const tb200_graph* sh = index == 0 ? g : g->shards[index - 1];
-    if (cuda_device) *cuda_device = sh->ctx->device;
-    if (first_image) *first_image = sh->first_image;
-    if (num_images) *num_images = sh->num_images;
+    if (!g || index < 0 || index >= (int)g->shards.size()) return fail(TB200_ERR_INVALID, "shard index out of range");
+    const Shard& sh = g->shards[index];
+    if (cuda_device) *cuda_device = sh.gpu->device;
+    if (first_image) *first_image = sh.first_image;
+    if (num_images) *num_images = sh.num_images;
     return 0;
 }
 
@@ -1905,55 +1883,51 @@ int tb200_graph_shard(tb200_graph* g, int index, int* cuda_device, int* first_im
 int tb200_graph_set_batch(tb200_graph* g, int n)
 {
     if (!g) return fail(TB200_ERR_INVALID, "null graph");
-    if (n < 1 || n > g->total_images) return fail(TB200_ERR_INVALID, "set_batch: %d images; the graph was prepared for 1..%d", n, g->total_images);
+    if (n < 1 || n > g->prepared_batch) return fail(TB200_ERR_INVALID, "set_batch: %d images; the graph was prepared for 1..%d", n, g->prepared_batch);
     if (n == g->batch) return 0;
-    for (const TensorInfo& t : g->tensors)
-        if (t.d.dims[0] != g->tensors[0].d.dims[0])
+    for (const TensorInfo& t : g->shards[0].tensors)
+        if (t.d.dims[0] != g->shards[0].tensors[0].d.dims[0])
             return fail(TB200_ERR_UNSUPPORTED, "set_batch: the graph's tensors differ in dim 0, so it runs only at the batch of %d it was prepared for",
-                        g->total_images);
-    int rc = for_each_shard(g, [&](tb200_graph* sh, int) -> int {
-        CUDA_OK(cudaSetDevice(sh->ctx->device));
+                        g->prepared_batch);
+    int rc = for_each_shard(g, [](Shard* sh, int) -> int {
         if (sh->copy_stream) CUDA_OK(cudaStreamSynchronize(sh->copy_stream));
         if (sh->d2h_stream) CUDA_OK(cudaStreamSynchronize(sh->d2h_stream));
-        CUDA_OK(cudaStreamSynchronize(sh->ctx->stream));
+        CUDA_OK(cudaStreamSynchronize(sh->gpu->stream));
         return 0;
     });
-    const int R = 1 + (int)g->shards.size();
-    auto shard = [&](int r) { return r == 0 ? g : g->shards[r - 1]; };
-    const bool prepared = n == g->total_images;
+    const int R = (int)g->shards.size();
+    const bool prepared = n == g->prepared_batch;
     if (rc == 0 && !prepared && n != g->other_batch)
     {
         // build every shard's plan before replacing any: a failure leaves the graph as it was
         std::vector<BatchPlan> fresh(R);
-        for (int r = 0; r < R && rc == 0; r++)
-        {
-            tb200_graph* sh = shard(r);
+        rc = for_each_shard(g, [&](Shard* sh, int r) -> int {
             int count = 0;
             tb200_shard_range(n, R, r, nullptr, &count);
-            const std::vector<const char*> names = sh->layer_kernel; // the kernel names stay those of prerun
-            cudaSetDevice(sh->ctx->device);
-            rc = build_batch_plan(sh, count, fresh[r]);
-            sh->layer_kernel = names;
-            if (rc) end_open_capture(sh->ctx->stream);
-        }
-        for (int r = 0; r < R; r++)
+            const int e = build_batch_plan(sh, count, fresh[r]);
+            if (e) end_open_capture(sh->gpu->stream);
+            return e;
+        });
+        for (int r = 0; r < R; r++) // on every shard, whatever fails
         {
-            tb200_graph* sh = shard(r);
-            cudaSetDevice(sh->ctx->device);
-            destroy_batch_plan(rc ? fresh[r] : sh->other);
-            if (!rc) sh->other = std::move(fresh[r]);
+            Shard& sh = g->shards[r];
+            cudaSetDevice(sh.gpu->device);
+            destroy_batch_plan(rc ? fresh[r] : sh.other);
+            if (!rc) sh.other = std::move(fresh[r]);
         }
+        cudaSetDevice(g->shards[0].gpu->device);
         if (!rc) g->other_batch = n;
     }
     if (rc == 0)
+    {
         for (int r = 0; r < R; r++)
         {
-            tb200_graph* sh = shard(r);
-            sh->cur = prepared ? &sh->prepared : &sh->other;
-            tb200_shard_range(n, R, r, &sh->first_image, &sh->num_images);
-            sh->batch = n;
+            Shard& sh = g->shards[r];
+            sh.cur = prepared ? &sh.prepared : &sh.other;
+            tb200_shard_range(n, R, r, &sh.first_image, &sh.num_images);
         }
-    cudaSetDevice(g->ctx->device);
+        g->batch = n;
+    }
     return rc;
 }
 
@@ -1966,24 +1940,22 @@ int tb200_graph_batch(tb200_graph* g)
 int tb200_graph_arena_bytes(tb200_graph* g, size_t* activation_bytes, size_t* unshared_bytes, size_t* weight_bytes)
 {
     if (!g) return fail(TB200_ERR_INVALID, "null graph");
-    if (activation_bytes) *activation_bytes = g->act_bytes;
-    if (unshared_bytes) *unshared_bytes = g->act_unshared_bytes;
-    if (weight_bytes) *weight_bytes = g->w_bytes;
+    const Shard& s0 = g->shards[0];
+    if (activation_bytes) *activation_bytes = s0.act_bytes;
+    if (unshared_bytes) *unshared_bytes = s0.act_unshared_bytes;
+    if (weight_bytes) *weight_bytes = s0.w_bytes;
     return 0;
 }
 
 int tb200_graph_upload(tb200_graph* g, int input_index, const void* host_nchw)
 {
-    if (!g || input_index < 0 || input_index >= (int)g->input_ids.size() || !host_nchw) return fail(TB200_ERR_INVALID, "bad upload arguments");
-    const int rc = for_each_busy_shard(g, [&](tb200_graph* sh, int) -> int {
-        CUDA_OK(cudaSetDevice(sh->ctx->device));
+    if (!g || input_index < 0 || input_index >= (int)g->shards[0].input_ids.size() || !host_nchw) return fail(TB200_ERR_INVALID, "bad upload arguments");
+    return for_each_busy_shard(g, [&](Shard* sh, int) -> int {
         const int id = sh->input_ids[input_index];
         CUDA_OK(host_copy(g->ctx, sh->in_nchw_dev[input_index], (const uint8_t*)host_nchw + (size_t)sh->first_image * image_bytes(sh, id),
-                                active_nchw_bytes(sh, sh->tensors[id]), cudaMemcpyHostToDevice, sh->ctx->stream));
+                                active_nchw_bytes(sh, sh->tensors[id]), cudaMemcpyHostToDevice, sh->gpu->stream));
         return 0;
     });
-    cudaSetDevice(g->ctx->device);
-    return rc;
 }
 
 // Checks shared by the image upload entry points: every descriptor of the batch names a 3- or 4-channel image of 2..32767 pixels a side
@@ -2013,10 +1985,9 @@ template <typename Launch>
 static int upload_staged_images(tb200_graph* g, const char* what, const void* pixels, size_t pixel_bytes, const tb200_image* images,
                                 const tb200_detect_geometry* geo, Launch launch)
 {
-    CUDA_OK(cudaSetDevice(g->ctx->device));
+    CUDA_OK(cudaSetDevice(g->ctx->gpus[0].device));
     host_pin(g->ctx, pixels, pixel_bytes);
-    const int rc = for_each_busy_shard(g, [&](tb200_graph* sh, int) -> int {
-        CUDA_OK(cudaSetDevice(sh->ctx->device));
+    return for_each_busy_shard(g, [&](Shard* sh, int) -> int {
         cudaGetLastError(); // the launch below reports cudaGetLastError(): a non-sticky error an earlier call left behind is not its own
         const int n = sh->num_images;
         const tb200_image* im = images + sh->first_image;
@@ -2044,7 +2015,7 @@ static int upload_staged_images(tb200_graph* g, const char* what, const void* pi
         for (int i = 0; i < n; i++)
             sh->img_desc_host[i] = gm ? ImageDesc{im[i].offset - lo, im[i].w, im[i].h, im[i].c, gm[i].resize_w, gm[i].resize_h, gm[i].left, gm[i].top}
                                       : ImageDesc{im[i].offset - lo, im[i].w, im[i].h, im[i].c, 0, 0, 0, 0};
-        cudaStream_t st = sh->ctx->stream;
+        cudaStream_t st = sh->gpu->stream;
         CUDA_OK(host_copy(g->ctx, sh->img_stage, (const uint8_t*)pixels + lo, hi - lo, cudaMemcpyHostToDevice, st));
         CUDA_OK(cudaMemcpyAsync(sh->img_desc, sh->img_desc_host, sizeof(ImageDesc) * n, cudaMemcpyHostToDevice, st));
         CUDA_OK(cudaEventRecord(sh->img_ev, st));
@@ -2052,8 +2023,6 @@ static int upload_staged_images(tb200_graph* g, const char* what, const void* pi
         if (e != cudaSuccess) return fail(TB200_ERR_CUDA, "%s: launch of its kernel failed: %s", what, cudaGetErrorString(e));
         return 0;
     });
-    cudaSetDevice(g->ctx->device);
-    return rc;
 }
 } // extern "C++"
 
@@ -2061,15 +2030,15 @@ int tb200_graph_upload_images(tb200_graph* g, int input_index, const void* pixel
                               const float scale[3])
 {
     static_assert(offsetof(ImageDesc, w) == offsetof(tb200_image, w) && offsetof(ImageDesc, c) == offsetof(tb200_image, c), "image descriptor layout");
-    if (!g || !pixels || !images || !mean || !scale || input_index < 0 || input_index >= (int)g->input_ids.size())
+    if (!g || !pixels || !images || !mean || !scale || input_index < 0 || input_index >= (int)g->shards[0].input_ids.size())
         return fail(TB200_ERR_INVALID, "bad upload_images arguments");
-    const tb200_tensor_desc& td = g->tensors[g->input_ids[input_index]].d;
+    const tb200_tensor_desc& td = g->shards[0].tensors[g->shards[0].input_ids[input_index]].d;
     if (td.dims[1] != 3) return fail(TB200_ERR_INVALID, "upload_images: input %d has %d channels, not 3", input_index, td.dims[1]);
     if (td.data_type != TB200_DT_INT8 && td.data_type != TB200_DT_UINT8) return fail(TB200_ERR_INVALID, "upload_images: input %d is not int8 / uint8", input_index);
     if (const int rc = check_images(g, "upload_images", pixel_bytes, images, mean, scale)) return rc;
     const bool u8 = td.data_type == TB200_DT_UINT8;
     return upload_staged_images(g, "upload_images", pixels, pixel_bytes, images, nullptr,
-                                [&](tb200_graph* sh, const uint8_t* px, const ImageDesc* desc, int n, cudaStream_t st) {
+                                [&](Shard* sh, const uint8_t* px, const ImageDesc* desc, int n, cudaStream_t st) {
                                     return launch_image_pre(px, desc, n, sh->in_nchw_dev[input_index], td.dims[2], td.dims[3], mean, scale, td.scale,
                                                             td.zero_point, u8, st);
                                 });
@@ -2096,11 +2065,11 @@ static tb200_detect_geometry detect_geometry(int mode, int src_w, int src_h, int
 int tb200_graph_upload_detect_images(tb200_graph* g, int input_index, const void* pixels, size_t pixel_bytes, const tb200_image* images,
                                      const tb200_detect_pre* pre, tb200_detect_geometry* geometry_out)
 {
-    if (!g || !pixels || !images || !pre || input_index < 0 || input_index >= (int)g->input_ids.size())
+    if (!g || !pixels || !images || !pre || input_index < 0 || input_index >= (int)g->shards[0].input_ids.size())
         return fail(TB200_ERR_INVALID, "bad upload_detect_images arguments");
     if (pre->mode != TB200_PRE_STRETCH && pre->mode != TB200_PRE_LETTERBOX) return fail(TB200_ERR_INVALID, "upload_detect_images: mode %d", pre->mode);
     if (pre->focus != 0 && pre->focus != 1) return fail(TB200_ERR_INVALID, "upload_detect_images: focus %d (0 or 1)", pre->focus);
-    const tb200_tensor_desc& td = g->tensors[g->input_ids[input_index]].d;
+    const tb200_tensor_desc& td = g->shards[0].tensors[g->shards[0].input_ids[input_index]].d;
     const bool focus = pre->focus == 1;
     if (td.dims[1] != (focus ? 12 : 3))
         return fail(TB200_ERR_INVALID, "upload_detect_images: input %d has %d channels, not %d", input_index, td.dims[1], focus ? 12 : 3);
@@ -2119,7 +2088,7 @@ int tb200_graph_upload_detect_images(tb200_graph* g, int input_index, const void
     }
     const bool u8 = td.data_type == TB200_DT_UINT8;
     const int rc = upload_staged_images(g, "upload_detect_images", pixels, pixel_bytes, images, geo.data(),
-                                        [&](tb200_graph* sh, const uint8_t* px, const ImageDesc* desc, int n, cudaStream_t st) {
+                                        [&](Shard* sh, const uint8_t* px, const ImageDesc* desc, int n, cudaStream_t st) {
                                             return launch_detect_pre(px, desc, n, sh->in_nchw_dev[input_index], H, W, focus, pre->mean, pre->scale, td.scale,
                                                                      td.zero_point, u8, st);
                                         });
@@ -2167,9 +2136,8 @@ int tb200_detections_to_source(int mode, const tb200_detect_geometry* geometry, 
     return 0;
 }
 
-static int launch_one(tb200_graph* g)
+static int launch_one(const Shard* g)
 {
-    CUDA_OK(cudaSetDevice(g->ctx->device));
     static const int dbg = getenv("TB200_DEBUG_HASH") ? atoi(getenv("TB200_DEBUG_HASH")) : 0;
     if (dbg >= 2)
     {
@@ -2180,9 +2148,9 @@ static int launch_one(tb200_graph* g)
         fprintf(stderr, "[tb200 dbg] weight arena %zu bytes hash %016llx\n", g->w_bytes, (unsigned long long)fnv1a(host.data(), g->w_bytes));
         for (const Step& s : g->cur->steps)
         {
-            int rc = run_step(g, s, g->ctx->stream);
+            int rc = run_step(g, s, g->gpu->stream);
             if (rc) return rc;
-            CUDA_OK(cudaStreamSynchronize(g->ctx->stream));
+            CUDA_OK(cudaStreamSynchronize(g->gpu->stream));
             if (s.layer < 0) continue;
             const TensorInfo& t = g->tensors[g->layers[s.layer].output];
             host.resize(t.nhwc_bytes);
@@ -2194,12 +2162,12 @@ static int launch_one(tb200_graph* g)
     }
     if (!g->cur->cu_execs.empty())
     {
-        CUDA_OK(cudaGraphLaunch(g->cur->cu_execs[0], g->ctx->stream)); // the whole-batch graph
+        CUDA_OK(cudaGraphLaunch(g->cur->cu_execs[0], g->gpu->stream)); // the whole-batch graph
         return 0;
     }
     for (const Step& s : g->cur->steps)
     {
-        int rc = run_step(g, s, g->ctx->stream);
+        int rc = run_step(g, s, g->gpu->stream);
         if (rc) return rc;
     }
     return 0;
@@ -2208,56 +2176,47 @@ static int launch_one(tb200_graph* g)
 int tb200_graph_launch(tb200_graph* g)
 {
     if (!g) return fail(TB200_ERR_INVALID, "null graph");
-    const int rc = for_each_busy_shard(g, [&](tb200_graph* sh, int) { return launch_one(sh); });
-    cudaSetDevice(g->ctx->device);
-    return rc;
+    return for_each_busy_shard(g, [](Shard* sh, int) { return launch_one(sh); });
 }
 
 int tb200_graph_download(tb200_graph* g, int output_index, void* host_nchw)
 {
-    if (!g || output_index < 0 || output_index >= (int)g->output_ids.size() || !host_nchw) return fail(TB200_ERR_INVALID, "bad download arguments");
-    const int rc = for_each_busy_shard(g, [&](tb200_graph* sh, int) -> int {
-        CUDA_OK(cudaSetDevice(sh->ctx->device));
+    if (!g || output_index < 0 || output_index >= (int)g->shards[0].output_ids.size() || !host_nchw) return fail(TB200_ERR_INVALID, "bad download arguments");
+    return for_each_busy_shard(g, [&](Shard* sh, int) -> int {
         const int id = sh->output_ids[output_index];
         CUDA_OK(host_copy(g->ctx, (uint8_t*)host_nchw + (size_t)sh->first_image * image_bytes(sh, id), sh->out_nchw_dev[output_index],
-                                active_nchw_bytes(sh, sh->tensors[id]), cudaMemcpyDeviceToHost, sh->ctx->stream));
+                                active_nchw_bytes(sh, sh->tensors[id]), cudaMemcpyDeviceToHost, sh->gpu->stream));
         return 0;
     });
-    cudaSetDevice(g->ctx->device);
-    return rc;
 }
 
 int tb200_graph_sync(tb200_graph* g)
 {
     if (!g) return fail(TB200_ERR_INVALID, "null graph");
-    const int rc = for_each_shard(g, [&](tb200_graph* sh, int) -> int {
-        CUDA_OK(cudaSetDevice(sh->ctx->device));
-        CUDA_OK(cudaStreamSynchronize(sh->ctx->stream));
+    return for_each_shard(g, [](Shard* sh, int) -> int {
+        CUDA_OK(cudaStreamSynchronize(sh->gpu->stream));
         return 0;
     });
-    cudaSetDevice(g->ctx->device);
-    return rc;
 }
 
 // ---- run: three phases over the shards so that every GPU's copy engine starts before any GPU's kernels are queued ----
 // (1) queue the H2D copies of all chunks on the shard's copy stream
-static int run_enqueue_h2d(tb200_context* root, tb200_graph* g, const void* const* host_inputs)
+static int run_enqueue_h2d(tb200_context* ctx, const Shard* g, const void* const* host_inputs)
 {
-    CUDA_OK(cudaSetDevice(g->ctx->device));
     if (g->cur->chunks <= 1 || g->cur->cu_execs.empty())
     {
         for (size_t i = 0; i < g->input_ids.size(); i++)
         {
             const int id = g->input_ids[i];
-            CUDA_OK(host_copy(root, g->in_nchw_dev[i], (const uint8_t*)host_inputs[i] + (size_t)g->first_image * image_bytes(g, id),
-                                    active_nchw_bytes(g, g->tensors[id]), cudaMemcpyHostToDevice, g->ctx->stream));
+            CUDA_OK(host_copy(ctx, g->in_nchw_dev[i], (const uint8_t*)host_inputs[i] + (size_t)g->first_image * image_bytes(g, id),
+                                    active_nchw_bytes(g, g->tensors[id]), cudaMemcpyHostToDevice, g->gpu->stream));
         }
         return 0;
     }
     // Pipelined: the H2D copies of all chunks are queued back to back on the copy stream (the link stays busy), chunk k's
     // kernels start as soon as ITS slice has landed, and its outputs leave on a third stream while chunk k+1 computes.
     const int K = g->cur->chunks;
-    CUDA_OK(cudaEventRecord(g->ev_done, g->ctx->stream)); // order after whatever the caller queued on the context stream
+    CUDA_OK(cudaEventRecord(g->ev_done, g->gpu->stream)); // order after whatever the caller queued on the context stream
     CUDA_OK(cudaStreamWaitEvent(g->copy_stream, g->ev_done, 0));
     for (int ck = 0; ck < K; ck++)
     {
@@ -2265,7 +2224,7 @@ static int run_enqueue_h2d(tb200_context* root, tb200_graph* g, const void* cons
         {
             const int id = g->input_ids[i];
             const size_t ib = image_bytes(g, id), off = ib * (size_t)g->cur->chunk_first[ck], bytes = ib * (size_t)g->cur->chunk_count[ck];
-            CUDA_OK(host_copy(root, g->in_nchw_dev[i] + off, (const uint8_t*)host_inputs[i] + (size_t)g->first_image * ib + off, bytes, cudaMemcpyHostToDevice,
+            CUDA_OK(host_copy(ctx, g->in_nchw_dev[i] + off, (const uint8_t*)host_inputs[i] + (size_t)g->first_image * ib + off, bytes, cudaMemcpyHostToDevice,
                                     g->copy_stream));
         }
         CUDA_OK(cudaEventRecord(g->ev_in[ck], g->copy_stream));
@@ -2273,10 +2232,9 @@ static int run_enqueue_h2d(tb200_context* root, tb200_graph* g, const void* cons
     return 0;
 }
 // (2) kernels + D2H
-static int run_enqueue_compute(tb200_context* root, tb200_graph* g, void* const* host_outputs)
+static int run_enqueue_compute(tb200_context* ctx, const Shard* g, void* const* host_outputs)
 {
-    CUDA_OK(cudaSetDevice(g->ctx->device));
-    cudaStream_t cs = g->ctx->stream;
+    cudaStream_t cs = g->gpu->stream;
     static const int dbg2 = getenv("TB200_DEBUG_HASH") ? atoi(getenv("TB200_DEBUG_HASH")) : 0;
     if (g->cur->chunks <= 1 || g->cur->cu_execs.empty() || dbg2 >= 2)
     {
@@ -2285,7 +2243,7 @@ static int run_enqueue_compute(tb200_context* root, tb200_graph* g, void* const*
         for (size_t i = 0; i < g->output_ids.size(); i++)
         {
             const int id = g->output_ids[i];
-            CUDA_OK(host_copy(root, (uint8_t*)host_outputs[i] + (size_t)g->first_image * image_bytes(g, id), g->out_nchw_dev[i], active_nchw_bytes(g, g->tensors[id]),
+            CUDA_OK(host_copy(ctx, (uint8_t*)host_outputs[i] + (size_t)g->first_image * image_bytes(g, id), g->out_nchw_dev[i], active_nchw_bytes(g, g->tensors[id]),
                                     cudaMemcpyDeviceToHost, cs));
         }
         return 0;
@@ -2301,46 +2259,45 @@ static int run_enqueue_compute(tb200_context* root, tb200_graph* g, void* const*
         {
             const int id = g->output_ids[i];
             const size_t ib = image_bytes(g, id), off = ib * (size_t)g->cur->chunk_first[ck], bytes = ib * (size_t)g->cur->chunk_count[ck];
-            CUDA_OK(host_copy(root, (uint8_t*)host_outputs[i] + (size_t)g->first_image * ib + off, g->out_nchw_dev[i] + off, bytes, cudaMemcpyDeviceToHost,
+            CUDA_OK(host_copy(ctx, (uint8_t*)host_outputs[i] + (size_t)g->first_image * ib + off, g->out_nchw_dev[i] + off, bytes, cudaMemcpyDeviceToHost,
                                     g->d2h_stream));
         }
     }
     return 0;
 }
 // (3) wait
-static int run_wait(tb200_graph* g)
+static int run_wait(const Shard* g)
 {
-    CUDA_OK(cudaSetDevice(g->ctx->device));
     if (g->d2h_stream && g->cur->chunks > 1 && !g->cur->cu_execs.empty()) CUDA_OK(cudaStreamSynchronize(g->d2h_stream));
-    CUDA_OK(cudaStreamSynchronize(g->ctx->stream));
+    CUDA_OK(cudaStreamSynchronize(g->gpu->stream));
     return 0;
 }
 
 int tb200_graph_run(tb200_graph* g, const void* const* host_inputs, void* const* host_outputs)
 {
     if (!g || !host_inputs || !host_outputs) return fail(TB200_ERR_INVALID, "bad run arguments");
-    for (size_t i = 0; i < g->input_ids.size(); i++)
+    const Shard& s0 = g->shards[0];
+    for (size_t i = 0; i < s0.input_ids.size(); i++)
         if (!host_inputs[i]) return fail(TB200_ERR_INVALID, "run: input %d has no host buffer", (int)i);
-    for (size_t i = 0; i < g->output_ids.size(); i++)
-        if (!host_outputs[i]) return fail(TB200_ERR_INVALID, "run: output %d has no host buffer (the graph has %d outputs)", (int)i, (int)g->output_ids.size());
+    for (size_t i = 0; i < s0.output_ids.size(); i++)
+        if (!host_outputs[i]) return fail(TB200_ERR_INVALID, "run: output %d has no host buffer (the graph has %d outputs)", (int)i, (int)s0.output_ids.size());
     // page-lock the caller's buffers (whole batch) on first sight
-    CUDA_OK(cudaSetDevice(g->ctx->device));
-    for (size_t i = 0; i < g->input_ids.size(); i++) host_pin(g->ctx, host_inputs[i], image_bytes(g, g->input_ids[i]) * (size_t)g->batch);
-    for (size_t i = 0; i < g->output_ids.size(); i++) host_pin(g->ctx, host_outputs[i], image_bytes(g, g->output_ids[i]) * (size_t)g->batch);
-    int rc = for_each_busy_shard(g, [&](tb200_graph* sh, int) { return run_enqueue_h2d(g->ctx, sh, host_inputs); });
-    if (!rc) rc = for_each_busy_shard(g, [&](tb200_graph* sh, int) { return run_enqueue_compute(g->ctx, sh, host_outputs); });
-    const int rc2 = for_each_shard(g, [&](tb200_graph* sh, int) { return run_wait(sh); }); // always drain what was queued
-    cudaSetDevice(g->ctx->device);
+    CUDA_OK(cudaSetDevice(s0.gpu->device));
+    for (size_t i = 0; i < s0.input_ids.size(); i++) host_pin(g->ctx, host_inputs[i], image_bytes(&s0, s0.input_ids[i]) * (size_t)g->batch);
+    for (size_t i = 0; i < s0.output_ids.size(); i++) host_pin(g->ctx, host_outputs[i], image_bytes(&s0, s0.output_ids[i]) * (size_t)g->batch);
+    int rc = for_each_busy_shard(g, [&](Shard* sh, int) { return run_enqueue_h2d(g->ctx, sh, host_inputs); });
+    if (!rc) rc = for_each_busy_shard(g, [&](Shard* sh, int) { return run_enqueue_compute(g->ctx, sh, host_outputs); });
+    const int rc2 = for_each_shard(g, [](Shard* sh, int) { return run_wait(sh); }); // always drain what was queued
     static const bool dbg = getenv("TB200_DEBUG_HASH") != nullptr;
     if (dbg)
     {
-        for (size_t i = 0; i < g->input_ids.size(); i++)
-            fprintf(stderr, "[tb200 run] input %zu: %zu bytes, hash %016llx\n", i, image_bytes(g, g->input_ids[i]) * (size_t)g->batch,
-                    (unsigned long long)fnv1a(host_inputs[i], image_bytes(g, g->input_ids[i]) * (size_t)g->batch));
-        for (size_t i = 0; i < g->output_ids.size(); i++)
-            fprintf(stderr, "[tb200 run] output %zu (tensor %d): %zu bytes, hash %016llx\n", i, g->output_ids[i], image_bytes(g, g->output_ids[i]) * (size_t)g->batch,
-                    (unsigned long long)fnv1a(host_outputs[i], image_bytes(g, g->output_ids[i]) * (size_t)g->batch));
-        fprintf(stderr, "[tb200 run] %zu layers, %d launches, chunks %d, shards %zu, flags %d\n", g->layers.size(), g->cur->num_launches, g->cur->chunks, g->shards.size() + 1, g->flags);
+        for (size_t i = 0; i < s0.input_ids.size(); i++)
+            fprintf(stderr, "[tb200 run] input %zu: %zu bytes, hash %016llx\n", i, image_bytes(&s0, s0.input_ids[i]) * (size_t)g->batch,
+                    (unsigned long long)fnv1a(host_inputs[i], image_bytes(&s0, s0.input_ids[i]) * (size_t)g->batch));
+        for (size_t i = 0; i < s0.output_ids.size(); i++)
+            fprintf(stderr, "[tb200 run] output %zu (tensor %d): %zu bytes, hash %016llx\n", i, s0.output_ids[i], image_bytes(&s0, s0.output_ids[i]) * (size_t)g->batch,
+                    (unsigned long long)fnv1a(host_outputs[i], image_bytes(&s0, s0.output_ids[i]) * (size_t)g->batch));
+        fprintf(stderr, "[tb200 run] %zu layers, %d launches, chunks %d, shards %zu, flags %d\n", s0.layers.size(), s0.cur->num_launches, s0.cur->chunks, g->shards.size(), s0.flags);
     }
     return rc ? rc : rc2;
 }
@@ -2348,30 +2305,24 @@ int tb200_graph_run(tb200_graph* g, const void* const* host_inputs, void* const*
 int tb200_graph_postrun(tb200_graph* g)
 {
     if (!g) return 0;
-    for_each_shard(g, [&](tb200_graph* sh, int) -> int {
-        cudaSetDevice(sh->ctx->device);
-        cudaStreamSynchronize(sh->ctx->stream);
-        return 0;
-    });
-    host_unregister_all(g->ctx); // the application may free its buffers after postrun_graph()
-    tb200_context* root = g->ctx;
+    tb200_context* ctx = g->ctx;
     destroy_graph(g);
-    cudaSetDevice(root->device);
+    host_unregister_all(ctx); // the application may free its buffers after postrun_graph()
     return 0;
 }
 
 int tb200_graph_weight_arena(tb200_graph* g, void** device_ptr, size_t* bytes)
 {
     if (!g || !device_ptr || !bytes) return fail(TB200_ERR_INVALID, "bad arguments");
-    *device_ptr = g->w_arena, *bytes = g->w_bytes;
+    *device_ptr = g->shards[0].w_arena, *bytes = g->shards[0].w_bytes;
     return 0;
 }
 
 int tb200_graph_num_launches(tb200_graph* g)
 {
     if (!g) return 0;
-    int n = g->cur->num_launches;
-    for (tb200_graph* sh : g->shards) n += sh->cur->num_launches;
+    int n = 0;
+    for (const Shard& sh : g->shards) n += sh.cur->num_launches;
     return n;
 }
 
@@ -2383,39 +2334,37 @@ const char* tb200_graph_layer_kernel(tb200_graph* g, int layer)
 
 int tb200_graph_read_tensor(tb200_graph* g, int tensor_id, void* host_nchw)
 {
-    if (!g || tensor_id < 0 || tensor_id >= (int)g->tensors.size() || !host_nchw) return fail(TB200_ERR_INVALID, "bad arguments");
-    const int rc = for_each_busy_shard(g, [&](tb200_graph* sh, int) -> int {
-        CUDA_OK(cudaSetDevice(sh->ctx->device));
+    if (!g || tensor_id < 0 || tensor_id >= (int)g->shards[0].tensors.size() || !host_nchw) return fail(TB200_ERR_INVALID, "bad arguments");
+    return for_each_busy_shard(g, [&](Shard* sh, int) -> int {
         const TensorInfo& t = sh->tensors[tensor_id];
         uint8_t* tmp = nullptr;
         const size_t bytes = active_nchw_bytes(sh, t);
         CUDA_OK(cudaMalloc(&tmp, bytes));
-        cudaError_t e = launch_nhwc_to_nchw(t.dev, tmp, active_dim0(sh, t), t.d.dims[1], t.d.dims[2], t.d.dims[3], sh->ctx->stream);
+        cudaError_t e = launch_nhwc_to_nchw(t.dev, tmp, active_dim0(sh, t), t.d.dims[1], t.d.dims[2], t.d.dims[3], sh->gpu->stream);
         if (e == cudaSuccess)
-            e = host_copy(g->ctx, (uint8_t*)host_nchw + (size_t)sh->first_image * image_bytes(sh, tensor_id), tmp, bytes, cudaMemcpyDeviceToHost, sh->ctx->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(sh->ctx->stream);
+            e = host_copy(g->ctx, (uint8_t*)host_nchw + (size_t)sh->first_image * image_bytes(sh, tensor_id), tmp, bytes, cudaMemcpyDeviceToHost, sh->gpu->stream);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(sh->gpu->stream);
         cudaFree(tmp);
         if (e != cudaSuccess) return fail(TB200_ERR_CUDA, "read_tensor: %s", cudaGetErrorString(e));
         return 0;
     });
-    cudaSetDevice(g->ctx->device);
-    return rc;
 }
 
 int tb200_graph_profile(tb200_graph* g, float* layer_ms, int num_layers)
 {
-    if (!g || !layer_ms || num_layers < (int)g->layers.size()) return fail(TB200_ERR_INVALID, "bad arguments");
-    CUDA_OK(cudaSetDevice(g->ctx->device)); // the shard of GPU 0 (every shard runs the same launch sequence on its slice)
+    if (!g || !layer_ms || num_layers < (int)g->shards[0].layers.size()) return fail(TB200_ERR_INVALID, "bad arguments");
+    const Shard& s0 = g->shards[0]; // every shard runs the same launch sequence on its slice
+    CUDA_OK(cudaSetDevice(s0.gpu->device));
     for (int i = 0; i < num_layers; i++) layer_ms[i] = 0.f;
     cudaEvent_t a, b;
     CUDA_OK(cudaEventCreate(&a));
     CUDA_OK(cudaEventCreate(&b));
     int rc = 0;
-    for (const Step& s : g->cur->steps)
+    for (const Step& s : s0.cur->steps)
     {
-        cudaEventRecord(a, g->ctx->stream);
-        rc = run_step(g, s, g->ctx->stream);
-        cudaEventRecord(b, g->ctx->stream);
+        cudaEventRecord(a, s0.gpu->stream);
+        rc = run_step(&s0, s, s0.gpu->stream);
+        cudaEventRecord(b, s0.gpu->stream);
         if (rc) break;
         if (cudaEventSynchronize(b) != cudaSuccess)
         {
@@ -2457,7 +2406,7 @@ static int yolo_detect(tb200_graph* g, const tb200_yolo_params* p, tb200_detecti
     if (!g || !p || !out || !counts || max_per_image < 1 || p->num_heads < 1 || p->num_heads > 3) return fail(TB200_ERR_INVALID, "bad arguments");
     const int max_cand = p->max_candidates > 0 ? p->max_candidates : 4096;
     static_assert(sizeof(YoloDet) == sizeof(tb200_detection), "detection record layout");
-    const int rc = for_each_busy_shard(g, [&](tb200_graph* sh, int) -> int {
+    return for_each_busy_shard(g, [&](Shard* sh, int) -> int {
         const TensorInfo* heads[3] = {};
         for (int hd = 0; hd < p->num_heads; hd++)
         {
@@ -2475,9 +2424,8 @@ static int yolo_detect(tb200_graph* g, const tb200_yolo_params* p, tb200_detecti
             float sig[3][256];
         } tab;
         for (int hd = 0; hd < p->num_heads; hd++) build_yolo_tables(heads[hd]->d, tab.sig[hd], tab.ex[hd]);
-        CUDA_OK(cudaSetDevice(sh->ctx->device));
         cudaGetLastError(); // the launches below report cudaGetLastError(): a non-sticky error an earlier call left behind is not theirs
-        cudaStream_t st = sh->ctx->stream;
+        cudaStream_t st = sh->gpu->stream;
         const int n_img = sh->num_images;
         YoloCand *cand = nullptr, *sorted = nullptr;
         YoloDet* det = nullptr;
@@ -2512,8 +2460,6 @@ static int yolo_detect(tb200_graph* g, const tb200_yolo_params* p, tb200_detecti
         if (e != cudaSuccess) return fail(TB200_ERR_CUDA, "yolo_detect: %s", cudaGetErrorString(e));
         return 0;
     });
-    cudaSetDevice(g->ctx->device);
-    return rc;
 }
 
 int tb200_graph_yolo_detect(tb200_graph* g, const tb200_yolo_params* p, tb200_detection* out, int max_per_image, int32_t* counts)
@@ -2543,16 +2489,15 @@ static int class_topk_check(int data_type, float scale, long long e, int k)
 
 int tb200_graph_topk(tb200_graph* g, int output_index, int k, tb200_class_score* out)
 {
-    if (!g || !out || output_index < 0 || output_index >= (int)g->output_ids.size()) return fail(TB200_ERR_INVALID, "bad topk arguments");
+    if (!g || !out || output_index < 0 || output_index >= (int)g->shards[0].output_ids.size()) return fail(TB200_ERR_INVALID, "bad topk arguments");
     {
-        const tb200_tensor_desc& d = g->tensors[g->output_ids[output_index]].d;
+        const tb200_tensor_desc& d = g->shards[0].tensors[g->shards[0].output_ids[output_index]].d;
         if (const int rc = class_topk_check(d.data_type, d.scale, (long long)d.dims[1] * d.dims[2] * d.dims[3], k)) return rc;
     }
-    const int rc = for_each_busy_shard(g, [&](tb200_graph* sh, int) -> int {
+    return for_each_busy_shard(g, [&](Shard* sh, int) -> int {
         const TensorInfo& t = sh->tensors[sh->output_ids[output_index]];
-        CUDA_OK(cudaSetDevice(sh->ctx->device));
         cudaGetLastError(); // the launch below reports cudaGetLastError(): a non-sticky error an earlier call left behind is not its own
-        cudaStream_t st = sh->ctx->stream;
+        cudaStream_t st = sh->gpu->stream;
         const size_t bytes = sizeof(ClassScore) * (size_t)sh->num_images * k;
         ClassScore* dev = nullptr;
         cudaError_t e = cudaMalloc(&dev, bytes);
@@ -2564,15 +2509,17 @@ int tb200_graph_topk(tb200_graph* g, int output_index, int k, tb200_class_score*
         if (e != cudaSuccess) return fail(TB200_ERR_CUDA, "topk: %s", cudaGetErrorString(e));
         return 0;
     });
-    cudaSetDevice(g->ctx->device);
-    return rc;
 }
 
 int tb200_graph_work(tb200_graph* g, double* ops, double* bytes)
 {
     if (!g) return fail(TB200_ERR_INVALID, "null graph");
-    double o = g->cur->work_ops, b = g->cur->work_bytes;
-    for (tb200_graph* sh : g->shards) o += sh->cur->work_ops, b += sh->cur->work_bytes - sh->cur->work_wbytes; // weights count once per launch
+    double o = 0, b = 0;
+    for (size_t r = 0; r < g->shards.size(); r++) // the weights count once per launch
+    {
+        const BatchPlan& bp = *g->shards[r].cur;
+        o += bp.work_ops, b += bp.work_bytes - (r ? bp.work_wbytes : 0);
+    }
     if (ops) *ops = o;
     if (bytes) *bytes = b;
     return 0;
