@@ -16,6 +16,7 @@
 #include <cstdio>
 #include <cstring>
 #include <string>
+#include <variant>
 #include <vector>
 
 #include "../../include/tengine_b200.h"
@@ -83,6 +84,7 @@ struct tb200_context
     std::vector<const void*> host_reg_failed;
 };
 
+// A layer's kernel (LayerPlan::kind, hashed into the pack-cache key) and a step's; the last three only a step takes (build_steps)
 enum StepKind
 {
     K_NCHW2NHWC,
@@ -101,39 +103,41 @@ enum StepKind
     K_LUT,
     K_SOFTMAX,
     K_RESHAPE,
-    K_NONE // a node folded into its producer
+    K_NONE,        // a node folded into its producer
+    K_CONV_WINDOW, // K_GATHER_TC with a window plan
+    K_CONV_DW_TMA, // K_CONV_DW with a TMA plan
+    K_CONCAT_LUT,  // K_CONCAT_PART for a 16-channel-aligned input
+    K_NUM_KINDS
 };
 static const char* kStepName[] = {"nchw_to_nhwc", "nhwc_to_nchw", "conv_stem_nchw_dp4a", "conv_gather_tcgen05", "conv_dw_direct", "conv_direct_dp4a",
                                   "gemm_i8_tcgen05", "conv_igemm_i8_tcgen05", "pool", "pointwise", "concat_requant", "upsample_nearest", "copy",
-                                  "byte_lut", "softmax", "reshape_nchw_order", "fused_into_producer"};
+                                  "byte_lut", "softmax", "reshape_nchw_order", "fused_into_producer", "conv_window_tcgen05", "conv_dw3x3_tma_dp4a",
+                                  "concat_requant"};
+static_assert(sizeof kStepName / sizeof kStepName[0] == K_NUM_KINDS, "one name per step kind");
+
+// The arguments of each step kind's launch
+struct LayoutArgs { const void* in; void* out; int n, c, h, w; }; // K_NCHW2NHWC, K_NHWC2NCHW
+struct ConvArgs { const void* in; const void* w; void* out; ConvShape cs; EpiParams epi; }; // K_CONV_STEM, K_CONV_DW, K_CONV_DIRECT
+struct GatherArgs { ConvArgs conv; int nhwc16; }; // nhwc16: the input is a 16-channel NHWC tensor (else the NCHW network input)
+struct WindowArgs { ConvArgs conv; WindowPlan wp; };
+struct DwTmaArgs { ConvArgs conv; DwPlan dwp; };
+struct GemmArgs { GemmPlan gemm; EpiParams epi; const int32_t* btab; }; // K_GEMM, K_IGEMM; btab: uint8 padding-tap corrections
+struct PoolArgs { const void* in; void* out; PoolShape ps; bool u8; };
+struct PointwiseArgs { const void* in; const void* in2; void* out; long long bytes; PointwiseParams pp; bool u8; }; // in2: eltwise operand
+struct ConcatArgs { const void* in; void* out; ConcatPart part; bool u8; }; // K_CONCAT_PART, K_CONCAT_LUT: one input of the concat
+struct ByteLutArgs { const void* in; void* out; const uint8_t* lut; long long bytes; int c, cp; };
+struct SoftmaxArgs { const void* in; void* out; SoftmaxShape sm; bool u8; };
+struct ReshapeArgs { const void* in; void* scratch; void* out; int n, c, h, w, oc, oh, ow; }; // through an NCHW-ordered scratch
+struct UpsampleArgs { const void* in; void* out; int n, h, w, cp, scale; };
+struct CopyArgs { const void* in; void* out; size_t bytes; };
 
 struct Step
 {
     int kind;
     int layer; // -1 for layout steps
-    const void* in = nullptr;
-    const void* in2 = nullptr;
-    const void* w = nullptr;
-    void* out = nullptr;
-    ConvShape cs{};
-    PoolShape ps{};
-    PointwiseParams pp{};
-    EpiParams epi{};
-    GemmPlan gemm{};
-    const int32_t* btab = nullptr; // uint8 tensor-core kinds: padding-tap corrections
-    DwPlan dwp{};
-    WindowPlan wp{}; // K_GATHER_TC: TMA-staged input window (conv_window.cu) when applicable
-    long long bytes = 0; // pointwise / copy
-    // concat / layout
-    long long npix = 0;
-    int c = 0, cp_in = 0, cp_out = 0, c_off = 0, n = 0, h = 0, w_ = 0, scale = 0;
-    int c_write = 0;             // concat: channels written from c_off (the last input also clears the pad lanes)
-    int oc_ = 0, oh_ = 0, ow_ = 0; // reshape: output dims
-    void* scratch = nullptr;     // reshape: NCHW-ordered staging
-    int nhwc16 = 0; // K_GATHER_TC: the input is a 16-channel NHWC tensor (else the NCHW network input)
-    float s_in = 0, s_out = 0;
-    int z_in = 0, z_out = 0;
-    bool u8 = false;
+    std::variant<LayoutArgs, ConvArgs, GatherArgs, WindowArgs, DwTmaArgs, GemmArgs, PoolArgs, PointwiseArgs, ConcatArgs, ByteLutArgs, SoftmaxArgs,
+                 ReshapeArgs, UpsampleArgs, CopyArgs>
+        args;
 };
 
 struct TensorInfo
@@ -458,42 +462,44 @@ static size_t gemm_weight_bytes(int ocp, int k)
     return (size_t)nt * bn * k;
 }
 
+// The record of step s, of the type build_steps gives its kind (std::get would export std::bad_variant_access from the library)
+template <class A> static const A& args(const Step& s)
+{
+    if (const A* a = std::get_if<A>(&s.args)) return *a;
+    abort(); // a bug in step building
+}
+
 static int run_step(const Shard* g, const Step& s, cudaStream_t st)
 {
+    const int sms = g->gpu->num_sms;
     cudaError_t err = cudaSuccess;
     switch (s.kind)
     {
-    case K_NCHW2NHWC: err = launch_nchw_to_nhwc(s.in, s.out, s.n, s.c, s.h, s.w_, st); break;
-    case K_NHWC2NCHW: err = launch_nhwc_to_nchw(s.in, s.out, s.n, s.c, s.h, s.w_, st); break;
-    case K_CONV_STEM: err = launch_conv_stem(s.in, s.w, s.out, s.cs, s.epi, st); break;
-    case K_GATHER_TC:
-        err = s.wp.valid ? launch_conv_window(s.wp, s.w, s.out, s.cs, s.epi, g->gpu->num_sms, st)
-                         : launch_conv_gather_tc(s.in, s.w, s.out, s.cs, s.epi, s.nhwc16, g->gpu->num_sms, st);
-        break;
-    case K_CONV_DW:
-        err = s.dwp.valid ? launch_conv_dw_tma(s.dwp, s.w, s.out, s.cs, s.epi, st) : launch_conv_dw(s.in, s.w, s.out, s.cs, s.epi, st);
-        break;
-    case K_CONV_DIRECT: err = launch_conv_direct(s.in, s.w, s.out, s.cs, s.epi, st); break;
+    case K_NCHW2NHWC: { auto& a = args<LayoutArgs>(s); err = launch_nchw_to_nhwc(a.in, a.out, a.n, a.c, a.h, a.w, st); break; }
+    case K_NHWC2NCHW: { auto& a = args<LayoutArgs>(s); err = launch_nhwc_to_nchw(a.in, a.out, a.n, a.c, a.h, a.w, st); break; }
+    case K_CONV_STEM: { auto& a = args<ConvArgs>(s); err = launch_conv_stem(a.in, a.w, a.out, a.cs, a.epi, st); break; }
+    case K_CONV_DW: { auto& a = args<ConvArgs>(s); err = launch_conv_dw(a.in, a.w, a.out, a.cs, a.epi, st); break; }
+    case K_CONV_DIRECT: { auto& a = args<ConvArgs>(s); err = launch_conv_direct(a.in, a.w, a.out, a.cs, a.epi, st); break; }
+    case K_GATHER_TC: { auto& a = args<GatherArgs>(s); err = launch_conv_gather_tc(a.conv.in, a.conv.w, a.conv.out, a.conv.cs, a.conv.epi, a.nhwc16, sms, st); break; }
+    case K_CONV_WINDOW: { auto& a = args<WindowArgs>(s); err = launch_conv_window(a.wp, a.conv.w, a.conv.out, a.conv.cs, a.conv.epi, sms, st); break; }
+    case K_CONV_DW_TMA: { auto& a = args<DwTmaArgs>(s); err = launch_conv_dw_tma(a.dwp, a.conv.w, a.conv.out, a.conv.cs, a.conv.epi, st); break; }
     case K_GEMM:
-    case K_IGEMM: err = launch_gemm_i8(s.gemm, s.epi, s.btab, g->gpu->num_sms, st); break;
-    case K_POOL: err = launch_pool(s.in, s.out, s.ps, s.u8, st); break;
-    case K_POINTWISE: err = launch_pointwise(s.in, s.in2, s.out, s.bytes, s.pp, s.u8, st); break;
-    case K_CONCAT_PART:
-        if (s.scale == 1) // 16-channel-aligned input: vectorised, requantisation as a byte table (s.w; nullptr = equal quantisation)
-        {
-            err = launch_concat_lut(s.in, s.out, (const uint8_t*)s.w, s.npix, s.c, s.c_write, s.cp_in, s.cp_out, s.c_off, st);
-            break;
-        }
-        err = launch_concat_part(s.in, s.out, s.npix, s.c, s.c_write, s.cp_in, s.cp_out, s.c_off, s.s_in, s.z_in, s.s_out, s.z_out, s.u8, st);
-        break;
-    case K_LUT: err = launch_byte_lut(s.in, s.out, (const uint8_t*)s.w, s.bytes, s.c, s.cp_in, st); break;
-    case K_SOFTMAX: err = launch_softmax(s.in, s.out, s.npix, s.c, s.cp_in, s.s_in, s.z_in, s.s_out, s.z_out, s.u8, st); break;
+    case K_IGEMM: { auto& a = args<GemmArgs>(s); err = launch_gemm_i8(a.gemm, a.epi, a.btab, sms, st); break; }
+    case K_POOL: { auto& a = args<PoolArgs>(s); err = launch_pool(a.in, a.out, a.ps, a.u8, st); break; }
+    case K_POINTWISE: { auto& a = args<PointwiseArgs>(s); err = launch_pointwise(a.in, a.in2, a.out, a.bytes, a.pp, a.u8, st); break; }
+    case K_CONCAT_PART: { auto& a = args<ConcatArgs>(s); err = launch_concat_part(a.in, a.out, a.part, a.u8, st); break; }
+    case K_CONCAT_LUT: { auto& a = args<ConcatArgs>(s); err = launch_concat_lut(a.in, a.out, a.part, st); break; }
+    case K_LUT: { auto& a = args<ByteLutArgs>(s); err = launch_byte_lut(a.in, a.out, a.lut, a.bytes, a.c, a.cp, st); break; }
+    case K_SOFTMAX: { auto& a = args<SoftmaxArgs>(s); err = launch_softmax(a.in, a.out, a.sm, a.u8, st); break; }
     case K_RESHAPE:
-        err = launch_nhwc_to_nchw(s.in, s.scratch, s.n, s.c, s.h, s.w_, st);
-        if (err == cudaSuccess) err = launch_nchw_to_nhwc(s.scratch, s.out, s.n, s.oc_, s.oh_, s.ow_, st);
+    {
+        auto& a = args<ReshapeArgs>(s);
+        err = launch_nhwc_to_nchw(a.in, a.scratch, a.n, a.c, a.h, a.w, st);
+        if (err == cudaSuccess) err = launch_nchw_to_nhwc(a.scratch, a.out, a.n, a.oc, a.oh, a.ow, st);
         break;
-    case K_UPSAMPLE: err = launch_upsample(s.in, s.out, s.n, s.h, s.w_, s.cp_in, s.scale, st); break;
-    case K_COPY: err = cudaMemcpyAsync(s.out, s.in, (size_t)s.bytes, cudaMemcpyDeviceToDevice, st); break;
+    }
+    case K_UPSAMPLE: { auto& a = args<UpsampleArgs>(s); err = launch_upsample(a.in, a.out, a.n, a.h, a.w, a.cp, a.scale, st); break; }
+    case K_COPY: { auto& a = args<CopyArgs>(s); err = cudaMemcpyAsync(a.out, a.in, a.bytes, cudaMemcpyDeviceToDevice, st); break; }
     }
     if (err != cudaSuccess) return fail(TB200_ERR_CUDA, "launch of %s (layer %d) failed: %s", kStepName[s.kind], s.layer, cudaGetErrorString(err));
     return 0;
@@ -1395,15 +1401,13 @@ static int fill_conv_step(Shard* g, int li, const LayerPlan& P, const Slice& sl,
     const int N = sl.nb, C = tin.d.dims[1], H = tin.d.dims[2], W = tin.d.dims[3];
     const int OC = tout.d.dims[1], OH = tout.d.dims[2], OW = tout.d.dims[3];
     const bool fc = L.op == TB200_OP_FC;
-    s.w = g->w_arena + P.blob.w_off;
-    s.epi = make_epi(L, tin.d, tout.d, fc);
-    s.epi.bias = (const int32_t*)(g->w_arena + P.blob.bias_off);
-    s.epi.w_scale = (const float*)(g->w_arena + P.blob.scale_off);
-    s.epi.fast_par = (const float2*)(g->w_arena + P.blob.fast_off);
-    s.btab = (const int32_t*)(g->w_arena + P.blob.btab_off);
-    s.epi.fuse_bias = P.fuse_bias;
-    if (!P.fast_ok) s.epi.fast_ok = 0;
-    ConvShape& cs = s.cs;
+    ConvArgs c{sl.dev(tin), g->w_arena + P.blob.w_off, sl.dev(tout), {}, make_epi(L, tin.d, tout.d, fc)};
+    c.epi.bias = (const int32_t*)(g->w_arena + P.blob.bias_off);
+    c.epi.w_scale = (const float*)(g->w_arena + P.blob.scale_off);
+    c.epi.fast_par = (const float2*)(g->w_arena + P.blob.fast_off);
+    c.epi.fuse_bias = P.fuse_bias;
+    if (!P.fast_ok) c.epi.fast_ok = 0;
+    ConvShape& cs = c.cs;
     cs.n = N, cs.h = H, cs.w = W, cs.c = C, cs.cp = tin.cp, cs.oh = OH, cs.ow = OW, cs.oc = OC, cs.ocp = tout.cp;
     if (fc)
     {
@@ -1425,28 +1429,34 @@ static int fill_conv_step(Shard* g, int li, const LayerPlan& P, const Slice& sl,
         work->work_bytes += (double)in_bytes + out_bytes + (double)OC * k + (L.bias ? 4.0 * OC : 0);
         work->work_wbytes += (double)OC * k + (L.bias ? 4.0 * OC : 0);
     }
-    if (P.reads_nchw) s.in = g->in_nchw_dev[tin.input_index] + sl.off(tin.nchw_bytes);
-    s.nhwc16 = P.nhwc16;
-    if (s.kind == K_GATHER_TC)
+    if (P.reads_nchw) c.in = g->in_nchw_dev[tin.input_index] + sl.off(tin.nchw_bytes);
+    if (P.kind == K_GATHER_TC)
     {
-        window_plan_create(&s.wp, s.in, s.cs, s.nhwc16); // falls back to the global-memory gather (16 channels / NCHW only)
-        if (!s.wp.valid && s.nhwc16 && tin.cp != 16) return fail(TB200_ERR_UNSUPPORTED, "layer %d: window plan failed for a 32-channel 3x3 convolution", li);
+        WindowArgs a{c, {}};
+        window_plan_create(&a.wp, c.in, c.cs, P.nhwc16); // falls back to the global-memory gather (16 channels / NCHW only)
+        if (a.wp.valid) s.kind = K_CONV_WINDOW, s.args = a;
+        else if (P.nhwc16 && tin.cp != 16) return fail(TB200_ERR_UNSUPPORTED, "layer %d: window plan failed for a 32-channel 3x3 convolution", li);
+        else s.args = GatherArgs{c, P.nhwc16};
     }
-    if (s.kind == K_CONV_DW && !(g->flags & TB200_PRERUN_NO_TENSORCORE)) dw_plan_create(&s.dwp, s.in, s.cs, s.epi); // falls back when not applicable
-    if (s.kind == K_IGEMM)
+    else if (P.kind == K_CONV_DW)
     {
-        int rc = gemm_plan_create_conv(&s.gemm, s.in, s.w, s.out, s.cs, P.gemm_zp);
-        if (rc) return fail(rc, "layer %d: implicit-GEMM plan failed", li);
-        s.gemm.fixq = g->gpu->fixq, s.gemm.fixq_cap = FIXQ_CAP;
+        DwTmaArgs a{c, {}};
+        if (!(g->flags & TB200_PRERUN_NO_TENSORCORE)) dw_plan_create(&a.dwp, c.in, c.cs, c.epi); // falls back when not applicable
+        if (a.dwp.valid) s.kind = K_CONV_DW_TMA, s.args = a;
+        else s.args = c;
     }
-    if (s.kind == K_GEMM)
+    else if (P.kind == K_GEMM || P.kind == K_IGEMM)
     {
+        GemmArgs& a = s.args.emplace<GemmArgs>(GemmArgs{{}, c.epi, (const int32_t*)(g->w_arena + P.blob.btab_off)});
         const long long m = fc ? N : (long long)N * H * W;
         const int kdim = fc ? H * W * tin.cp : tin.cp;
-        int rc = gemm_plan_create(&s.gemm, s.in, kdim, s.w, s.out, m, kdim, OC, tout.cp, tout.cp, P.gemm_zp);
+        int rc = P.kind == K_IGEMM ? gemm_plan_create_conv(&a.gemm, c.in, c.w, c.out, c.cs, P.gemm_zp)
+                                   : gemm_plan_create(&a.gemm, c.in, kdim, c.w, c.out, m, kdim, OC, tout.cp, tout.cp, P.gemm_zp);
+        if (rc && P.kind == K_IGEMM) return fail(rc, "layer %d: implicit-GEMM plan failed", li);
         if (rc) return fail(rc, "layer %d: TMA descriptor creation failed (m=%lld k=%d oc=%d)", li, m, kdim, OC);
-        s.gemm.fixq = g->gpu->fixq, s.gemm.fixq_cap = FIXQ_CAP;
+        a.gemm.fixq = g->gpu->fixq, a.gemm.fixq_cap = FIXQ_CAP;
     }
+    else s.args = c;
     return 0;
 }
 
@@ -1456,13 +1466,14 @@ static int fill_pool_step(const Shard* g, int li, const LayerPlan& P, const Slic
     const TensorInfo& tin = g->tensors[L.inputs[0]];
     const TensorInfo& tout = g->tensors[L.output];
     const int H = tin.d.dims[2], W = tin.d.dims[3], C = tin.d.dims[1];
-    PoolShape& p = s.ps;
+    PoolArgs& a = s.args.emplace<PoolArgs>(PoolArgs{sl.dev(tin), sl.dev(tout), {}, tin.d.data_type == TB200_DT_UINT8});
+    PoolShape& p = a.ps;
     p.n = sl.nb, p.h = H, p.w = W, p.c = C, p.cp = tin.cp, p.oh = tout.d.dims[2], p.ow = tout.d.dims[3];
     p.kh = L.kernel_h, p.kw = L.kernel_w, p.sh = L.stride_h, p.sw = L.stride_w, p.ph0 = L.pad_h0, p.pw0 = L.pad_w0;
     p.method = L.pool_method, p.caffe_flavor = L.caffe_flavor;
     p.in_scale = tin.d.scale, p.out_scale = tout.d.scale, p.in_zero = tin.d.zero_point, p.out_zero = tout.d.zero_point;
     if (L.pool_global) p.kh = H, p.kw = W, p.sh = p.sw = 1, p.ph0 = p.pw0 = 0;
-    p.lut = P.pool_relu >= 0 ? g->w_arena + P.blob.w_off : nullptr, p.c_real = s.u8 ? C : tin.cp;
+    p.lut = P.pool_relu >= 0 ? g->w_arena + P.blob.w_off : nullptr, p.c_real = a.u8 ? C : tin.cp;
     if (tout.d.dims[1] != C) return fail(TB200_ERR_INVALID, "layer %d: pool channel mismatch", li);
     return 0;
 }
@@ -1473,7 +1484,8 @@ static int fill_pointwise_step(const Shard* g, int li, const LayerPlan& P, const
     const tb200_layer_desc& L = g->layers[li];
     const TensorInfo& tin = g->tensors[L.inputs[0]];
     const TensorInfo& tout = g->tensors[L.output];
-    PointwiseParams& p = s.pp;
+    PointwiseArgs& a = s.args.emplace<PointwiseArgs>(PointwiseArgs{sl.dev(tin), nullptr, sl.dev(tout), sl.bytes(tin), {}, tin.d.data_type == TB200_DT_UINT8});
+    PointwiseParams& p = a.pp;
     p.c = tin.d.dims[1], p.cp = tin.cp;
     p.scale0 = tin.d.scale, p.zero0 = tin.d.zero_point, p.out_scale = tout.d.scale, p.out_zero = tout.d.zero_point;
     p.negative_slope = L.negative_slope;
@@ -1486,9 +1498,8 @@ static int fill_pointwise_step(const Shard* g, int li, const LayerPlan& P, const
         if (t1.nhwc_bytes != tin.nhwc_bytes) return fail(TB200_ERR_UNSUPPORTED, "layer %d: eltwise broadcast", li);
         p.mode = L.elt_type == TB200_ELT_SUM ? 1 : 2;
         p.scale1 = t1.d.scale, p.zero1 = t1.d.zero_point;
-        s.in2 = sl.dev(t1);
+        a.in2 = sl.dev(t1);
     }
-    s.bytes = sl.bytes(tin);
     if (tout.nhwc_bytes != tin.nhwc_bytes) return fail(TB200_ERR_INVALID, "layer %d: pointwise shape mismatch", li);
     return 0;
 }
@@ -1499,18 +1510,18 @@ static int fill_concat_steps(const Shard* g, int li, const LayerPlan& P, const S
     const tb200_layer_desc& L = g->layers[li];
     const TensorInfo& tin = g->tensors[L.inputs[0]];
     const TensorInfo& tout = g->tensors[L.output];
+    const bool u8 = tin.d.data_type == TB200_DT_UINT8;
     int coff = 0;
     for (int k = 0; k < L.num_inputs; k++)
     {
         const TensorInfo& tk = g->tensors[L.inputs[k]];
-        Step p = s;
-        p.in = sl.dev(tk);
-        p.npix = (long long)sl.nb * tin.d.dims[2] * tin.d.dims[3], p.c = tk.d.dims[1], p.cp_in = tk.cp, p.cp_out = tout.cp, p.c_off = coff;
-        p.s_in = tk.d.scale, p.z_in = tk.d.zero_point, p.s_out = tout.d.scale, p.z_out = tout.d.zero_point;
-        p.c_write = (k + 1 == L.num_inputs) ? tout.cp - coff : tk.d.dims[1];
+        ConcatPart q{};
+        q.npix = (long long)sl.nb * tin.d.dims[2] * tin.d.dims[3], q.c = tk.d.dims[1], q.cp_in = tk.cp, q.cp_out = tout.cp, q.c_off = coff;
+        q.s_in = tk.d.scale, q.z_in = tk.d.zero_point, q.s_out = tout.d.scale, q.z_out = tout.d.zero_point;
+        q.c_write = (k + 1 == L.num_inputs) ? tout.cp - coff : tk.d.dims[1];
         // vectorised table path when everything is 16-channel aligned; identical quantisation -> no table at all
-        p.scale = (tk.d.dims[1] % 16 == 0 && coff % 16 == 0) ? 1 : 0;
-        p.w = (tk.d.scale == tout.d.scale && tk.d.zero_point == tout.d.zero_point) ? nullptr : g->w_arena + P.blob.w_off + 256 * k;
+        q.lut = (tk.d.scale == tout.d.scale && tk.d.zero_point == tout.d.zero_point) ? nullptr : g->w_arena + P.blob.w_off + 256 * k;
+        const Step p{tk.d.dims[1] % 16 == 0 && coff % 16 == 0 ? K_CONCAT_LUT : K_CONCAT_PART, li, ConcatArgs{sl.dev(tk), sl.dev(tout), q, u8}};
         coff += tk.d.dims[1];
         if (k + 1 < L.num_inputs) steps.push_back(p);
         else s = p;
@@ -1527,29 +1538,28 @@ static int fill_data_step(const Shard* g, int li, const LayerPlan& P, const Slic
     const TensorInfo& tout = g->tensors[L.output];
     const int N = sl.nb, C = tin.d.dims[1], H = tin.d.dims[2], W = tin.d.dims[3];
     const int OC = tout.d.dims[1], OH = tout.d.dims[2], OW = tout.d.dims[3];
+    const void* in = sl.dev(tin);
+    void* out = sl.dev(tout);
     switch (P.kind)
     {
     case K_UPSAMPLE:
-        s.n = N, s.h = H, s.w_ = W, s.cp_in = tin.cp, s.scale = L.up_scale;
+        s.args = UpsampleArgs{in, out, N, H, W, tin.cp, L.up_scale};
         if (OH != H * L.up_scale || OW != W * L.up_scale) return fail(TB200_ERR_INVALID, "layer %d: upsample shape", li);
         break;
     case K_LUT:
-        s.w = g->w_arena + P.blob.w_off;
-        s.bytes = sl.bytes(tin);
-        s.c = C, s.cp_in = tin.cp;
+        s.args = ByteLutArgs{in, out, g->w_arena + P.blob.w_off, sl.bytes(tin), C, tin.cp};
         if (tout.nhwc_bytes != tin.nhwc_bytes) return fail(TB200_ERR_INVALID, "layer %d: unary op changes the shape", li);
         break;
     case K_SOFTMAX:
         if (tout.nhwc_bytes != tin.nhwc_bytes) return fail(TB200_ERR_INVALID, "layer %d: softmax changes the shape", li);
-        s.npix = (long long)N * H * W, s.c = C, s.cp_in = tin.cp;
-        s.s_in = tin.d.scale, s.z_in = tin.d.zero_point, s.s_out = tout.d.scale, s.z_out = tout.d.zero_point;
+        s.args = SoftmaxArgs{in, out, {(long long)N * H * W, C, tin.cp, tin.d.scale, tout.d.scale, tin.d.zero_point, tout.d.zero_point},
+                             tin.d.data_type == TB200_DT_UINT8};
         break;
-    case K_RESHAPE:
-        s.n = N, s.c = C, s.h = H, s.w_ = W, s.oc_ = OC, s.oh_ = OH, s.ow_ = OW;
-        s.scratch = g->act_arena + P.scratch_off; // NCHW-ordered bytes of this chunk (chunks never run concurrently)
+    case K_RESHAPE: // the scratch holds the NCHW-ordered bytes of this chunk (chunks never run concurrently)
+        s.args = ReshapeArgs{in, g->act_arena + P.scratch_off, out, N, C, H, W, OC, OH, OW};
         break;
     case K_COPY:
-        s.bytes = sl.bytes(tin);
+        s.args = CopyArgs{in, out, (size_t)sl.bytes(tin)};
         if (tout.nhwc_bytes != tin.nhwc_bytes) return fail(TB200_ERR_UNSUPPORTED, "layer %d: identity changes the NHWC footprint", li);
         break;
     }
@@ -1563,12 +1573,7 @@ static int build_steps(Shard* g, int first, int nb, std::vector<Step>& steps, Ba
     const std::vector<LayerPlan>& plan = g->plan;
     const Slice sl{first, nb, g->tensors[0].d.dims[0]};
     auto layout_step = [&](int kind, const void* in, void* out, const TensorInfo& t)
-    {
-        Step s;
-        s.kind = kind, s.layer = -1, s.in = in, s.out = out;
-        s.n = nb, s.c = t.d.dims[1], s.h = t.d.dims[2], s.w_ = t.d.dims[3];
-        steps.push_back(s);
-    };
+    { steps.push_back(Step{kind, -1, LayoutArgs{in, out, nb, t.d.dims[1], t.d.dims[2], t.d.dims[3]}}); };
     for (size_t i = 0; i < g->input_ids.size(); i++)
     {
         const TensorInfo& t = g->tensors[g->input_ids[i]];
@@ -1579,10 +1584,7 @@ static int build_steps(Shard* g, int first, int nb, std::vector<Step>& steps, Ba
         const tb200_layer_desc& L = g->layers[li];
         const LayerPlan& P = plan[li];
         if (P.kind == K_NONE) continue;
-        const TensorInfo& tin = g->tensors[L.inputs[0]];
-        Step s;
-        s.kind = P.kind, s.layer = li, s.u8 = tin.d.data_type == TB200_DT_UINT8;
-        s.in = sl.dev(tin), s.out = sl.dev(g->tensors[L.output]);
+        Step s{P.kind, li, {}};
         int rc;
         if (L.op == TB200_OP_CONV || L.op == TB200_OP_FC) rc = fill_conv_step(g, li, P, sl, work, s);
         else if (P.kind == K_POOL) rc = fill_pool_step(g, li, P, sl, s);
@@ -1820,7 +1822,7 @@ int tb200_graph_prerun(tb200_context* ctx, const tb200_tensor_desc* tensors, int
         g->layer_kernel.assign(num_layers, kStepName[K_NONE]);
         for (const Step& s : g->shards[0].prepared.steps)
             if (s.layer >= 0)
-                g->layer_kernel[s.layer] = (s.kind == K_CONV_DW && s.dwp.valid) ? "conv_dw3x3_tma_dp4a" : ((s.kind == K_GATHER_TC && s.wp.valid) ? "conv_window_tcgen05" : kStepName[s.kind]);
+                g->layer_kernel[s.layer] = kStepName[s.kind];
         if (!(flags & TB200_PRERUN_NO_WEIGHTS) && (rc = upload_weights(g)) == 0) rc = broadcast_arena(g);
     }
     if (rc)

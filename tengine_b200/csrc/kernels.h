@@ -37,19 +37,36 @@ struct PointwiseParams
     uint32_t post_floor4; // uint8: the output zero point replicated x4
 };
 
+// One input of a concat: its c channels (pitch cp_in) of npix pixels go to output channels [c_off, c_off + c_write) (pitch cp_out);
+// the last input's c_write reaches cp_out, so it also clears the output's pad lanes.
+struct ConcatPart
+{
+    long long npix;
+    int c, c_write, cp_in, cp_out, c_off;
+    float s_in, s_out; // requantisation from the input's quantisation to the output's
+    int z_in, z_out;
+    const uint8_t* lut; // the same requantisation as a 256-entry byte table (launch_concat_lut); nullptr = equal quantisation
+};
+
+struct SoftmaxShape
+{
+    long long npix;
+    int c, cp;
+    float s_in, s_out;
+    int z_in, z_out;
+};
+
 cudaError_t launch_conv_direct(const void* in, const void* w, void* out, const ConvShape& s, const EpiParams& e, cudaStream_t st);
 cudaError_t launch_conv_dw(const void* in, const void* w, void* out, const ConvShape& s, const EpiParams& e, cudaStream_t st);
 cudaError_t launch_conv_stem(const void* in, const void* w, void* out, const ConvShape& s, const EpiParams& e, cudaStream_t st);
 cudaError_t launch_pool(const void* in, void* out, const PoolShape& p, bool u8, cudaStream_t st);
 cudaError_t launch_pointwise(const void* a, const void* b, void* out, long long bytes, const PointwiseParams& p, bool u8, cudaStream_t st);
-cudaError_t launch_concat_part(const void* in, void* out, long long npix, int c, int c_write, int cp_in, int cp_out, int c_off, float s_in,
-                               int z_in, float s_out, int z_out, bool u8, cudaStream_t st);
+cudaError_t launch_concat_part(const void* in, void* out, const ConcatPart& p, bool u8, cudaStream_t st);
 // unary byte ops (sigmoid, hardswish) as a 256-entry table built at prerun; pad lanes (channel >= c) stay 0
 cudaError_t launch_byte_lut(const void* in, void* out, const uint8_t* lut, long long bytes, int c, int cp, cudaStream_t st);
 // softmax over the channel axis (softmax_kernel_ref_int8.c / _uint8.c), one thread per pixel
-cudaError_t launch_softmax(const void* in, void* out, long long npix, int c, int cp, float s_in, int z_in, float s_out, int z_out, bool u8,
-                           cudaStream_t st);
-cudaError_t launch_concat_lut(const void* in, void* out, const uint8_t* lut, long long npix, int c, int c_write, int cp_in, int cp_out, int c_off, cudaStream_t st);
+cudaError_t launch_softmax(const void* in, void* out, const SoftmaxShape& p, bool u8, cudaStream_t st);
+cudaError_t launch_concat_lut(const void* in, void* out, const ConcatPart& p, cudaStream_t st);
 cudaError_t launch_upsample(const void* in, void* out, int n, int h, int w, int cp, int scale, cudaStream_t st);
 cudaError_t launch_nchw_to_nhwc(const void* in, void* out, int n, int c, int h, int w, cudaStream_t st);
 cudaError_t launch_nhwc_to_nchw(const void* in, void* out, int n, int c, int h, int w, cudaStream_t st);

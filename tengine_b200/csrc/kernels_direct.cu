@@ -940,22 +940,21 @@ __global__ void __launch_bounds__(256) concat_lut_kernel(const uint4* __restrict
     *reinterpret_cast<uint4*>(out + (size_t)pix * cp_out + c_off + v * 16) = r;
 }
 
-cudaError_t launch_concat_lut(const void* in, void* out, const uint8_t* lut, long long npix, int c, int c_write, int cp_in, int cp_out, int c_off, cudaStream_t st)
+cudaError_t launch_concat_lut(const void* in, void* out, const ConcatPart& p, cudaStream_t st)
 {
-    if ((c % 16) || (c_off % 16) || (c_write % 16)) return cudaErrorInvalidValue;
-    const long long total = npix * (c_write / 16);
+    if ((p.c % 16) || (p.c_off % 16) || (p.c_write % 16)) return cudaErrorInvalidValue;
+    const long long total = p.npix * (p.c_write / 16);
     TB200_CHECK_32BIT(total * 16);
-    concat_lut_kernel<<<blocks_for(total, 256), 256, 0, st>>>((const uint4*)in, (uint8_t*)out, lut, npix, c / 16, c_write / 16, cp_in, cp_out, c_off);
+    concat_lut_kernel<<<blocks_for(total, 256), 256, 0, st>>>((const uint4*)in, (uint8_t*)out, p.lut, p.npix, p.c / 16, p.c_write / 16, p.cp_in, p.cp_out, p.c_off);
     return cudaGetLastError();
 }
 
-cudaError_t launch_concat_part(const void* in, void* out, long long npix, int c, int c_write, int cp_in, int cp_out, int c_off, float s_in,
-                               int z_in, float s_out, int z_out, bool u8, cudaStream_t st)
+cudaError_t launch_concat_part(const void* in, void* out, const ConcatPart& p, bool u8, cudaStream_t st)
 {
-    const long long total = npix * c_write;
+    const long long total = p.npix * p.c_write;
     TB200_CHECK_32BIT(total);
-    if (u8) concat_kernel<true><<<blocks_for(total, 256), 256, 0, st>>>((const uint8_t*)in, (uint8_t*)out, npix, c, c_write, cp_in, cp_out, c_off, s_in, z_in, s_out, z_out);
-    else concat_kernel<false><<<blocks_for(total, 256), 256, 0, st>>>((const uint8_t*)in, (uint8_t*)out, npix, c, c_write, cp_in, cp_out, c_off, s_in, z_in, s_out, z_out);
+    auto kern = u8 ? concat_kernel<true> : concat_kernel<false>;
+    kern<<<blocks_for(total, 256), 256, 0, st>>>((const uint8_t*)in, (uint8_t*)out, p.npix, p.c, p.c_write, p.cp_in, p.cp_out, p.c_off, p.s_in, p.z_in, p.s_out, p.z_out);
     return cudaGetLastError();
 }
 
@@ -1036,12 +1035,11 @@ __global__ void __launch_bounds__(128) softmax_kernel(const uint8_t* __restrict_
     for (int k = c; k < cp; k++) op[k] = 0;
 }
 
-cudaError_t launch_softmax(const void* in, void* out, long long npix, int c, int cp, float s_in, int z_in, float s_out, int z_out, bool u8,
-                           cudaStream_t st)
+cudaError_t launch_softmax(const void* in, void* out, const SoftmaxShape& p, bool u8, cudaStream_t st)
 {
-    TB200_CHECK_32BIT(npix);
-    if (u8) softmax_kernel<true><<<blocks_for(npix, 128), 128, 0, st>>>((const uint8_t*)in, (uint8_t*)out, npix, c, cp, s_in, z_in, s_out, z_out);
-    else softmax_kernel<false><<<blocks_for(npix, 128), 128, 0, st>>>((const uint8_t*)in, (uint8_t*)out, npix, c, cp, s_in, z_in, s_out, z_out);
+    TB200_CHECK_32BIT(p.npix);
+    if (u8) softmax_kernel<true><<<blocks_for(p.npix, 128), 128, 0, st>>>((const uint8_t*)in, (uint8_t*)out, p.npix, p.c, p.cp, p.s_in, p.z_in, p.s_out, p.z_out);
+    else softmax_kernel<false><<<blocks_for(p.npix, 128), 128, 0, st>>>((const uint8_t*)in, (uint8_t*)out, p.npix, p.c, p.cp, p.s_in, p.z_in, p.s_out, p.z_out);
     return cudaGetLastError();
 }
 

@@ -124,7 +124,7 @@ def dw_geometry(u8, kh, kw, stride, oh, ow, dil=1):
     return D
 
 
-# ---- engine.cu plan_conv (:768-809): the kernel of a convolution -----------------------------------------------------------
+# ---- engine.cu plan_conv: the kernel of a convolution ------------------------------------------------------------------------
 def conv_kind(g, L, no_tc=False):
     """'gemm', 'igemm', 'dw', 'direct', 'stem', 'gather' (NCHW stem / 16-channel input) or 'window32' (32-channel 3x3: decided by
     window_nhwc_fits, which is not restated: no entry here takes that branch)."""
@@ -179,12 +179,12 @@ def layer_geometry(g, L):
     return dict(kind=kind)
 
 
-KERNEL_NAME = {"gemm": "gemm_i8_tcgen05", "igemm": "conv_igemm_i8_tcgen05", "direct": "conv_direct_dp4a"}  # engine.cu kStepName
+KERNEL_NAME = {"gemm": "gemm_i8_tcgen05", "igemm": "conv_igemm_i8_tcgen05", "direct": "conv_direct_dp4a"}  # engine.cu kStepName, per step kind
 
 
 def kernel_name(geo):
     if geo["kind"] == "dw":
-        return "conv_dw3x3_tma_dp4a" if geo["valid"] else "conv_dw_direct"  # engine.cu:1653
+        return "conv_dw3x3_tma_dp4a" if geo["valid"] else "conv_dw_direct"  # engine.cu fill_conv_step: K_CONV_DW_TMA or K_CONV_DW
     return KERNEL_NAME[geo["kind"]]
 
 
@@ -207,7 +207,7 @@ def geometry(g, L):
     if L["op"] == abi.OP_POOL:
         return pool_geometry(g, L)
     if L["op"] == abi.OP_CONCAT:
-        # engine.cu concat step: an input takes the byte table when its channel count and channel offset are multiples of 16
+        # engine.cu fill_concat_steps: an input takes the byte table (K_CONCAT_LUT) when its channel count and offset are multiples of 16
         offs = np.cumsum([0] + [g.tensors[t]["dims"][1] for t in L["inputs"]])
         table = [g.tensors[t]["dims"][1] % 16 == 0 and o % 16 == 0 for t, o in zip(L["inputs"], offs)]
         return dict(kind="concat", inputs=len(table), mixed=any(table) and not all(table))
@@ -304,7 +304,7 @@ def _repad(case, pad):
 
 def concat_n(rng, u8, chans, shape=(2, 5, 7)):
     """Concat of len(chans) inputs with s_in / s_out = 1/2, 1/4, 1/2, ... (t = q/2, q/4): inputs whose channel count and offset
-    are multiples of 16 take the byte table, the others the bytewise path (engine.cu concat step)."""
+    are multiples of 16 take the byte table, the others the bytewise path (engine.cu fill_concat_steps)."""
     g = GraphDef(abi.DT_UINT8 if u8 else abi.DT_INT8)
     n, h, w = shape
     ins, xs = [], []
