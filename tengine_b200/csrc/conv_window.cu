@@ -187,9 +187,12 @@ __global__ void __launch_bounds__(128) conv_window_tc_kernel(const __grid_consta
 #pragma unroll
                 for (int j = 0; j < NW; j++) sx = (int32_t)__dp4a(row[j], 0x01010101u, (unsigned)sx);
             }
+            // only the a.ks k-steps shared memory holds (C < 3 7x7: 2 or 4 of 5); the B tiles start right after them
+            constexpr int KS_MIN = (KHW * KHW + 31) / 32; // one channel's k-steps: always present
 #pragma unroll
             for (int j = 0; j < NW / 4; j++)
-                sts_u4(sA + (uint32_t)(j >> 1) * 4096u + sw32_offset(tid, j & 1), row[4 * j], row[4 * j + 1], row[4 * j + 2], row[4 * j + 3]);
+                if ((j >> 1) < KS_MIN || (j >> 1) < a.ks)
+                    sts_u4(sA + (uint32_t)(j >> 1) * 4096u + sw32_offset(tid, j & 1), row[4 * j], row[4 * j + 1], row[4 * j + 2], row[4 * j + 3]);
         }
         else
         {
@@ -316,7 +319,10 @@ cudaError_t launch_conv_window(const WindowPlan& p, const void* w, void* out, co
         err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, conv_window_tc_kernel<MD, U, LY>, 128, (size_t)p.smem_bytes);          \
         if (err != cudaSuccess) return err;                                                                                                 \
         const unsigned cap = (unsigned)num_sms * (unsigned)(per_sm > 1 ? per_sm : 1), grid = a.ntiles < cap ? a.ntiles : cap;             \
-        if (debug_launch()) fprintf(stderr, "tengine_b200: launch conv_window_tc_kernel<MODE=%d,U8=%d,LAYOUT=%d>\n", MD, (int)U, LY);     \
+        if (debug_launch())                                                                                                                 \
+            fprintf(stderr, "tengine_b200: launch conv_window_tc_kernel<MODE=%d,U8=%d,LAYOUT=%d> layout=%d xoff=%d box_w=%d box_h=%d ks=%d "   \
+                            "smem=%d tiles_w=%d tiles_h=%d grid=%u\n", MD, (int)U, LY, p.layout, p.xoff, p.box_w, p.box_h, p.ks,              \
+                    p.smem_bytes, a.tiles_w, a.tiles_h, grid);                                                                              \
         conv_window_tc_kernel<MD, U, LY><<<grid, 128, (size_t)p.smem_bytes, st>>>(tm, a, e);                                                \
         return cudaGetLastError();                                                                                                          \
     }
@@ -427,9 +433,12 @@ __global__ void __launch_bounds__(128) conv_gather_tc_kernel(const GatherArgs a,
 #pragma unroll
                 for (int j = 0; j < NW; j++) sx = (int32_t)__dp4a(row[j], 0x01010101u, (unsigned)sx);
             }
+            // only the a.ks k-steps shared memory holds (C < 3 7x7: 2 or 4 of 5); the B tiles start right after them
+            constexpr int KS_MIN = (KHW * KHW + 31) / 32; // one channel's k-steps: always present
 #pragma unroll
             for (int j = 0; j < NW / 4; j++)
-                sts_u4(sA + (uint32_t)(j >> 1) * 4096u + sw32_offset(tid, j & 1), row[4 * j], row[4 * j + 1], row[4 * j + 2], row[4 * j + 3]);
+                if ((j >> 1) < KS_MIN || (j >> 1) < a.ks)
+                    sts_u4(sA + (uint32_t)(j >> 1) * 4096u + sw32_offset(tid, j & 1), row[4 * j], row[4 * j + 1], row[4 * j + 2], row[4 * j + 3]);
         }
         fence_proxy_async_smem(); // the MMAs read these generic-proxy writes through the async proxy
         __syncthreads();          // (first iteration: also publishes the B tiles and the constants)
@@ -478,7 +487,9 @@ cudaError_t launch_conv_gather_tc(const void* in, const void* w, void* out, cons
             cudaError_t err = cudaFuncSetAttribute(conv_gather_tc_kernel<MD, U, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
             if (err != cudaSuccess) return err;                                                                                    \
         }                                                                                                                          \
-        if (debug_launch()) fprintf(stderr, "tengine_b200: launch conv_gather_tc_kernel<MODE=%d,U8=%d,KHW=%d>\n", MD, (int)U, K);  \
+        if (debug_launch())                                                                                                        \
+            fprintf(stderr, "tengine_b200: launch conv_gather_tc_kernel<MODE=%d,U8=%d,KHW=%d> ks=%d ntiles=%u\n", MD, (int)U, K, a.ks, \
+                    a.ntiles);                                                                                                     \
         conv_gather_tc_kernel<MD, U, K><<<grid, 128, smem, st>>>(a, e);                                                            \
         return cudaGetLastError();                                                                                                 \
     }

@@ -4,9 +4,10 @@ restated in Python.
 The tie-dense builders of tests/ties.py make the layers (power-of-two scales: `ties.exact_run` is an exact reference, independent
 of the oracle); ops that `ties.exact_layer` does not cover (softmax, upsample, sigmoid) are compared with the oracle instead.
 
-`gemm_geometry`, `dw_geometry` and `conv_kind` restate the C planners line by line (cited at each function).  They only describe
-what the library decides -- no plan logic lives here -- so that the CPU test can show every entry reaches the geometry it is
-meant to, and the GPU test can tie the restatement to the library (TB200_DEBUG_LAUNCH prints the GEMM's plan).
+`gemm_geometry`, `dw_geometry`, `window_geometry`, `gather_geometry`, `epi_clamp` and `conv_kind` restate the C planners line by
+line (cited at each function).  They only describe what the library decides -- no plan logic lives here -- so that the CPU test
+can show every entry reaches the geometry it is meant to, and the GPU test can tie the restatement to the library
+(TB200_DEBUG_LAUNCH prints the plans of the GEMM, the window and the gather kernel).
 
 Every boundary is probed from both sides: an entry per side, listed in `BOUNDARIES`.
 """
@@ -124,10 +125,95 @@ def dw_geometry(u8, kh, kw, stride, oh, ow, dil=1):
     return D
 
 
-# ---- engine.cu plan_conv: the kernel of a convolution ------------------------------------------------------------------------
+# ---- conv_window.cu: the window kernel's plan and the gather kernel's tiles ---------------------------------------------------
+WINDOW_SMEM_MAX = 200 * 1024
+
+
+def _acc_pitch(ocp):
+    return ocp * 4 + 16  # tc_common.cuh acc_pitch
+
+
+def window_smem_bytes(ks, ocp, in_bytes):
+    return ks * 4096 + ks * ocp * 32 + ocp * 8 + 128 + 2 * ((in_bytes + 127) & ~127) + 128 * _acc_pitch(ocp) + 1024
+
+
+def window_nhwc_fits(cp, ocp, stride):
+    box_w, box_h = 15 * stride + 3, 7 * stride + 3
+    return window_smem_bytes((9 * cp + 31) // 32, ocp, box_w * box_h * cp) <= WINDOW_SMEM_MAX
+
+
+def window_geometry(n, c, cp, w, oh, ow, k, stride, pw0, ocp, nhwc):
+    """window_plan_create's checks beyond plan_conv's (group 1, no dilation, one stride, square kernel), its box and shared
+    memory, and the tile arithmetic of launch_conv_window: 16 x 8 output pixels per tile, the two tile counts divided by
+    multiply-high with a magic number, 0 for a divisor of 1."""
+    W = dict(valid=False, layout=None)
+    if stride > 2 or ocp > 256:
+        return W
+    if nhwc:
+        if k != 3 or cp not in (16, 32):
+            return W
+        layout, xoff = (2 if cp == 16 else 3), 0
+        box_w, box_h = 15 * stride + 3, 7 * stride + 3
+        in_bytes, ks = box_w * box_h * cp, (9 * cp + 31) // 32
+    else:
+        if k not in (3, 7) or c > 3 or w % 16:
+            return W
+        layout, xoff = (0 if k == 3 else 1), (16 - pw0 % 16) % 16
+        box_w, box_h = (xoff + 15 * stride + k + 15) & ~15, 7 * stride + k
+        if box_w > 256 or box_h > 256:
+            return W
+        in_bytes, ks = box_w * box_h * c, (c * k * k + 31) // 32
+    W.update(layout=layout, xoff=xoff, box_w=box_w, box_h=box_h, ks=ks, smem_bytes=window_smem_bytes(ks, ocp, in_bytes))
+    if W["smem_bytes"] > WINDOW_SMEM_MAX:
+        return W
+    W["valid"] = True
+    W["tiles_w"], W["tiles_h"] = tw, th = (ow + 15) // 16, (oh + 7) // 8
+    W["ntiles"] = tw * th * n
+    W["tw_magic0"], W["th_magic0"], W["batch1"] = tw == 1, th == 1, n == 1
+    W["ow_mod16"], W["oh_mod8"] = ow % 16, oh % 8
+    return W
+
+
+def gather_geometry(n, c, oh, ow, k, nhwc16):
+    """launch_conv_gather_tc: 128 output pixels per tile; ks k-steps of 32 bytes (NHWC16: nine 16-byte taps and a zero half)."""
+    npix = n * oh * ow
+    return dict(ks=5 if nhwc16 else (c * k * k + 31) // 32, ntiles=(npix + 127) // 128, npix_mod128=npix % 128)
+
+
+# ---- engine.cu make_epi: the activation's clamp in the fast epilogues -------------------------------------------------------
+def epi_clamp(g, L):
+    """The activation's bounds in real units (flo, fhi), over s_out: whether one is a half-integer (the reference rounds the
+    clipped value, away from zero), and whether one lies beyond the byte range (the integer clamp is then saturation's)."""
+    fc = L["op"] == abi.OP_FC
+    act = -1 if fc else L["activation"]
+    flo, fhi = -np.inf, np.inf
+    if L["recipe"] == abi.RECIPE_HCL or fc:
+        if act == 0:
+            flo = 0.0
+        if act > 0:
+            flo, fhi = 0.0, 6.0
+    elif act >= 0:
+        flo, fhi = (-1.0, 1.0) if act == 1 else (0.0, 6.0 if act == 6 else np.inf)
+    tout = g.tensors[L["output"]]
+    so, zo = np.float32(tout["scale"]), tout["zero_point"]
+    bounds = [b / so for b in (flo, fhi) if np.isfinite(b)]
+    lo, hi = (-zo, 255 - zo) if g.data_type == abi.DT_UINT8 else (-127, 127)
+    name = "none" if act < 0 else ("hcl" if L["recipe"] == abi.RECIPE_HCL else "ref") + str(act)
+    return dict(act=name, bound_half=any(b - np.floor(b) == 0.5 for b in bounds),
+                bound_beyond_sat=any(ties._round_away(b) < lo or ties._round_away(b) > hi for b in bounds))
+
+
+# ---- engine.cu plan_conv and fill_conv_step: the kernel of a convolution ----------------------------------------------------
+def _window_of(g, L, nhwc):
+    n, C, _, W = g.tensors[L["inputs"][0]]["dims"]
+    _, OC, OH, OW = g.tensors[L["output"]]["dims"]
+    return window_geometry(n, C, cpad(C), W, OH, OW, L["kernel_h"], L["stride_h"], L["pad_w0"], cpad(OC), nhwc)
+
+
 def conv_kind(g, L, no_tc=False):
-    """'gemm', 'igemm', 'dw', 'direct', 'stem', 'gather' (NCHW stem / 16-channel input) or 'window32' (32-channel 3x3: decided by
-    window_nhwc_fits, which is not restated: no entry here takes that branch)."""
+    """'gemm', 'igemm', 'dw', 'direct', 'stem', 'window' or 'gather'.  plan_conv's K_GATHER_TC (NCHW stem, 16-channel input)
+    becomes 'window' when window_plan_create makes a plan, else 'gather' (fill_conv_step); its 32-channel branch needs
+    window_nhwc_fits and otherwise falls through to the implicit GEMM."""
     tin, tout = g.tensors[L["inputs"][0]], g.tensors[L["output"]]
     _, C, _, _ = tin["dims"]
     OC, OW = tout["dims"][1], tout["dims"][3]
@@ -140,13 +226,13 @@ def conv_kind(g, L, no_tc=False):
     gather = tc and plain and ocp <= 256
     nopad = not (L["pad_h0"] or L["pad_h1"] or L["pad_w0"] or L["pad_w1"])
     if is_input and C <= 3 and gather and kh == kw and kh in (3, 7):
-        return "gather"
+        return "window" if _window_of(g, L, 0)["valid"] else "gather"
     if is_input and C <= 4 and grp == 1:
         return "stem"
     if gather and k3 and cp == 16:
-        return "gather"
-    if gather and k3 and cp == 32 and sh in (1, 2):
-        return "window32"
+        return "window" if _window_of(g, L, 1)["valid"] else "gather"
+    if gather and k3 and cp == 32 and sh in (1, 2) and window_nhwc_fits(32, ocp, sh):
+        return "window"
     if grp == C and OC == C and C > 1:
         return "dw"
     if tc and kh == 1 and kw == 1 and sh == 1 and sw == 1 and nopad:
@@ -156,30 +242,50 @@ def conv_kind(g, L, no_tc=False):
     return "direct"
 
 
-def layer_geometry(g, L):
-    """The restated plan of a conv / FC layer: dict with 'kind' and the kind's geometry."""
+def layer_geometry(g, L, no_tc=False):
+    """The restated plan of a conv / FC layer: dict with 'kind', the kind's geometry and the epilogue's clamp."""
     u8 = g.data_type == abi.DT_UINT8
     n, C, Hh, W = g.tensors[L["inputs"][0]]["dims"]
     _, OC, OH, OW = g.tensors[L["output"]]["dims"]
     cp, ocp = cpad(C), cpad(OC)
     zp = (1 + L["weight_zero"]) if u8 else 0
+    epi = epi_clamp(g, L)
     if L["op"] == abi.OP_FC:
-        return dict(kind="gemm", **gemm_geometry(ocp, zp, m=n, k=Hh * W * cp))
-    kind = conv_kind(g, L)
+        if no_tc:
+            return dict(kind="direct", oct=8, **epi)
+        return dict(kind="gemm", **gemm_geometry(ocp, zp, m=n, k=Hh * W * cp), **epi)
+    kind = conv_kind(g, L, no_tc)
     if kind == "gemm":
-        return dict(kind=kind, **gemm_geometry(ocp, zp, m=n * Hh * W, k=cp))
+        return dict(kind=kind, **gemm_geometry(ocp, zp, m=n * Hh * W, k=cp), **epi)
     if kind == "igemm":
         return dict(kind=kind, **gemm_geometry(ocp, zp, conv=dict(n=n, h=Hh, w=W, cp=cp, oh=OH, ow=OW, kh=L["kernel_h"],
                                                                    kw=L["kernel_w"], stride=L["stride_h"], ph0=L["pad_h0"],
-                                                                   pw0=L["pad_w0"])))
+                                                                   pw0=L["pad_w0"])), **epi)
     if kind == "dw":
-        D = dw_geometry(u8, L["kernel_h"], L["kernel_w"], L["stride_h"] if L["stride_h"] == L["stride_w"] else 0, OH, OW,
-                        max(L["dilation_h"], L["dilation_w"]))
-        return dict(kind=kind, cp_mod32=cp % 32, **D)
-    return dict(kind=kind)
+        s = L["stride_h"] if L["stride_h"] == L["stride_w"] else 0
+        D = dw_geometry(u8, L["kernel_h"], L["kernel_w"], s, OH, OW, max(L["dilation_h"], L["dilation_w"]))
+        if no_tc:
+            D["valid"] = False  # fill_conv_step makes no TMA plan
+        # kernels_direct.cu launch_conv_dw without a TMA plan: int8 3x3 at stride 1 / 2 takes TW output pixels per thread
+        i8_3x3 = not u8 and L["kernel_h"] == L["kernel_w"] == 3 and max(L["dilation_h"], L["dilation_w"]) == 1 and s in (1, 2)
+        if not D["valid"]:
+            D["dw_kernel"] = "dw3x3_i8" if i8_3x3 else "generic"
+            D["dw_ow_tail"] = OW % (8 if s == 1 else 4) if i8_3x3 else None
+        return dict(kind=kind, cp_mod32=cp % 32, **D, **epi)
+    nhwc = cp in (16, 32) and not (C <= 3 and L["inputs"][0] in g.inputs)
+    if kind == "window":
+        return dict(kind=kind, window_valid=True, **_window_of(g, L, int(nhwc)), **epi)
+    if kind == "gather":
+        return dict(kind=kind, window_valid=False, **gather_geometry(n, C, OH, OW, L["kernel_h"], int(nhwc)), **epi)
+    if kind == "stem":
+        return dict(kind=kind, oct=32 if ocp % 32 == 0 else 16, **epi)  # kernels_direct.cu launch_conv_stem
+    og = OC // L["group"]
+    return dict(kind=kind, oct=4 if L["group"] > 1 and og % 8 else 8, **epi)  # kernels_direct.cu launch_conv_direct
 
 
-KERNEL_NAME = {"gemm": "gemm_i8_tcgen05", "igemm": "conv_igemm_i8_tcgen05", "direct": "conv_direct_dp4a"}  # engine.cu kStepName, per step kind
+# engine.cu kStepName, per step kind
+KERNEL_NAME = {"gemm": "gemm_i8_tcgen05", "igemm": "conv_igemm_i8_tcgen05", "direct": "conv_direct_dp4a", "stem": "conv_stem_nchw_dp4a",
+               "window": "conv_window_tcgen05", "gather": "conv_gather_tcgen05"}
 
 
 def kernel_name(geo):
@@ -201,9 +307,9 @@ def pool_geometry(g, L):
                 one_sided_pad=(L["pad_h0"] > 0) != (L["pad_h1"] > 0) or (L["pad_w0"] > 0) != (L["pad_w1"] > 0))
 
 
-def geometry(g, L):
+def geometry(g, L, no_tc=False):
     if L["op"] in (abi.OP_CONV, abi.OP_FC):
-        return layer_geometry(g, L)
+        return layer_geometry(g, L, no_tc)
     if L["op"] == abi.OP_POOL:
         return pool_geometry(g, L)
     if L["op"] == abi.OP_CONCAT:
@@ -227,6 +333,7 @@ class Entry:
     ref: str = "exact"     # "exact": ties.exact_run; "oracle": the oracle (ops outside ties.exact_layer)
     fused: bool = False    # run under the default plan (node fusion on); only the graph output is compared
     ties: bool = True      # built tie-dense (ties.check_not_vacuous applies)
+    flags: int = 0         # prerun flags ORed into the run's (PRERUN_NO_TENSORCORE: the CUDA-core kernels)
     notes: dict = field(default_factory=dict)
 
 
@@ -277,29 +384,58 @@ def int8_fc_hw(rng, n, c, h, w, oc, mode=0, m_exps=ties.M_EXPS, tie_frac=0.10):
     return cs
 
 
-def u8_conv_pad(rng, n, c, h, w, oc, k, stride, pad, mode=0):
-    """uint8 conv with a 4-tuple padding (h0, h1, w0, w1): ties.uint8_conv's layer, rebuilt through g.conv(..., pad=...)."""
+def u8_conv_pad(rng, n, c, h, w, oc, k, stride, pad, mode=0, dilation=1):
+    """uint8 conv with a 4-tuple padding (h0, h1, w0, w1) or a dilation: ties.uint8_conv's layer, rebuilt through
+    g.conv(..., pad=..., dilation=...)."""
     case = ties.uint8_conv(rng, n, c, h, w, oc, k=k, stride=stride, pad=0, mode=mode)
-    return _repad(case, pad)
+    return _repad(case, pad, dilation)
 
 
-def i8_conv_pad(rng, n, c, h, w, oc, k, stride, pad, mode=1):
+def i8_conv_pad(rng, n, c, h, w, oc, k, stride, pad, mode=1, dilation=1):
     case = ties.int8_conv(rng, n, c, h, w, oc, k=k, stride=stride, pad=0, mode=mode)
-    return _repad(case, pad)
+    return _repad(case, pad, dilation)
 
 
-def _repad(case, pad):
+def _repad(case, pad, dilation=1):
     g0 = case.g
     L = g0.layers[0]
     t0, to = g0.tensors[L["inputs"][0]], g0.tensors[L["output"]]
     g = GraphDef(g0.data_type)
     x = g.input(*t0["dims"], t0["scale"], t0["zero_point"])
     y = g.conv(x, L["weight"], L["bias"], L["weight_scales"], to["scale"], to["zero_point"], stride=L["stride_h"], pad=pad,
-               group=L["group"], activation=L["activation"], recipe=L["recipe"], weight_zero=L["weight_zero"])
+               dilation=dilation, group=L["group"], activation=L["activation"], recipe=L["recipe"], weight_zero=L["weight_zero"])
     g.mark_output(y)
     case.g = g
     case.mode = ties.planned_mode(g, g.layers[0])
     return case
+
+
+def act_conv(rng, u8, n, c, h, w, oc, activation, recipe, s_out, k=3, stride=1, pad=1, group=1, zo=110, t_mid=0.0):
+    """A conv whose t = f / s_out lies within a few units of t_mid, so that the activation's clamp cuts it: the clamp bounds over
+    a power-of-two s_out (6 / 4 = 1.5, 1 / 2 = 0.5) are half-integers, which the reference rounds away from zero.  M = 2^-1
+    (every odd accumulator is a tie); weights +-1 on about six taps per output, inputs in [-2, 2] about the zero point, so t
+    spreads over about +-2 whatever K is."""
+    g = GraphDef(abi.DT_UINT8 if u8 else abi.DT_INT8)
+    s_in, M = 2.0 ** -4, 0.5
+    cg = c // group
+    kk = cg * k * k
+    zx, zw = (ties.U8_ZX, ties.U8_ZW) if u8 else (0, 0)
+    x = g.input(n, c, h, w, s_in, zx)
+    wd = rng.choice(np.array([-1, 1]), (oc, cg, k, k)) * (rng.random((oc, cg, k, k)) < min(1.0, 6.0 / kk))
+    b = (np.round(t_mid / M) + rng.integers(-2, 3, oc)).astype(np.int32)
+    s_w = M * s_out / s_in
+    if u8:
+        y = g.conv(x, (zw + wd).astype(np.uint8), b, [s_w], s_out, zo, stride=stride, pad=pad, group=group,
+                   activation=activation, recipe=recipe, weight_zero=zw)
+    else:
+        y = g.conv(x, wd.astype(np.int8), b, np.full(oc, s_w, np.float32), s_out, stride=stride, pad=pad, group=group,
+                   activation=activation, recipe=recipe)
+    g.mark_output(y)
+    xin = (zx + rng.integers(-2, 3, (n, c, h, w))).astype(np.uint8 if u8 else np.int8)
+    cs = ties.Case(("uint8" if u8 else "int8") + f"_act{activation}_r{recipe}_so{s_out}_n{n}c{c}_{h}x{w}_oc{oc}_k{k}", g, [xin],
+                   min_tie_frac=0.05)
+    cs.mode = ties.planned_mode(g, g.layers[0])
+    return cs
 
 
 def concat_n(rng, u8, chans, shape=(2, 5, 7)):
@@ -454,6 +590,105 @@ _add("dw3x3s1_i8_oh1_capped", _i8(3, 32, 1, 20, 32, k=3, pad=1, group=32, mode=0
 _add("dw3x3s2_i8_oh2_capped", _i8(2, 48, 3, 30, 48, k=3, stride=2, pad=1, group=48, mode=1), D_, dict(valid=True, rows_capped=True))
 _add("dw3x3s1_i8_oh17_full", _i8(1, 32, 17, 30, 32, k=3, pad=1, group=32, mode=1), D_, dict(valid=True, rows_capped=False, rows_per_cta=4))
 
+# ---- NCHW stems: the window kernel (W % 16 == 0, stride 1 / 2) and the gather kernel -----------------------------------------
+WI, GA, ST, DR = "conv_window_tcgen05", "conv_gather_tcgen05", "conv_stem_nchw_dp4a", "conv_direct_dp4a"
+NO_TC = abi.PRERUN_NO_TENSORCORE
+
+
+def _both(name, n, c, h, w, oc, k, stride, pad, kernel, edges, group=1, **kw):
+    """The int8 and the uint8 entry of one conv shape (pad: an int or the 4-tuple (h0, h1, w0, w1)); modes as ties' defaults."""
+    if isinstance(pad, tuple):
+        _add(name.format("i8"), lambda r: i8_conv_pad(r, n, c, h, w, oc, k, stride, pad), kernel, edges, **kw)
+        _add(name.format("u8"), lambda r: u8_conv_pad(r, n, c, h, w, oc, k, stride, pad), kernel, edges, **kw)
+    else:
+        _add(name.format("i8"), _i8(n, c, h, w, oc, k=k, stride=stride, pad=pad, group=group), kernel, edges, **kw)
+        _add(name.format("u8"), _u8(n, c, h, w, oc, k=k, stride=stride, pad=pad, group=group), kernel, edges, **kw)
+
+
+# 7x7 over 1 and 2 channels: 2 and 4 k-steps of A in shared memory (of the 5 a 147-byte row could fill), B right after them
+_both("win7x7s2_{}_c1_p3", 2, 1, 21, 32, 24, 7, 2, 3, WI, dict(layout=1, ks=2, xoff=13, tiles_w=1, tw_magic0=True, tiles_h=2, ow_mod16=0))
+_both("win7x7s2_{}_c2_p2", 3, 2, 30, 32, 24, 7, 2, 2, WI, dict(layout=1, ks=4, xoff=14, ow_mod16=15, batch1=False))
+_both("win7x7s1_{}_c3_p0", 1, 3, 14, 32, 40, 7, 1, 0, WI, dict(layout=1, ks=5, xoff=0, tiles_w=2, tiles_h=1, th_magic0=True,
+                                                                          oh_mod8=0, batch1=True))
+_both("win7x7s1_{}_c1_p1", 1, 1, 22, 48, 24, 7, 1, 1, WI, dict(layout=1, ks=2, xoff=15, tiles_w=3, th_magic0=False))
+_both("win3x3s1_{}_c1_p1", 2, 1, 15, 32, 24, 3, 1, 1, WI, dict(layout=0, ks=1, xoff=15, oh_mod8=7, tw_magic0=False, window_valid=True))
+_both("win3x3s2_{}_c2_p2", 3, 2, 16, 64, 24, 3, 2, 2, WI, dict(layout=0, ks=1, xoff=14, ow_mod16=1, tiles_w=3))
+_both("win3x3s2_{}_c3_pad01", 2, 3, 16, 32, 24, 3, 2, (0, 1, 0, 1), WI, dict(layout=0, xoff=0, ow_mod16=0, oh_mod8=0))
+_both("win3x3s1_{}_c3_p3", 1, 3, 9, 32, 24, 3, 1, 3, WI, dict(layout=0, xoff=13, tiles_h=2, oh_mod8=5))
+# W % 16 != 0 (no tensor map) or stride 3: the gather kernel; the last tile of 128 pixels full, one pixel, 127 pixels
+_both("gat7x7s2_{}_c1_p3", 2, 1, 21, 30, 24, 7, 2, 3, GA, dict(ks=2, window_valid=False))
+_both("gat7x7s1_{}_c2_p3", 1, 2, 12, 20, 24, 7, 1, 3, GA, dict(ks=4, npix_mod128=112))
+_both("gat7x7s2_{}_c3_p3", 2, 3, 16, 24, 40, 7, 2, 3, GA, dict(ks=5))
+_both("gat3x3s1_{}_c1_n2_8x8", 2, 1, 8, 8, 24, 3, 1, 1, GA, dict(ks=1, ntiles=1, npix_mod128=0))
+_both("gat3x3s1_{}_c2_3x43", 1, 2, 3, 43, 24, 3, 1, 1, GA, dict(ks=1, ntiles=2, npix_mod128=1))
+_both("gat3x3s1_{}_c3_5x51", 1, 3, 5, 51, 24, 3, 1, 1, GA, dict(ks=1, ntiles=2, npix_mod128=127))
+_both("gat3x3s3_{}_c3_w32", 2, 3, 14, 32, 24, 3, 3, 1, GA, dict(ks=1, window_valid=False))
+# the planner around the stems: OCp 256 is the tensor-core kernels' (a 7x7 window at xoff 13 no longer fits in shared memory),
+# 272 the stem kernel's; 4 channels, a 5x5 kernel or a dilation take the stem kernel too (OCT 32 when OCp % 32 == 0, else 16)
+_both("win7x7s2_{}_c3_oc256_p0", 1, 3, 16, 32, 256, 7, 2, 0, WI, dict(layout=1, ks=5, smem_bytes=203904))
+_both("gat7x7s2_{}_c3_oc256_p3", 1, 3, 16, 32, 256, 7, 2, 3, GA, dict(ks=5, window_valid=False))
+_both("win3x3s1_{}_c3_oc256", 1, 3, 8, 32, 256, 3, 1, 1, WI, dict(layout=0))
+_both("stem3x3s1_{}_c3_oc272", 1, 3, 8, 32, 272, 3, 1, 1, ST, dict(oct=16))
+_both("stem3x3s2_{}_c4", 2, 4, 11, 14, 32, 3, 2, 1, ST, dict(oct=32))
+_both("stem5x5s2_{}_c3_oc48", 2, 3, 13, 15, 48, 5, 2, 2, ST, dict(oct=16))
+_add("stem3x3d2_i8_c3", lambda r: i8_conv_pad(r, 2, 3, 12, 16, 24, 3, 1, 2, dilation=2), ST, dict(oct=32))
+_add("stem3x3d2_u8_c3", lambda r: u8_conv_pad(r, 2, 3, 12, 16, 24, 3, 1, 2, dilation=2), ST, dict(oct=32))
+_both("stem3x3s1_{}_c3_notc", 2, 3, 9, 16, 24, 3, 1, 1, ST, dict(oct=32), flags=NO_TC)
+
+# ---- NHWC 16- and 32-byte pixels: the window kernel, the gather kernel past its limits, the implicit GEMM past window32's --------
+_both("win3x3s1_{}_c16", 3, 16, 10, 20, 40, 3, 1, 1, WI, dict(layout=2, ks=5, tiles_w=2, tiles_h=2, batch1=False))
+_both("win3x3s2_{}_c16_ocp224", 1, 16, 10, 12, 224, 3, 2, 1, WI, dict(layout=2, ks=5))
+_both("gat3x3s2_{}_c16_ocp240", 1, 16, 10, 12, 240, 3, 2, 1, GA, dict(ks=5, window_valid=False))
+_both("gat3x3s3_{}_c16", 2, 16, 11, 13, 40, 3, 3, 1, GA, dict(ks=5, window_valid=False))
+_both("win3x3s1_{}_c32_ocp176", 1, 32, 8, 18, 176, 3, 1, 1, WI, dict(layout=3, ks=9))
+_both("igemm3x3s1_{}_c32_ocp192", 1, 32, 8, 18, 192, 3, 1, 1, I_, dict(taps=9, block_k=32))
+_both("win3x3s2_{}_c32_ocp144", 1, 32, 9, 20, 144, 3, 2, 1, WI, dict(layout=3, ks=9))
+_both("igemm3x3s2_{}_c32_ocp160", 1, 32, 9, 20, 160, 3, 2, 1, I_, dict(taps=9))
+# uint8 pad lanes (c >= C) inside a 16- / 32-byte pixel: the zero-point fill of border taps must leave them 0
+_add("win3x3s1_u8_c8", _u8(3, 8, 9, 18, 40, k=3, pad=1), WI, dict(layout=2))
+_add("gat3x3s3_u8_c12", _u8(2, 12, 10, 13, 40, k=3, stride=3, pad=1), GA, dict(ks=5))
+_add("win3x3s2_u8_c24", _u8(3, 24, 9, 20, 40, k=3, stride=2, pad=1), WI, dict(layout=3, ks=9))
+
+# ---- CUDA-core kernels: grouped direct conv (OCT 8 / 4), generic depthwise, the int8 depthwise 3x3 without a TMA plan -------
+_both("direct3x3_{}_g4_og8", 2, 32, 7, 9, 32, 3, 1, 1, DR, dict(oct=8), group=4)
+_both("direct3x3_{}_g4_og12", 2, 32, 7, 9, 48, 3, 2, 1, DR, dict(oct=4), group=4)
+_add("dw5x5s1_i8_c32", _i8(2, 32, 9, 11, 32, k=5, pad=2, group=32), DD, dict(valid=False, dw_kernel="generic"))
+_add("dw3x3s2_u8_c32", _u8(2, 32, 9, 11, 32, k=3, stride=2, pad=1, group=32), DD, dict(valid=False, dw_kernel="generic"))
+_add("dw3x3s1_i8_c32_notc", _i8(2, 32, 7, 13, 32, k=3, pad=1, group=32), DD, dict(dw_kernel="dw3x3_i8", dw_ow_tail=5), flags=NO_TC)
+_add("dw3x3s2_i8_c48_notc", _i8(2, 48, 9, 13, 48, k=3, stride=2, pad=1, group=48, mode=0), DD, dict(dw_kernel="dw3x3_i8", dw_ow_tail=3),
+     flags=NO_TC)
+_add("dw3x3s1_i8_c32_w16_notc", _i8(1, 32, 5, 16, 32, k=3, pad=1, group=32), DD, dict(dw_kernel="dw3x3_i8", dw_ow_tail=0), flags=NO_TC)
+
+# ---- activation clamps in the epilogues: ReLU and ReLU6 (HCL), [-1, 1] and ReLU6 (REF) ------------------------------------------
+# s_out = 4 puts ReLU6's bound at t = 1.5, s_out = 2 REF's [-1, 1] at t = +-0.5: half-integer bounds, which the reference's
+# round() takes away from zero; [-1, 1] is the only clamp whose lower integer bound is neither 0 nor -127 (int8: q_byte_add 0xff)
+ACTS = {"hcl0": (0, abi.RECIPE_HCL, 2.0 ** -2), "hcl6": (6, abi.RECIPE_HCL, 4.0), "ref1": (1, abi.RECIPE_REF, 2.0),
+        "ref6": (6, abi.RECIPE_REF, 4.0)}
+_ACT_SHAPES = {  # kernel, (n, c, h, w, oc, k, stride, pad, group), dtypes
+    "win3x3": (WI, (2, 3, 9, 32, 24, 3, 1, 1, 1), ("i8", "u8")),
+    "gat3x3": (GA, (2, 3, 9, 30, 24, 3, 1, 1, 1), ("i8", "u8")),
+    "stem3x3": (ST, (2, 4, 9, 11, 24, 3, 1, 1, 1), ("i8", "u8")),
+    "gemm1x1": (G_, (2, 64, 9, 7, 40, 1, 1, 0, 1), ("i8", "u8")),
+    "dw3x3": (D_, (2, 32, 9, 10, 32, 3, 1, 1, 32), ("i8",)),
+}
+for sh, (kern, (n, c, h, w, oc, k, st, pd, gp), dts) in _ACT_SHAPES.items():
+    for a, (act, rec, so) in ACTS.items():
+        for d in dts:
+            edges = dict(act=a, bound_half=a != "hcl0", bound_beyond_sat=False)
+            if kern == D_:
+                edges["valid"] = True
+            _add(f"{sh}_{d}_{a}", lambda r, d=d, act=act, rec=rec, so=so, n=n, c=c, h=h, w=w, oc=oc, k=k, st=st, pd=pd, gp=gp:
+                 act_conv(r, d == "u8", n, c, h, w, oc, act, rec, so, k=k, stride=st, pad=pd, group=gp, t_mid=0.75), kern, edges)
+# bounds beyond the byte range: ReLU6 at t = 192 > 127 (int8); uint8 output zero points 254 (ReLU6's 2 + 254 > 255) and 0
+# ([-1, 1]'s -1 + 0 < 0)
+_add("win3x3_i8_hcl6_sat", lambda r: act_conv(r, False, 2, 3, 9, 32, 24, 6, abi.RECIPE_HCL, 2.0 ** -5, t_mid=126.5), WI,
+     dict(act="hcl6", bound_half=False, bound_beyond_sat=True))
+_add("win3x3_u8_hcl6_zo254", lambda r: act_conv(r, True, 2, 3, 9, 32, 24, 6, abi.RECIPE_HCL, 4.0, zo=254, t_mid=0.75), WI,
+     dict(act="hcl6", bound_half=True, bound_beyond_sat=True))
+_add("gat3x3_u8_ref1_zo0", lambda r: act_conv(r, True, 2, 3, 9, 30, 24, 1, abi.RECIPE_REF, 2.0, zo=0), GA,
+     dict(act="ref1", bound_half=True, bound_beyond_sat=True))
+_add("stem3x3_u8_ref6_zo254", lambda r: act_conv(r, True, 2, 4, 9, 11, 24, 6, abi.RECIPE_REF, 4.0, zo=254, t_mid=0.75), ST,
+     dict(act="ref6", bound_beyond_sat=True))
 # ---- glue ----------------------------------------------------------------------------------------------------------------
 _P = "pool"
 for d, u in (("i8", False), ("u8", True)):
@@ -518,6 +753,25 @@ BOUNDARIES = {
     "one_sided_pad": {True, False},
     "c_mod16": {0, 8},
     "mixed": {True, False},
+    # the window and the gather kernel
+    "layout": {0, 1, 2, 3},
+    "ks": {1, 2, 4, 5, 9},
+    "xoff": {0, 13, 14, 15},
+    "window_valid": {True, False},
+    "tw_magic0": {True, False},
+    "th_magic0": {True, False},
+    "batch1": {True, False},
+    "ow_mod16": {0, 1, 15},
+    "oh_mod8": {0, 7},
+    "npix_mod128": {0, 1, 127},
+    # the CUDA-core kernels
+    "oct": {4, 8, 16, 32},
+    "dw_kernel": {"dw3x3_i8", "generic"},
+    "dw_ow_tail": {0, 3, 5},
+    # the epilogue's clamp
+    "act": {"hcl0", "hcl6", "ref1", "ref6"},
+    "bound_half": {True, False},
+    "bound_beyond_sat": {True, False},
 }
 
 # Edges no graph can reach, and why (none so far).
@@ -531,3 +785,13 @@ def gemm_entries():
 def uint8_gemm_entries():
     return [n for n in gemm_entries() if "_u8_" in n or n.startswith("fc_u8")]
 
+
+def window_entries():
+    """The window and gather entries: the GPU test ties their printed plans to window_geometry / gather_geometry."""
+    return [n for n, e in ENTRIES.items() if e.kernel in (WI, GA)]
+
+
+def window_batch_entries():
+    """Window entries of 3 or more images: run again on all images but the last (tb200_graph_set_batch), where every slice's
+    tensor map is built from its own n."""
+    return [n for n in window_entries() if ENTRIES[n].kernel == WI and build(n).g.tensors[0]["dims"][0] >= 3]

@@ -1,9 +1,9 @@
 """The edge cases of tests/kernel_edges.py on the device: every layer bit-exact against the exact reference (or the oracle, for
 ops outside ties.exact_layer), with the kernel each entry is meant to reach asserted by name.
 
-Two child processes (`python -m tests.test_gpu_kernel_edges <entry>...`) cover what the library reads once per process:
-  - TB200_DEBUG_LAUNCH: the GEMM's printed plan equals kernel_edges.gemm_geometry for every GEMM entry, so the Python
-    restatement cannot drift from the code unnoticed;
+Child processes (`python -m tests.test_gpu_kernel_edges <entry>...`) cover what the library reads once per process:
+  - TB200_DEBUG_LAUNCH: the printed plans of the GEMM, the window and the gather kernel equal kernel_edges.gemm_geometry,
+    window_geometry and gather_geometry for every entry of theirs, so the Python restatement cannot drift from the code unnoticed;
   - TB200_DEBUG_NO_CPLANE (documented to give wrong uint8 results): the uint8 GEMM entries must FAIL there -- a sweep that passed
     under a known-wrong kernel would prove nothing."""
 import os
@@ -35,7 +35,7 @@ def run_entry(ctx, oracle, name):
         want, rs = ties.exact_run(g, case.inputs)
     else:
         want, rs = oracle.run(g, case.inputs, uint8_mode=0), {}
-    flags = abi.PRERUN_POISON_ARENA | (0 if e.fused else abi.PRERUN_NO_GRAPH)
+    flags = abi.PRERUN_POISON_ARENA | (0 if e.fused else abi.PRERUN_NO_GRAPH) | e.flags
     gr = rt.Graph(ctx, g, flags)
     try:
         outs = gr.run(case.inputs)
@@ -100,6 +100,69 @@ def test_gemm_plan_equals_restatement():
         if not got or any(x != want for x in got):
             bad.append(f"{name}: printed (cs, border, out_mode, conv, n_tiles, b_res, mt, par_all) {got}, restated {want}")
     assert not bad, "\n".join(bad)
+
+
+_WINDOW = re.compile(r"tengine_b200: launch conv_window_tc_kernel<MODE=\d,U8=\d,LAYOUT=(\d)> layout=(\d) xoff=(\d+) box_w=(\d+) box_h=(\d+) "
+                     r"ks=(\d+) smem=(\d+) tiles_w=(\d+) tiles_h=(\d+) grid=(\d+)")
+_GATHER = re.compile(r"tengine_b200: launch conv_gather_tc_kernel<MODE=\d,U8=\d,KHW=(\d)> ks=(\d+) ntiles=(\d+)")
+
+
+def test_window_and_gather_plans_equal_restatement():
+    """Every window / gather entry launches its kernel once, with the plan window_geometry / gather_geometry restate; the window
+    kernel's grid is at most one CTA per tile."""
+    names = ke.window_entries()
+    r = _child(names, {"TB200_DEBUG_LAUNCH": "1"})
+    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
+    printed, cur = {}, None
+    for line in r.stderr.splitlines():
+        if line.startswith(MARK):
+            cur = line[len(MARK):].strip()
+            continue
+        for kind, rx in (("window", _WINDOW), ("gather", _GATHER)):
+            m = rx.match(line)
+            if m and cur:
+                printed.setdefault(cur, []).append((kind,) + tuple(int(v) for v in m.groups()))
+    bad = []
+    for name in names:
+        case = ke.build(name)
+        L = case.g.layers[ke.ENTRIES[name].layer]
+        geo = ke.geometry(case.g, L)
+        if geo["kind"] == "window":
+            want = ("window", geo["layout"], geo["layout"], geo["xoff"], geo["box_w"], geo["box_h"], geo["ks"], geo["smem_bytes"],
+                    geo["tiles_w"], geo["tiles_h"])
+            got = [p[:-1] for p in printed.get(name, [])]
+            if any(p[0] == "window" and not 1 <= p[-1] <= geo["ntiles"] for p in printed.get(name, [])):
+                bad.append(f"{name}: grid {[p[-1] for p in printed[name]]} for {geo['ntiles']} tiles")
+        else:
+            khw = 3 if L["kernel_h"] == 3 else 7
+            want = ("gather", khw, geo["ks"], geo["ntiles"])
+            got = printed.get(name, [])
+        if len(got) != 1 or got[0] != want:
+            bad.append(f"{name}: printed {got}, restated {want}")
+    assert not bad, "\n".join(bad)
+
+
+@pytest.mark.parametrize("name", ke.window_batch_entries())
+def test_window_entry_on_part_of_the_batch(ctx, name):
+    """fill_conv_step builds each slice's window tensor map from the slice's own n: a graph prepared for n images runs on the
+    first n - 1 (tb200_graph_set_batch) and then on all n again, bit-exact to the reference each time."""
+    from tengine_b200 import runtime as rt
+
+    e = ke.ENTRIES[name]
+    case = ke.build(name)
+    g, x = case.g, case.inputs[0]
+    want, _ = ties.exact_run(g, case.inputs)
+    n = x.shape[0]
+    gr = rt.Graph(ctx, g, abi.PRERUN_POISON_ARENA | abi.PRERUN_NO_GRAPH | e.flags)
+    try:
+        for b in (n - 1, n):
+            gr.set_batch(b)
+            outs = gr.run([x[:b]])
+            assert gr.layer_kernels()[e.layer] == e.kernel
+            for o, t in zip(outs, g.outputs):
+                assert o.shape[0] == b and np.array_equal(o, want[t][:b]), (name, b, int((o != want[t][:b]).sum()))
+    finally:
+        gr.close()
 
 
 def test_negative_control_without_the_uint8_correction():

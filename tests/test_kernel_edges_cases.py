@@ -13,7 +13,7 @@ NAMES = list(ke.ENTRIES)
 def _geometry(name):
     e = ke.ENTRIES[name]
     case = ke.build(name)
-    return e, case, ke.geometry(case.g, case.g.layers[e.layer])
+    return e, case, ke.geometry(case.g, case.g.layers[e.layer], no_tc=bool(e.flags & ke.abi.PRERUN_NO_TENSORCORE))
 
 
 @pytest.mark.parametrize("name", NAMES)
@@ -22,7 +22,7 @@ def test_entry_reaches_its_geometry(name):
     for k, v in e.edges.items():
         assert k in geo, f"{name}: the geometry has no {k!r}: {geo}"
         assert geo[k] == v, f"{name}: {k} = {geo[k]}, meant {v}; geometry {geo}"
-    if geo["kind"] in ("gemm", "igemm", "dw"):
+    if geo["kind"] in ke.KERNEL_NAME or geo["kind"] == "dw":
         assert ke.kernel_name(geo) == e.kernel, (name, geo)
     if e.fused:
         assert e.kernel == "fused_into_producer"
@@ -42,6 +42,25 @@ def test_par_all_boundary_sits_at_par_max():
     """ocp 2048 keeps every channel's epilogue constants resident, one more N tile of channels (2064) does not."""
     assert ke.gemm_geometry(2048, 0, m=16, k=64)["par_all"] == 1
     assert ke.gemm_geometry(2064, 0, m=16, k=64)["par_all"] == 0
+
+
+def test_window_limits_sit_where_shared_memory_ends():
+    """window_nhwc_fits: 32-byte pixels fit up to OCp 176 at stride 1 and 144 at stride 2; 16-byte pixels at stride 2 up to 224
+    (the gather kernel takes 240); a 7x7 NCHW window over 3 channels at OCp 256 fits at xoff 0, not at xoff 13."""
+    assert [ke.window_nhwc_fits(32, o, 1) for o in (176, 192)] == [True, False]
+    assert [ke.window_nhwc_fits(32, o, 2) for o in (144, 160)] == [True, False]
+    assert [ke.window_nhwc_fits(16, o, 2) for o in (224, 240)] == [True, False]
+    assert ke.window_nhwc_fits(16, 256, 1)
+    g = dict(n=1, c=3, cp=16, w=32, oh=8, ow=16, k=7, stride=2, ocp=256, nhwc=0)
+    assert ke.window_geometry(pw0=0, **g)["valid"] and not ke.window_geometry(pw0=3, **g)["valid"]
+
+
+def test_window_and_gather_entries_are_listed():
+    """The NCHW stems over 1 and 2 channels with a 7x7 kernel (k-steps 2 and 4 of the 5 a 147-byte row could fill) through both
+    kernels, and window entries of 3 or more images for the partial-batch test."""
+    ks = {(ke.ENTRIES[n].kernel, ke.layer_geometry(ke.build(n).g, ke.build(n).g.layers[0]).get("ks")) for n in ke.window_entries()}
+    assert {(k, s) for k in (ke.WI, ke.GA) for s in (2, 4)} <= ks
+    assert len(ke.window_batch_entries()) >= 4
 
 
 @pytest.mark.parametrize("name", [n for n in NAMES if ke.ENTRIES[n].ties])
