@@ -45,6 +45,10 @@ struct EpiParams
     uint32_t q_byte_add;      // lower clamp (as a byte) replicated x4; 0 for ReLU-type layers
 };
 
+// The epilogue a tensor-core kernel is instantiated with (its MODE): 0 fast, 1 fast with the bias fused into the FMA (int8
+// only), 2 exact.  u8: the layer is uint8.
+static inline int epi_mode(const EpiParams& e, bool u8) { return !e.fast_ok ? 2 : (!u8 && e.fuse_bias ? 1 : 0); }
+
 // C round(): half away from zero, exact for every float (CUDA's roundf is the exact, slow-path version).
 __device__ __forceinline__ float round_half_away(float x) { return roundf(x); }
 

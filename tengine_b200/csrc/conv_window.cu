@@ -29,18 +29,6 @@
 
 namespace tb200 {
 
-struct WindowArgs
-{
-    const uint8_t* w; // [OCp][ks*32]; NCHW: k = (c*KH + kh)*KW + kw ; NHWC: k = (kh*3 + kw)*CB + c ; zero padded
-    uint8_t* out;     // NHWC, OCp bytes per pixel
-    int n, c, h, w_in, oh, ow, ocp, oc, stride, ph, pw;
-    unsigned ntiles;
-    int tiles_w, tiles_h;
-    uint32_t tw_magic, th_magic; // floor(2^32 / d) + 1: q = umulhi(x, magic) is x / d for the tile counts that occur (checked by the launcher)
-    int box_w, box_h, xoff, in_bytes, ks;
-    uint32_t fill; // uint8: the input zero point replicated x4 (0 for int8: the TMA zero fill already is the padding)
-};
-
 // The B tiles (weights [OCp][ks*32] -> one SW32 K-major tile of OCp rows per k-step) and the epilogue constants into shared
 // memory: identical for every CTA, L2 resident.  Int8 MODE 2 reads no constants.
 template <int MODE, bool U8>
@@ -251,66 +239,63 @@ bool window_nhwc_fits(int cp, int ocp, int stride)
 }
 // nhwc == 0: `in` is the NCHW network input (C <= 3); the tensor map is (W, H, C, N) with box (box_w, box_h, C, 1).
 // nhwc == 1: `in` is an NHWC tensor with cp = 16 or 32 bytes per pixel; the map is (cp, W, H, N) with box (cp, box_w, box_h, 1).
-int window_plan_create(WindowPlan* p, const void* in, const ConvShape& s, int nhwc)
+int window_plan_create(WindowPlan* p, const void* in, const void* w, void* out, const ConvShape& s, const EpiParams& e, int nhwc, int num_sms)
 {
     memset(p, 0, sizeof *p);
-    if (s.group != 1 || s.dh != 1 || s.dw != 1 || s.sh != s.sw || s.sh < 1 || s.sh > 2 || s.kh != s.kw || s.ocp > 256) return -1;
+    WindowArgs& a = p->a;
+    if (s.group != 1 || s.dh != 1 || s.dw != 1 || s.sh != s.sw || s.sh < 1 || s.sh > 2 || s.kh != s.kw || s.ocp > 256) return 1;
     if (nhwc)
     {
-        if (s.kh != 3 || (s.cp != 16 && s.cp != 32)) return -1;
+        if (s.kh != 3 || (s.cp != 16 && s.cp != 32)) return 1;
         p->layout = s.cp == 16 ? 2 : 3;
-        p->xoff = 0;
-        p->box_w = 15 * s.sw + 3, p->box_h = 7 * s.sh + 3;
-        p->in_bytes = p->box_w * p->box_h * s.cp;
-        p->ks = (9 * s.cp + 31) / 32;
+        a.xoff = 0;
+        a.box_w = 15 * s.sw + 3, a.box_h = 7 * s.sh + 3;
+        a.in_bytes = a.box_w * a.box_h * s.cp;
+        a.ks = (9 * s.cp + 31) / 32;
         const uint64_t dims[4] = {(uint64_t)s.cp, (uint64_t)s.w, (uint64_t)s.h, (uint64_t)s.n};
         const uint64_t strides[3] = {(uint64_t)s.cp, (uint64_t)s.w * s.cp, (uint64_t)s.h * s.w * s.cp};
-        const uint32_t box[4] = {(uint32_t)s.cp, (uint32_t)p->box_w, (uint32_t)p->box_h, 1u};
-        if (tmap_encode(p->tmap_in, in, 4, dims, strides, box, nullptr, 0)) return -1;
+        const uint32_t box[4] = {(uint32_t)s.cp, (uint32_t)a.box_w, (uint32_t)a.box_h, 1u};
+        if (tmap_encode(&p->tmap_in, in, 4, dims, strides, box, nullptr, 0)) return 1;
     }
     else
     {
-        if ((s.kh != 3 && s.kh != 7) || s.c > 3 || (s.w % 16)) return -1; // global strides of a tensor map are multiples of 16 bytes
+        if ((s.kh != 3 && s.kh != 7) || s.c > 3 || (s.w % 16)) return 1; // global strides of a tensor map are multiples of 16 bytes
         p->layout = s.kh == 3 ? 0 : 1;
         // the innermost coordinate ow0*S - pw - xoff must be a multiple of 16 (ow0*S is one)
-        p->xoff = (16 - (s.pw0 % 16)) % 16;
-        p->box_w = (p->xoff + 15 * s.sw + s.kw + 15) & ~15, p->box_h = 7 * s.sh + s.kh;
-        if (p->box_w > 256 || p->box_h > 256) return -1;
-        p->in_bytes = p->box_w * p->box_h * s.c;
-        p->ks = (s.c * s.kh * s.kw + 31) / 32;
+        a.xoff = (16 - (s.pw0 % 16)) % 16;
+        a.box_w = (a.xoff + 15 * s.sw + s.kw + 15) & ~15, a.box_h = 7 * s.sh + s.kh;
+        if (a.box_w > 256 || a.box_h > 256) return 1;
+        a.in_bytes = a.box_w * a.box_h * s.c;
+        a.ks = (s.c * s.kh * s.kw + 31) / 32;
         const uint64_t dims[4] = {(uint64_t)s.w, (uint64_t)s.h, (uint64_t)s.c, (uint64_t)s.n};
         const uint64_t strides[3] = {(uint64_t)s.w, (uint64_t)s.w * s.h, (uint64_t)s.w * s.h * s.c};
-        const uint32_t box[4] = {(uint32_t)p->box_w, (uint32_t)p->box_h, (uint32_t)s.c, 1u};
-        if (tmap_encode(p->tmap_in, in, 4, dims, strides, box, nullptr, 0)) return -1;
+        const uint32_t box[4] = {(uint32_t)a.box_w, (uint32_t)a.box_h, (uint32_t)s.c, 1u};
+        if (tmap_encode(&p->tmap_in, in, 4, dims, strides, box, nullptr, 0)) return 1;
     }
-    p->smem_bytes = window_smem_bytes(p->ks, s.ocp, p->in_bytes);
-    if (p->smem_bytes > WINDOW_SMEM_MAX) return -1;
-    p->valid = 1;
-    return 0;
-}
-
-cudaError_t launch_conv_window(const WindowPlan& p, const void* w, void* out, const ConvShape& s, const EpiParams& e, int num_sms, cudaStream_t st)
-{
-    if (!p.valid) return cudaErrorInvalidValue;
-    if ((long long)s.n * s.oh * s.ow >= (1ll << 31)) return cudaErrorInvalidValue; // 32-bit pixel index
-    WindowArgs a;
+    p->smem_bytes = window_smem_bytes(a.ks, s.ocp, a.in_bytes);
+    if (p->smem_bytes > WINDOW_SMEM_MAX) return 1;
+    if ((long long)s.n * s.oh * s.ow >= (1ll << 31)) return TB200_ERR_UNSUPPORTED; // 32-bit pixel index
     a.w = (const uint8_t*)w, a.out = (uint8_t*)out;
     a.n = s.n, a.c = s.c, a.h = s.h, a.w_in = s.w, a.oh = s.oh, a.ow = s.ow, a.ocp = s.ocp, a.oc = s.oc, a.stride = s.sh, a.ph = s.ph0, a.pw = s.pw0;
     a.tiles_w = (s.ow + 15) / 16, a.tiles_h = (s.oh + 7) / 8;
     a.ntiles = (unsigned)((long long)a.tiles_w * a.tiles_h * s.n);
     // umulhi(x, floor(2^32/d) + 1) == x / d whenever x * d < 2^32 (error term x * (d - 2^32 mod d) / (d * 2^32) < 1 / d)
-    if ((unsigned long long)a.ntiles * (unsigned)a.tiles_w >= (1ull << 32) || (unsigned long long)a.ntiles * (unsigned)a.tiles_h >= (1ull << 32)) return cudaErrorInvalidValue;
+    if ((unsigned long long)a.ntiles * (unsigned)a.tiles_w >= (1ull << 32) || (unsigned long long)a.ntiles * (unsigned)a.tiles_h >= (1ull << 32)) return TB200_ERR_UNSUPPORTED;
     a.tw_magic = a.tiles_w == 1 ? 0u : (uint32_t)((1ull << 32) / (unsigned)a.tiles_w) + 1u;
     a.th_magic = a.tiles_h == 1 ? 0u : (uint32_t)((1ull << 32) / (unsigned)a.tiles_h) + 1u;
-    a.box_w = p.box_w, a.box_h = p.box_h, a.xoff = p.xoff, a.in_bytes = p.in_bytes, a.ks = p.ks;
     a.fill = e.is_uint8 ? ((uint32_t)(e.in_zero & 0xff) * 0x01010101u) : 0u;
-    const int mode = !e.fast_ok ? 2 : ((!e.is_uint8 && e.fuse_bias) ? 1 : 0);
-    CUtensorMap tm;
-    memcpy(&tm, p.tmap_in, sizeof tm);
+    p->e = e;
+    p->mode = epi_mode(e, e.is_uint8);
+    p->num_sms = num_sms;
+    return 0;
+}
+
+cudaError_t launch_conv_window(const WindowPlan& p, cudaStream_t st)
+{
     // Several resident CTAs per SM overlap gather / MMA / epilogue of different tiles; each loops over its share.  The grid is
     // exactly the CTAs that can be resident at once (registers and shared memory): a larger one leaves a tail of late CTAs.
 #define TB200_WIN_CASE(MD, U, LY)                                                                                                           \
-    if (mode == MD && (e.is_uint8 != 0) == U && p.layout == LY)                                                                             \
+    if (p.mode == MD && (p.e.is_uint8 != 0) == U && p.layout == LY)                                                                         \
     {                                                                                                                                       \
         /* the opt-in is per device AND per context: set it before every launch (launches happen at graph capture only) */ \
         cudaError_t err = cudaFuncSetAttribute(conv_window_tc_kernel<MD, U, LY>, cudaFuncAttributeMaxDynamicSharedMemorySize, WINDOW_SMEM_MAX); \
@@ -318,12 +303,12 @@ cudaError_t launch_conv_window(const WindowPlan& p, const void* w, void* out, co
         int per_sm = 0;                                                                                                                     \
         err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, conv_window_tc_kernel<MD, U, LY>, 128, (size_t)p.smem_bytes);          \
         if (err != cudaSuccess) return err;                                                                                                 \
-        const unsigned cap = (unsigned)num_sms * (unsigned)(per_sm > 1 ? per_sm : 1), grid = a.ntiles < cap ? a.ntiles : cap;             \
+        const unsigned cap = (unsigned)p.num_sms * (unsigned)(per_sm > 1 ? per_sm : 1), grid = p.a.ntiles < cap ? p.a.ntiles : cap;       \
         if (debug_launch())                                                                                                                 \
             fprintf(stderr, "tengine_b200: launch conv_window_tc_kernel<MODE=%d,U8=%d,LAYOUT=%d> layout=%d xoff=%d box_w=%d box_h=%d ks=%d "   \
-                            "smem=%d tiles_w=%d tiles_h=%d grid=%u\n", MD, (int)U, LY, p.layout, p.xoff, p.box_w, p.box_h, p.ks,              \
-                    p.smem_bytes, a.tiles_w, a.tiles_h, grid);                                                                              \
-        conv_window_tc_kernel<MD, U, LY><<<grid, 128, (size_t)p.smem_bytes, st>>>(tm, a, e);                                                \
+                            "smem=%d tiles_w=%d tiles_h=%d grid=%u\n", MD, (int)U, LY, p.layout, p.a.xoff, p.a.box_w, p.a.box_h, p.a.ks,      \
+                    p.smem_bytes, p.a.tiles_w, p.a.tiles_h, grid);                                                                          \
+        conv_window_tc_kernel<MD, U, LY><<<grid, 128, (size_t)p.smem_bytes, st>>>(p.tmap_in, p.a, p.e);                                     \
         return cudaGetLastError();                                                                                                          \
     }
 #define TB200_WIN_LAYOUTS(MD, U) TB200_WIN_CASE(MD, U, 0) TB200_WIN_CASE(MD, U, 1) TB200_WIN_CASE(MD, U, 2) TB200_WIN_CASE(MD, U, 3)
@@ -342,18 +327,6 @@ cudaError_t launch_conv_window(const WindowPlan& p, const void* w, void* out, co
 // (zx-zx)(w-zw) = 0, exactly like the reference, which skips them), padding K positions hold 0 in A and B, and the thread
 // sums its own row (dp4a) so that  sum (x-zx)(w-zw) = acc - zw*sum(x) + corr[oc]  needs no ones-row and no border table.
 // Takes the role of im2col + sgemm of conv_hcl_run for these shapes (conv_kernel_x86.c:187-242, 1008-1631).
-struct GatherArgs
-{
-    const uint8_t* in;
-    const uint8_t* w; // [OCp][ks*32]; NCHW: k = (c*3 + kh)*3 + kw ; NHWC16: k = (kh*3 + kw)*16 + c ; zero padded
-    uint8_t* out;
-    int n, c, h, w_in, oh, ow, ocp, oc, stride, ph, pw;
-    unsigned npix, ntiles;
-    int ks, nhwc16;
-    uint32_t fill; // byte for taps outside the image, replicated x4 (uint8: the input zero point; int8: 0)
-    uint32_t fill16[4]; // NHWC16: the same for a whole 16-channel tap; pad channels (c >= C) stay 0 like in the tensor itself
-};
-
 template <int MODE, bool U8, int KHW> // MODE: 0 fast, 1 fast + fused bias (int8), 2 exact; KHW: 3 or 7 (NCHW stems; NHWC16 is 3x3)
 __global__ void __launch_bounds__(128) conv_gather_tc_kernel(const GatherArgs a, const __grid_constant__ EpiParams e)
 {
@@ -459,10 +432,10 @@ __global__ void __launch_bounds__(128) conv_gather_tc_kernel(const GatherArgs a,
     }
 }
 
-cudaError_t launch_conv_gather_tc(const void* in, const void* w, void* out, const ConvShape& s, const EpiParams& e, int nhwc16, int num_sms, cudaStream_t st)
+void gather_plan_create(GatherPlan* p, const void* in, const void* w, void* out, const ConvShape& s, const EpiParams& e, int nhwc16, int num_sms)
 {
-    const int khw = nhwc16 ? 3 : s.kh;
-    GatherArgs a;
+    memset(p, 0, sizeof *p);
+    GatherArgs& a = p->a;
     a.in = (const uint8_t*)in, a.w = (const uint8_t*)w, a.out = (uint8_t*)out;
     a.n = s.n, a.c = s.c, a.h = s.h, a.w_in = s.w, a.oh = s.oh, a.ow = s.ow, a.ocp = s.ocp, a.oc = s.oc, a.stride = s.sh, a.ph = s.ph0, a.pw = s.pw0;
     a.npix = (unsigned)((long long)s.n * s.oh * s.ow);
@@ -470,27 +443,30 @@ cudaError_t launch_conv_gather_tc(const void* in, const void* w, void* out, cons
     a.ks = nhwc16 ? 5 : (s.c * s.kh * s.kw + 31) / 32, a.nhwc16 = nhwc16;
     a.fill = e.is_uint8 ? ((uint32_t)(e.in_zero & 0xff) * 0x01010101u) : 0u;
     for (int j = 0; j < 4; j++)
-    {
-        a.fill16[j] = 0;
         for (int t = 0; t < 4; t++)
             if (j * 4 + t < s.c) a.fill16[j] |= (a.fill & 0xffu) << (8 * t);
-    }
-    const size_t smem = (size_t)a.ks * 4096 + (size_t)a.ks * s.ocp * 32 + (size_t)s.ocp * 8 + 16 + 128 * (size_t)acc_pitch(s.ocp) + 1024;
+    p->e = e;
+    p->smem_bytes = a.ks * 4096 + a.ks * s.ocp * 32 + s.ocp * 8 + 16 + 128 * (int)acc_pitch(s.ocp) + 1024;
     const unsigned cap = (unsigned)num_sms * 6u;
-    const unsigned grid = a.ntiles < cap ? a.ntiles : cap;
-    const int mode = !e.fast_ok ? 2 : ((!e.is_uint8 && e.fuse_bias) ? 1 : 0);
+    p->grid = a.ntiles < cap ? a.ntiles : cap;
+    p->mode = epi_mode(e, e.is_uint8);
+    p->khw = nhwc16 ? 3 : s.kh;
+}
+
+cudaError_t launch_conv_gather_tc(const GatherPlan& p, cudaStream_t st)
+{
 #define TB200_GAT_CASE(MD, U, K)                                                                                                   \
-    if (mode == MD && (e.is_uint8 != 0) == U && khw == K)                                                                          \
+    if (p.mode == MD && (p.e.is_uint8 != 0) == U && p.khw == K)                                                                    \
     {                                                                                                                              \
         /* the opt-in is per device AND per context: set it before every launch (launches happen at graph capture only) */ \
         {                                                                                                                          \
-            cudaError_t err = cudaFuncSetAttribute(conv_gather_tc_kernel<MD, U, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
+            cudaError_t err = cudaFuncSetAttribute(conv_gather_tc_kernel<MD, U, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, p.smem_bytes); \
             if (err != cudaSuccess) return err;                                                                                    \
         }                                                                                                                          \
         if (debug_launch())                                                                                                        \
-            fprintf(stderr, "tengine_b200: launch conv_gather_tc_kernel<MODE=%d,U8=%d,KHW=%d> ks=%d ntiles=%u\n", MD, (int)U, K, a.ks, \
-                    a.ntiles);                                                                                                     \
-        conv_gather_tc_kernel<MD, U, K><<<grid, 128, smem, st>>>(a, e);                                                            \
+            fprintf(stderr, "tengine_b200: launch conv_gather_tc_kernel<MODE=%d,U8=%d,KHW=%d> ks=%d ntiles=%u\n", MD, (int)U, K, p.a.ks, \
+                    p.a.ntiles);                                                                                                   \
+        conv_gather_tc_kernel<MD, U, K><<<p.grid, 128, (size_t)p.smem_bytes, st>>>(p.a, p.e);                                      \
         return cudaGetLastError();                                                                                                 \
     }
     TB200_GAT_CASE(0, false, 3) TB200_GAT_CASE(1, false, 3) TB200_GAT_CASE(2, false, 3) TB200_GAT_CASE(0, true, 3) TB200_GAT_CASE(2, true, 3)

@@ -247,17 +247,16 @@ __global__ void __launch_bounds__(DW_THREADS, DW_MIN_CTAS)
 
 // Plan: tile geometry + the 4-D tensor map (C, W, H, N) of the input.  Returns 0, or <0 when this layer must use the
 // generic depthwise kernel (uint8, stride > 2, very wide rows ...).
-int dw_plan_create(DwPlan* p, const void* in, const ConvShape& s, const EpiParams& e)
+int dw_plan_create(DwPlan* p, const void* in, const void* w, void* out, const ConvShape& s, const EpiParams& e)
 {
-    p->valid = 0;
     if (e.is_uint8 || s.kh != 3 || s.kw != 3 || s.dh != 1 || s.dw != 1 || s.sh != s.sw || (s.sh != 1 && s.sh != 2)) return -1;
     const int S = s.sh;
-    p->tw = (S == 1) ? 8 : 4;
-    p->gpr = (s.ow + p->tw - 1) / p->tw;
+    const int tw = (S == 1) ? 8 : 4; // output pixels per thread
+    p->gpr = (s.ow + tw - 1) / tw;
     if (p->gpr > 16) return -1; // rows wider than 16 pixel groups: generic kernel
     p->rows_per_cta = 16 / p->gpr;
     if (p->rows_per_cta > s.oh) p->rows_per_cta = s.oh;
-    p->tile_cols = (p->gpr * p->tw - 1) * S + 3;
+    p->tile_cols = (p->gpr * tw - 1) * S + 3;
     p->tile_rows = (p->rows_per_cta - 1) * S + 3;
     if (p->tile_cols > 256 || p->tile_rows > 256) return -1;
     p->smem_bytes = p->tile_rows * p->tile_cols * DW_CH;
@@ -265,26 +264,24 @@ int dw_plan_create(DwPlan* p, const void* in, const ConvShape& s, const EpiParam
     const uint64_t dims[4] = {(uint64_t)s.cp, (uint64_t)s.w, (uint64_t)s.h, (uint64_t)s.n};
     const uint64_t strides[3] = {(uint64_t)s.cp, (uint64_t)s.w * s.cp, (uint64_t)s.h * s.w * s.cp};
     const uint32_t box[4] = {(uint32_t)DW_CH, (uint32_t)p->tile_cols, (uint32_t)p->tile_rows, 1u};
-    if (tmap_encode(p->tmap_in, in, 4, dims, strides, box, nullptr, 0) != 0) return -2;
-    p->valid = 1;
+    if (tmap_encode(&p->tmap_in, in, 4, dims, strides, box, nullptr, 0) != 0) return -2;
+    p->w = (const uint8_t*)w, p->out = (uint8_t*)out, p->s = s, p->e = e;
+    p->grid = dim3((s.cp + DW_CH - 1) / DW_CH, (s.oh + p->rows_per_cta - 1) / p->rows_per_cta, s.n);
+    p->mode = epi_mode(e, e.is_uint8);
     return 0;
 }
 
-cudaError_t launch_conv_dw_tma(const DwPlan& p, const void* w, void* out, const ConvShape& s, const EpiParams& e, cudaStream_t st)
+cudaError_t launch_conv_dw_tma(const DwPlan& p, cudaStream_t st)
 {
-    dim3 grid((s.cp + DW_CH - 1) / DW_CH, (s.oh + p.rows_per_cta - 1) / p.rows_per_cta, s.n);
-    CUtensorMap tm;
-    memcpy(&tm, p.tmap_in, sizeof tm);
-    // not templated on the epilogue: MODE is the run-time choice of the same rule as the other launchers (2 = exact)
+    // not templated on the epilogue: MODE is the kernels' run-time choice, by the rule that instantiates the others (2 = exact)
     if (debug_launch())
-        fprintf(stderr, "tengine_b200: launch %s MODE=%d\n", s.sh == 1 ? "conv_dw3x3_tma_pack3_kernel" : "conv_dw3x3_tma_kernel<4,2>",
-                !e.fast_ok ? 2 : (!e.is_uint8 && e.fuse_bias ? 1 : 0));
-    if (s.sh == 1)
-        conv_dw3x3_tma_pack3_kernel<<<grid, DW_THREADS, p.smem_bytes, st>>>(tm, (const uint8_t*)w, (uint8_t*)out, s, e, p.rows_per_cta, p.gpr,
-                                                                           p.tile_cols, p.tile_rows);
+        fprintf(stderr, "tengine_b200: launch %s MODE=%d\n", p.s.sh == 1 ? "conv_dw3x3_tma_pack3_kernel" : "conv_dw3x3_tma_kernel<4,2>", p.mode);
+    if (p.s.sh == 1)
+        conv_dw3x3_tma_pack3_kernel<<<p.grid, DW_THREADS, p.smem_bytes, st>>>(p.tmap_in, p.w, p.out, p.s, p.e, p.rows_per_cta, p.gpr, p.tile_cols,
+                                                                             p.tile_rows);
     else
-        conv_dw3x3_tma_kernel<4, 2><<<grid, DW_THREADS, p.smem_bytes, st>>>(tm, (const uint8_t*)w, (uint8_t*)out, s, e, p.rows_per_cta, p.gpr,
-                                                                            p.tile_cols, p.tile_rows);
+        conv_dw3x3_tma_kernel<4, 2><<<p.grid, DW_THREADS, p.smem_bytes, st>>>(p.tmap_in, p.w, p.out, p.s, p.e, p.rows_per_cta, p.gpr, p.tile_cols,
+                                                                              p.tile_rows);
     return cudaGetLastError();
 }
 

@@ -118,10 +118,6 @@ static_assert(sizeof kStepName / sizeof kStepName[0] == K_NUM_KINDS, "one name p
 // The arguments of each step kind's launch
 struct LayoutArgs { const void* in; void* out; int n, c, h, w; }; // K_NCHW2NHWC, K_NHWC2NCHW
 struct ConvArgs { const void* in; const void* w; void* out; ConvShape cs; EpiParams epi; }; // K_CONV_STEM, K_CONV_DW, K_CONV_DIRECT
-struct GatherArgs { ConvArgs conv; int nhwc16; }; // nhwc16: the input is a 16-channel NHWC tensor (else the NCHW network input)
-struct WindowArgs { ConvArgs conv; WindowPlan wp; };
-struct DwTmaArgs { ConvArgs conv; DwPlan dwp; };
-struct GemmArgs { GemmPlan gemm; EpiParams epi; const int32_t* btab; }; // K_GEMM, K_IGEMM; btab: uint8 padding-tap corrections
 struct PoolArgs { const void* in; void* out; PoolShape ps; bool u8; };
 struct PointwiseArgs { const void* in; const void* in2; void* out; long long bytes; PointwiseParams pp; bool u8; }; // in2: eltwise operand
 struct ConcatArgs { const void* in; void* out; ConcatPart part; bool u8; }; // K_CONCAT_PART, K_CONCAT_LUT: one input of the concat
@@ -135,7 +131,8 @@ struct Step
 {
     int kind;
     int layer; // -1 for layout steps
-    std::variant<LayoutArgs, ConvArgs, GatherArgs, WindowArgs, DwTmaArgs, GemmArgs, PoolArgs, PointwiseArgs, ConcatArgs, ByteLutArgs, SoftmaxArgs,
+    // K_GATHER_TC, K_CONV_WINDOW, K_CONV_DW_TMA, K_GEMM and K_IGEMM: the plan their kernel is launched with
+    std::variant<LayoutArgs, ConvArgs, GatherPlan, WindowPlan, DwPlan, GemmPlan, PoolArgs, PointwiseArgs, ConcatArgs, ByteLutArgs, SoftmaxArgs,
                  ReshapeArgs, UpsampleArgs, CopyArgs>
         args;
 };
@@ -471,7 +468,6 @@ template <class A> static const A& args(const Step& s)
 
 static int run_step(const Shard* g, const Step& s, cudaStream_t st)
 {
-    const int sms = g->gpu->num_sms;
     cudaError_t err = cudaSuccess;
     switch (s.kind)
     {
@@ -480,11 +476,11 @@ static int run_step(const Shard* g, const Step& s, cudaStream_t st)
     case K_CONV_STEM: { auto& a = args<ConvArgs>(s); err = launch_conv_stem(a.in, a.w, a.out, a.cs, a.epi, st); break; }
     case K_CONV_DW: { auto& a = args<ConvArgs>(s); err = launch_conv_dw(a.in, a.w, a.out, a.cs, a.epi, st); break; }
     case K_CONV_DIRECT: { auto& a = args<ConvArgs>(s); err = launch_conv_direct(a.in, a.w, a.out, a.cs, a.epi, st); break; }
-    case K_GATHER_TC: { auto& a = args<GatherArgs>(s); err = launch_conv_gather_tc(a.conv.in, a.conv.w, a.conv.out, a.conv.cs, a.conv.epi, a.nhwc16, sms, st); break; }
-    case K_CONV_WINDOW: { auto& a = args<WindowArgs>(s); err = launch_conv_window(a.wp, a.conv.w, a.conv.out, a.conv.cs, a.conv.epi, sms, st); break; }
-    case K_CONV_DW_TMA: { auto& a = args<DwTmaArgs>(s); err = launch_conv_dw_tma(a.dwp, a.conv.w, a.conv.out, a.conv.cs, a.conv.epi, st); break; }
+    case K_GATHER_TC: err = launch_conv_gather_tc(args<GatherPlan>(s), st); break;
+    case K_CONV_WINDOW: err = launch_conv_window(args<WindowPlan>(s), st); break;
+    case K_CONV_DW_TMA: err = launch_conv_dw_tma(args<DwPlan>(s), st); break;
     case K_GEMM:
-    case K_IGEMM: { auto& a = args<GemmArgs>(s); err = launch_gemm_i8(a.gemm, a.epi, a.btab, sms, st); break; }
+    case K_IGEMM: err = launch_gemm_i8(args<GemmPlan>(s), st); break;
     case K_POOL: { auto& a = args<PoolArgs>(s); err = launch_pool(a.in, a.out, a.ps, a.u8, st); break; }
     case K_POINTWISE: { auto& a = args<PointwiseArgs>(s); err = launch_pointwise(a.in, a.in2, a.out, a.bytes, a.pp, a.u8, st); break; }
     case K_CONCAT_PART: { auto& a = args<ConcatArgs>(s); err = launch_concat_part(a.in, a.out, a.part, a.u8, st); break; }
@@ -1430,31 +1426,33 @@ static int fill_conv_step(Shard* g, int li, const LayerPlan& P, const Slice& sl,
         work->work_wbytes += (double)OC * k + (L.bias ? 4.0 * OC : 0);
     }
     if (P.reads_nchw) c.in = g->in_nchw_dev[tin.input_index] + sl.off(tin.nchw_bytes);
+    const int sms = g->gpu->num_sms;
     if (P.kind == K_GATHER_TC)
     {
-        WindowArgs a{c, {}};
-        window_plan_create(&a.wp, c.in, c.cs, P.nhwc16); // falls back to the global-memory gather (16 channels / NCHW only)
-        if (a.wp.valid) s.kind = K_CONV_WINDOW, s.args = a;
+        // falls back to the global-memory gather (16 channels / NCHW only)
+        const int rc = window_plan_create(&s.args.emplace<WindowPlan>(), c.in, c.w, c.out, c.cs, c.epi, P.nhwc16, sms);
+        if (rc < 0) return fail(rc, "layer %d: window plan failed: more output pixels or tiles than 32-bit indices address", li);
+        if (rc == 0) s.kind = K_CONV_WINDOW;
         else if (P.nhwc16 && tin.cp != 16) return fail(TB200_ERR_UNSUPPORTED, "layer %d: window plan failed for a 32-channel 3x3 convolution", li);
-        else s.args = GatherArgs{c, P.nhwc16};
+        else gather_plan_create(&s.args.emplace<GatherPlan>(), c.in, c.w, c.out, c.cs, c.epi, P.nhwc16, sms);
     }
     else if (P.kind == K_CONV_DW)
     {
-        DwTmaArgs a{c, {}};
-        if (!(g->flags & TB200_PRERUN_NO_TENSORCORE)) dw_plan_create(&a.dwp, c.in, c.cs, c.epi); // falls back when not applicable
-        if (a.dwp.valid) s.kind = K_CONV_DW_TMA, s.args = a;
+        DwPlan d;
+        // falls back when not applicable
+        if (!(g->flags & TB200_PRERUN_NO_TENSORCORE) && dw_plan_create(&d, c.in, c.w, c.out, c.cs, c.epi) == 0) s.kind = K_CONV_DW_TMA, s.args = d;
         else s.args = c;
     }
     else if (P.kind == K_GEMM || P.kind == K_IGEMM)
     {
-        GemmArgs& a = s.args.emplace<GemmArgs>(GemmArgs{{}, c.epi, (const int32_t*)(g->w_arena + P.blob.btab_off)});
+        GemmPlan& gp = s.args.emplace<GemmPlan>();
+        const int32_t* btab = (const int32_t*)(g->w_arena + P.blob.btab_off);
         const long long m = fc ? N : (long long)N * H * W;
         const int kdim = fc ? H * W * tin.cp : tin.cp;
-        int rc = P.kind == K_IGEMM ? gemm_plan_create_conv(&a.gemm, c.in, c.w, c.out, c.cs, P.gemm_zp)
-                                   : gemm_plan_create(&a.gemm, c.in, kdim, c.w, c.out, m, kdim, OC, tout.cp, tout.cp, P.gemm_zp);
+        int rc = P.kind == K_IGEMM ? gemm_plan_create_conv(&gp, c.in, c.w, c.out, c.cs, P.gemm_zp, c.epi, btab, g->gpu->fixq, FIXQ_CAP, sms)
+                                   : gemm_plan_create(&gp, c.in, kdim, c.w, c.out, m, kdim, OC, tout.cp, tout.cp, P.gemm_zp, c.epi, btab, g->gpu->fixq, FIXQ_CAP, sms);
         if (rc && P.kind == K_IGEMM) return fail(rc, "layer %d: implicit-GEMM plan failed", li);
         if (rc) return fail(rc, "layer %d: TMA descriptor creation failed (m=%lld k=%d oc=%d)", li, m, kdim, OC);
-        a.gemm.fixq = g->gpu->fixq, a.gemm.fixq_cap = FIXQ_CAP;
     }
     else s.args = c;
     return 0;
@@ -2581,11 +2579,10 @@ int tb200k_gemm_i8(const void* in, const void* weight, void* out, int64_t m, int
     int dev = 0, sms = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
         return fail(TB200_ERR_NO_DEVICE, "no CUDA device");
-    GemmPlan plan;
-    int rc = gemm_plan_create(&plan, in, k_pad, weight, out, m, k_pad, oc, cpad(oc), cpad(oc), 0);
+    GemmPlan plan; // the exact epilogue of epi_from_abi, no fix-up queue, no border table
+    int rc = gemm_plan_create(&plan, in, k_pad, weight, out, m, k_pad, oc, cpad(oc), cpad(oc), 0, epi_from_abi(e), nullptr, nullptr, 0, sms);
     if (rc) return fail(rc, "gemm plan failed");
-    EpiParams p = epi_from_abi(e);
-    K_LAUNCH(launch_gemm_i8(plan, p, nullptr, sms, (cudaStream_t)stream));
+    K_LAUNCH(launch_gemm_i8(plan, (cudaStream_t)stream));
 }
 size_t tb200k_conv_winograd43_f32_workspace(const tb200k_conv_shape* s) { return s ? wino43_workspace_bytes(s->n, s->c, s->oc, s->oh, s->ow) : 0; }
 int tb200k_conv_winograd43_f32(const float* in, const float* weight, const float* bias, float* out, const tb200k_conv_shape* s, int activation, void* workspace,

@@ -79,38 +79,6 @@ static void gemm_launch_debug(const void* fn, const char* what, cudaError_t err,
     cudaGetLastError();
 }
 
-struct GemmArgs
-{
-    int m_tiles, num_super; // 32-bit on purpose: 64-bit divisions in the tile decode cost ~100 instructions each
-    int k_blocks, n_tiles, block_n, block_k, stages, swizzle;
-    int mt;     // m-tiles (128 rows each) per accumulator stage
-    uint32_t bw_rcp, bh_rcp; // ceil(65536/d): q = (x * rcp) >> 16 is exact for x < 4096, d <= 256
-    int oc, ocp;
-    // conv mode (implicit GEMM): an m-tile is a bw x bh x bn patch of output pixels, a k-block is (tap, channel block)
-    int conv, cblocks, kw_n, pad_h, pad_w, cstride, cp;
-    int bw, bh, bn, tiles_w, tiles_h, oh, ow, nimg;
-    uint32_t a_tx_bytes; // bytes one A load delivers (block_k * rows of the patch)
-    // uint8 (unsigned A): B holds w - 128 as int8 (plain w when zw == 0), so the accumulator is sum x*(w - 128); what is left of
-    // sum x*(w - zw) is cplane * sum(x) with cplane = 128 - zw, and the epilogue adds cplane * sum(x) inside the IADD3 that also
-    // adds the per-channel constant.
-    // sum(x) comes from two extra warps that add up the rows of every A tile in shared memory (cplane != 0 only).
-    int u8, taps, in_h, in_w, b_signed, cplane;
-    // epilogue / stores
-    int cs, ngroups; // 16-column chunks per store group (1 or 2) and groups per m-tile
-    int rows_valid;  // rows of an m-tile that are output pixels (128, or bw*bh*bn of a smaller conv patch)
-    int out_mode;    // coordinates of the output map: 0 (c, row, 0)  1 (c, pixel in image, image)  2 (c, x, image row)
-    int par_all;     // the constants of every channel are resident (loaded once); else reloaded per N tile
-    int b_res;       // the N tile's weights (all k-blocks) are loaded once and stay in smem; the ring carries A only
-    // deferred rare path: a guarded element is queued {m-tile, row, channel, accumulator} and recomputed literally by all threads of the
-    // CTA after its last tile, instead of holding up its epilogue warp (and with it the accumulator stage); null = inline
-    uint4* fixq;
-    int fixq_cap; // entries per CTA
-    uint8_t* out_base;
-    int ldo, m_rows; // output row pitch in bytes; rows of the flat GEMM
-    const int32_t* btab; // uint8 convolutions: [border pattern][OCp] summed corrections of the taps a border pixel misses (engine.cu)
-    unsigned long long* trace; // debug (TB200_GEMM_TRACE): event timeline of CTA 0, see gemm_trace_report
-};
-
 // m-tile -> first output pixel coordinates (conv mode)
 __device__ __forceinline__ void tile_origin(const GemmArgs& g, int mt, int& n0, int& oh0, int& ow0)
 {
@@ -957,161 +925,183 @@ int gemm_block_n(int ocp)
 // anyway (a single N tile): that amortises the per-stage synchronisation over up to ACC_COLS_MAX image columns of work.  A
 // store group is 32 rows x 16*cs channels; cs is 2 when that divides the N tile's chunk count and deals the stage's groups
 // evenly to the four warps of a 32-row image quarter, else 1.
-static void plan_stage(GemmPlan* p)
+static void plan_stage(GemmArgs& g, long long m_tiles)
 {
-    p->mt = 1;
-    if (p->n_tiles == 1)
-        while (p->mt < 4 && (p->mt * 2) * p->block_n <= ACC_COLS_MAX && p->mt * 2 <= p->m_tiles) p->mt *= 2;
-    const int nch = p->block_n / 16;
-    p->cs = (nch % 2 == 0 && (p->mt * (nch / 2)) % 4 == 0) ? 2 : 1;
-    p->ngroups = nch / p->cs;
+    g.mt = 1;
+    if (g.n_tiles == 1)
+        while (g.mt < 4 && (g.mt * 2) * g.block_n <= ACC_COLS_MAX && g.mt * 2 <= m_tiles) g.mt *= 2;
+    const int nch = g.block_n / 16;
+    g.cs = (nch % 2 == 0 && (g.mt * (nch / 2)) % 4 == 0) ? 2 : 1;
+    g.ngroups = nch / g.cs;
 }
 
 // Output tensor maps: a box of 32 rows x one store group; 32-byte groups are swizzled like the warp's staging buffer.
 static int plan_epilogue(GemmPlan* p, const void* out, uint64_t d1, uint64_t d2)
 {
-    const int cs = p->cs;
-    const uint64_t dims[3] = {(uint64_t)p->ocp, d1, d2};
-    const uint64_t strides[2] = {(uint64_t)p->ldo, (uint64_t)p->ldo * d1};
+    const int cs = p->g.cs;
+    const uint64_t dims[3] = {(uint64_t)p->g.ocp, d1, d2};
+    const uint64_t strides[2] = {(uint64_t)p->g.ldo, (uint64_t)p->g.ldo * d1};
     const int swz = cs == 2 ? 32 : 0;
     const uint32_t box[3] = {(uint32_t)(16 * cs), 32u, 1u};
-    int rc = tmap_encode(p->tmap_out, out, 3, dims, strides, box, nullptr, swz);
+    int rc = tmap_encode(&p->tmap_out, out, 3, dims, strides, box, nullptr, swz);
     if (rc) return rc;
-    const int tail = p->rows_valid % 32;
+    const int tail = p->g.rows_valid % 32;
     const uint32_t box_t[3] = {(uint32_t)(16 * cs), (uint32_t)(tail ? tail : 32), 1u};
-    return tmap_encode(p->tmap_out_tail, out, 3, dims, strides, box_t, nullptr, swz);
+    return tmap_encode(&p->tmap_out_tail, out, 3, dims, strides, box_t, nullptr, swz);
 }
 
-// shared memory the epilogue needs next to the operand ring
-static int epilogue_smem_bytes(const GemmPlan* p)
+// shared memory the epilogue needs next to the operand ring, with `warps` output staging warps: their double-buffered store
+// groups, the control block, the epilogue constants and the accumulator image
+static int epilogue_smem_bytes(const GemmArgs& g, int warps)
 {
-    const int par_ch = p->n_tiles * p->block_n;
-    return PLAN_STG_WARPS * 2 * 512 * p->cs + (par_ch <= PAR_MAX ? par_ch : p->block_n) * 8 + (int)sizeof(GemmSmemCtl) + 2048 +
-           128 * (int)acc_pitch(p->mt * p->block_n) + 16;
+    return warps * 2 * 512 * g.cs + (int)sizeof(GemmSmemCtl) + (g.par_all ? g.n_tiles * g.block_n : g.block_n) * 8 + 16 +
+           128 * (int)acc_pitch(g.mt * g.block_n);
 }
 
 // Operand ring depth and the resident-B decision.  With the N tile's weights resident the ring carries A tiles only,
 // which for the small-K layers (K = 32..128, one 4-16 KB A tile per m-tile) is the difference between 8 and 24 m-tiles
-// of prefetch distance.
-static int plan_ring(GemmPlan* p)
+// of prefetch distance.  Then the launch: one persistent CTA per SM at most, and the dynamic shared memory.
+static int plan_ring(GemmPlan* p, long long m_tiles, int num_sms)
 {
-    const int a_bytes = BLOCK_M * p->block_k, b_al = (p->block_n * p->block_k + 1023) & ~1023;
-    const int budget = 224 * 1024 - epilogue_smem_bytes(p) - (p->cplane ? 4096 : 0);
-    p->b_res = (long long)p->k_blocks * b_al <= B_RESIDENT_MAX ? 1 : 0;
-    int stages = p->b_res ? (budget - p->k_blocks * b_al) / a_bytes : budget / (a_bytes + b_al);
-    if (p->b_res && stages < 3) p->b_res = 0, stages = budget / (a_bytes + b_al);
+    GemmArgs& g = p->g;
+    g.m_tiles = (int)m_tiles;
+    plan_stage(g, m_tiles);
+    g.par_all = g.n_tiles * g.block_n <= PAR_MAX ? 1 : 0;
+    const int a_bytes = BLOCK_M * g.block_k, b_al = (g.block_n * g.block_k + 1023) & ~1023, sx_bytes = g.cplane ? 4096 : 0;
+    const int budget = 224 * 1024 - epilogue_smem_bytes(g, PLAN_STG_WARPS) - 2048 - sx_bytes;
+    g.b_res = (long long)g.k_blocks * b_al <= B_RESIDENT_MAX ? 1 : 0;
+    int stages = g.b_res ? (budget - g.k_blocks * b_al) / a_bytes : budget / (a_bytes + b_al);
+    if (g.b_res && stages < 3) g.b_res = 0, stages = budget / (a_bytes + b_al);
     if (stages > MAX_STAGES) stages = MAX_STAGES;
     if (stages < 2) return TB200_ERR_INVALID;
-    p->stages = stages;
+    g.stages = stages;
+    // + 1024: the kernel aligns the ring to 1024 bytes
+    p->smem_bytes = stages * (a_bytes + (g.b_res ? 0 : b_al)) + (g.b_res ? g.k_blocks * b_al : 0) + sx_bytes + epilogue_smem_bytes(g, EPI_WARPS) + 1024;
+    g.num_super = (int)(((m_tiles + g.mt - 1) / g.mt) * g.n_tiles);
+    p->grid = g.num_super < num_sms ? g.num_super : num_sms;
+    if (g.b_res) p->grid -= p->grid % g.n_tiles; // a CTA must see one N tile only (num_super is a multiple of n_tiles, so grid >= n_tiles)
     return 0;
 }
 
-int gemm_plan_create(GemmPlan* p, const void* a, long long lda, const void* b, void* out, long long m, int k, int oc, int ocp, int ldo, int u8)
+// What both planners set first: the output, the epilogue, the N tiles and the operands.  u8 = 1 + weight zero point for uint8
+// layers: A is unsigned, and unless zw == 0 B holds w - 128 and the epilogue adds cplane * sum(x).
+static void plan_begin(GemmPlan* p, void* out, int oc, int ocp, int ldo, int u8, const EpiParams& e, const int32_t* btab, void* fixq, int fixq_cap)
+{
+    memset(p, 0, sizeof *p);
+    GemmArgs& g = p->g;
+    g.oc = oc, g.ocp = ocp, g.ldo = ldo, g.out_base = (uint8_t*)out;
+    g.block_n = gemm_block_n(ocp);
+    g.n_tiles = (ocp + g.block_n - 1) / g.block_n;
+    g.u8 = u8 != 0;
+    g.b_signed = !g.u8 || u8 != 1;
+    g.cplane = (g.u8 && u8 != 1 && !getenv("TB200_DEBUG_NO_CPLANE")) ? 128 - (u8 - 1) : 0; // (debug switch: WRONG results, timing experiments only)
+    g.btab = btab, g.fixq = (uint4*)fixq, g.fixq_cap = fixq_cap;
+    p->e = e;
+    p->mode = epi_mode(e, g.u8);
+}
+
+int gemm_plan_create(GemmPlan* p, const void* a, long long lda, const void* b, void* out, long long m, int k, int oc, int ocp, int ldo, int u8,
+                     const EpiParams& e, const int32_t* btab, void* fixq, int fixq_cap, int num_sms)
 {
     if (m <= 0 || k <= 0 || (k & 15) || (ocp & 15) || (lda & 15) || (ldo & 15)) return TB200_ERR_INVALID;
-    memset(p, 0, sizeof *p);
-    p->m = m, p->k = k, p->oc = oc, p->ocp = ocp, p->ldo = ldo, p->out = out;
-    p->block_k = k <= 32 ? 32 : (k <= 64 ? 64 : 128);
-    p->swizzle = p->block_k;
-    p->k_blocks = (k + p->block_k - 1) / p->block_k;
-    p->u8 = u8 != 0; // u8 = 1 + weight zero point for uint8 layers
-    p->b_signed = !p->u8 || u8 != 1;
-    p->cplane = (p->u8 && u8 != 1 && !getenv("TB200_DEBUG_NO_CPLANE")) ? 128 - (u8 - 1) : 0; // (debug switch: WRONG results, timing experiments only)
-    p->block_n = gemm_block_n(ocp);
-    p->taps = 1;
-    p->n_tiles = (ocp + p->block_n - 1) / p->block_n;
-    p->m_tiles = (m + BLOCK_M - 1) / BLOCK_M;
-    plan_stage(p);
-    int rc = plan_ring(p);
+    plan_begin(p, out, oc, ocp, ldo, u8, e, btab, fixq, fixq_cap);
+    GemmArgs& g = p->g;
+    g.m_rows = (int)m;
+    g.block_k = k <= 32 ? 32 : (k <= 64 ? 64 : 128);
+    g.swizzle = g.block_k;
+    g.k_blocks = (k + g.block_k - 1) / g.block_k;
+    g.taps = 1;
+    int rc = plan_ring(p, (m + BLOCK_M - 1) / BLOCK_M, num_sms);
     if (rc) return rc;
-    rc = encode_2d(p->tmap_a, a, (uint64_t)k, (uint64_t)m, (uint64_t)lda, p->block_k, BLOCK_M, p->swizzle);
+    rc = encode_2d(&p->tmap_a, a, (uint64_t)k, (uint64_t)m, (uint64_t)lda, g.block_k, BLOCK_M, g.swizzle);
     if (rc) return rc;
-    rc = encode_2d(p->tmap_b, b, (uint64_t)k, (uint64_t)p->n_tiles * p->block_n, (uint64_t)k, p->block_k, p->block_n, p->swizzle);
+    rc = encode_2d(&p->tmap_b, b, (uint64_t)k, (uint64_t)g.n_tiles * g.block_n, (uint64_t)k, g.block_k, g.block_n, g.swizzle);
     if (rc) return rc;
-    p->rows_valid = BLOCK_M, p->out_mode = 0;
+    g.rows_valid = BLOCK_M, g.out_mode = 0;
     return plan_epilogue(p, out, (uint64_t)m, 1);
 }
 
 // Implicit-GEMM plan for a dense (group 1, dilation 1) convolution with any kernel size and stride 1 or 2:
 // A = 4-D tensor map (C, W, H, N) over the NHWC input with traversal strides (1, s, s, 1); B = [OCp][taps*Cp].
-int gemm_plan_create_conv(GemmPlan* p, const void* in, const void* w, void* out, const ConvShape& s, int u8)
+int gemm_plan_create_conv(GemmPlan* p, const void* in, const void* w, void* out, const ConvShape& s, int u8, const EpiParams& e,
+                          const int32_t* btab, void* fixq, int fixq_cap, int num_sms)
 {
     if (s.group != 1 || s.dh != 1 || s.dw != 1 || s.sh != s.sw || (s.sh != 1 && s.sh != 2)) return TB200_ERR_UNSUPPORTED;
     const int taps = s.kh * s.kw;
     if (taps > 1 && (s.cp % 32)) return TB200_ERR_UNSUPPORTED; // a k-block must not straddle two taps
-    memset(p, 0, sizeof *p);
-    p->conv = 1;
-    p->m = (long long)s.n * s.oh * s.ow, p->oc = s.oc, p->ocp = s.ocp, p->ldo = s.ocp, p->out = out;
-    if (taps == 1) p->block_k = s.cp <= 32 ? 32 : (s.cp <= 64 ? 64 : 128);
-    else p->block_k = (s.cp % 128 == 0) ? 128 : ((s.cp % 64 == 0) ? 64 : 32);
-    p->swizzle = p->block_k;
-    p->cblocks = (s.cp + p->block_k - 1) / p->block_k;
-    p->k_blocks = taps * p->cblocks;
-    p->k = taps * s.cp;
-    p->u8 = u8 != 0; // u8 = 1 + weight zero point for uint8 layers
-    p->b_signed = !p->u8 || u8 != 1;
-    p->cplane = (p->u8 && u8 != 1 && !getenv("TB200_DEBUG_NO_CPLANE")) ? 128 - (u8 - 1) : 0; // (debug switch: WRONG results, timing experiments only)
-    p->block_n = gemm_block_n(s.ocp);
-    p->taps = taps, p->in_h = s.h, p->in_w = s.w;
     if (taps > 64) return TB200_ERR_UNSUPPORTED;
-    p->n_tiles = (s.ocp + p->block_n - 1) / p->block_n;
+    plan_begin(p, out, s.oc, s.ocp, s.ocp, u8, e, btab, fixq, fixq_cap);
+    GemmArgs& g = p->g;
+    g.conv = 1;
+    g.m_rows = (int)((long long)s.n * s.oh * s.ow);
+    if (taps == 1) g.block_k = s.cp <= 32 ? 32 : (s.cp <= 64 ? 64 : 128);
+    else g.block_k = (s.cp % 128 == 0) ? 128 : ((s.cp % 64 == 0) ? 64 : 32);
+    g.swizzle = g.block_k;
+    g.cblocks = (s.cp + g.block_k - 1) / g.block_k;
+    g.k_blocks = taps * g.cblocks;
+    const int k = taps * s.cp;
+    g.taps = taps, g.in_h = s.h, g.in_w = s.w;
     // output patch of one m-tile: whole rows when they fit (then the patch is contiguous in the NHWC output)
     if (s.ow <= BLOCK_M)
     {
-        p->bw = s.ow;
-        p->bh = BLOCK_M / s.ow < s.oh ? BLOCK_M / s.ow : s.oh;
-        p->bn = (p->bh == s.oh) ? BLOCK_M / (s.ow * s.oh) : 1;
-        if (p->bn > s.n) p->bn = s.n;
-        if (p->bn < 1) p->bn = 1;
+        g.bw = s.ow;
+        g.bh = BLOCK_M / s.ow < s.oh ? BLOCK_M / s.ow : s.oh;
+        g.bn = (g.bh == s.oh) ? BLOCK_M / (s.ow * s.oh) : 1;
+        if (g.bn > s.n) g.bn = s.n;
+        if (g.bn < 1) g.bn = 1;
     }
     else
-        p->bw = BLOCK_M, p->bh = 1, p->bn = 1;
-    p->tiles_w = (s.ow + p->bw - 1) / p->bw;
-    p->tiles_h = (s.oh + p->bh - 1) / p->bh;
-    const long long tiles_n = (s.n + p->bn - 1) / p->bn;
-    p->m_tiles = (long long)p->tiles_w * p->tiles_h * tiles_n;
-    p->kw_n = s.kw, p->pad_h = s.ph0, p->pad_w = s.pw0, p->cstride = s.sh, p->cp = s.cp, p->oh = s.oh, p->ow = s.ow, p->nimg = s.n;
-    p->a_tx_bytes = (uint32_t)(p->block_k * p->bw * p->bh * p->bn);
-    plan_stage(p);
-    int rc = plan_ring(p);
+        g.bw = BLOCK_M, g.bh = 1, g.bn = 1;
+    g.bw_rcp = (65536u + (uint32_t)g.bw - 1) / (uint32_t)g.bw;
+    g.bh_rcp = (65536u + (uint32_t)g.bh - 1) / (uint32_t)g.bh;
+    g.tiles_w = (s.ow + g.bw - 1) / g.bw;
+    g.tiles_h = (s.oh + g.bh - 1) / g.bh;
+    const long long tiles_n = (s.n + g.bn - 1) / g.bn;
+    g.kw_n = s.kw, g.pad_h = s.ph0, g.pad_w = s.pw0, g.cstride = s.sh, g.cp = s.cp, g.oh = s.oh, g.ow = s.ow, g.nimg = s.n;
+    g.a_tx_bytes = (uint32_t)(g.block_k * g.bw * g.bh * g.bn);
+    // uint8 border corrections only exist for convolutions with taps that can fall into the padding: any window larger than one
+    // pixel, or a 1x1 window whose last row / column lies past the image (bottom / right padding, e.g. TF-style (0, 1))
+    const bool pad_1x1 = s.ph0 || s.pw0 || (s.oh - 1) * s.sh >= s.h || (s.ow - 1) * s.sh >= s.w;
+    p->border = g.u8 && (taps > 1 || pad_1x1);
+    int rc = plan_ring(p, (long long)g.tiles_w * g.tiles_h * tiles_n, num_sms);
     if (rc) return rc;
     const uint64_t dims[4] = {(uint64_t)s.cp, (uint64_t)s.w, (uint64_t)s.h, (uint64_t)s.n};
     const uint64_t strides[3] = {(uint64_t)s.cp, (uint64_t)s.w * s.cp, (uint64_t)s.h * s.w * s.cp};
-    const uint32_t box[4] = {(uint32_t)p->block_k, (uint32_t)((p->bw - 1) * s.sw + 1), (uint32_t)((p->bh - 1) * s.sh + 1), (uint32_t)p->bn};
+    const uint32_t box[4] = {(uint32_t)g.block_k, (uint32_t)((g.bw - 1) * s.sw + 1), (uint32_t)((g.bh - 1) * s.sh + 1), (uint32_t)g.bn};
     const uint32_t estr[4] = {1u, (uint32_t)s.sw, (uint32_t)s.sh, 1u};
     if (box[1] > 256 || box[2] > 256 || box[3] > 256) return TB200_ERR_UNSUPPORTED;
-    rc = tmap_encode(p->tmap_a, in, 4, dims, strides, box, estr, p->swizzle);
+    rc = tmap_encode(&p->tmap_a, in, 4, dims, strides, box, estr, g.swizzle);
     if (rc) return rc;
-    rc = encode_2d(p->tmap_b, w, (uint64_t)p->k, (uint64_t)p->n_tiles * p->block_n, (uint64_t)p->k, p->block_k, p->block_n, p->swizzle);
+    rc = encode_2d(&p->tmap_b, w, (uint64_t)k, (uint64_t)g.n_tiles * g.block_n, (uint64_t)k, g.block_k, g.block_n, g.swizzle);
     if (rc) return rc;
     // The rows of an m-tile are consecutive output pixels along one axis of the NHWC output (see the patch shapes above):
     //   bn > 1 (whole images)   : rows = pixels of bn consecutive images        -> map (C, N*OH*OW, 1), clipped at the end
     //   bn == 1, bw == OW       : rows = pixels of image n from row oh0 on       -> map (C, OH*OW, N), clipped per image
     //   bw == 128 < OW          : rows = 128 pixels of one image row             -> map (C, OW, N*OH), clipped per row
-    p->rows_valid = p->bw * p->bh * p->bn;
-    if (p->bw != s.ow)
+    g.rows_valid = g.bw * g.bh * g.bn;
+    if (g.bw != s.ow)
     {
-        p->out_mode = 2;
+        g.out_mode = 2;
         return plan_epilogue(p, out, (uint64_t)s.ow, (uint64_t)s.n * s.oh);
     }
-    if (p->bn > 1)
+    if (g.bn > 1)
     {
-        p->out_mode = 0;
+        g.out_mode = 0;
         return plan_epilogue(p, out, (uint64_t)s.n * s.oh * s.ow, 1);
     }
-    p->out_mode = 1;
+    g.out_mode = 1;
     return plan_epilogue(p, out, (uint64_t)s.oh * s.ow, (uint64_t)s.n);
 }
 
 // debug: event timeline of CTA 0 of the launch that just went out (needs a stream that is not being captured).
 // One line per event, sorted by time: cycles since the first event, role (P producer, M mma, E8/E15 epilogue warps), tag.
-static void gemm_trace_report(const GemmPlan& p, const GemmArgs& g, int grid, cudaStream_t st)
+static void gemm_trace_report(const GemmArgs& g, int grid, cudaStream_t st)
 {
     static unsigned long long h[4 * 1024];
     if (cudaStreamSynchronize(st) != cudaSuccess) return;
     cudaMemcpy(h, g.trace, sizeof h, cudaMemcpyDeviceToHost);
-    fprintf(stderr, "[gemm timeline] m_tiles=%lld k_blocks=%d bn=%d mt=%d stages=%d b_res=%d cs=%d grid=%d\n", (long long)p.m_tiles, p.k_blocks,
-            p.block_n, p.mt, p.stages, p.b_res, p.cs, grid);
+    fprintf(stderr, "[gemm timeline] m_tiles=%lld k_blocks=%d bn=%d mt=%d stages=%d b_res=%d cs=%d grid=%d\n", (long long)g.m_tiles, g.k_blocks,
+            g.block_n, g.mt, g.stages, g.b_res, g.cs, grid);
     unsigned long long t0 = ~0ull;
     for (int i = 0; i < 4 * 1024; i++)
         if (h[i] && (h[i] >> 8) < t0) t0 = h[i] >> 8;
@@ -1128,54 +1118,24 @@ static void gemm_trace_report(const GemmPlan& p, const GemmArgs& g, int grid, cu
         }
 }
 
-cudaError_t launch_gemm_i8(const GemmPlan& p, const EpiParams& e, const int32_t* btab, int num_sms, cudaStream_t st)
+cudaError_t launch_gemm_i8(const GemmPlan& p, cudaStream_t st)
 {
-    if (p.block_n <= 0 || p.mt <= 0 || p.stages <= 0 || p.cs <= 0) return cudaErrorInvalidValue; // plan was never created
-    GemmArgs g;
-    g.m_tiles = (int)p.m_tiles, g.k_blocks = p.k_blocks, g.n_tiles = p.n_tiles, g.block_n = p.block_n;
-    g.conv = p.conv, g.cblocks = p.cblocks, g.kw_n = p.kw_n, g.pad_h = p.pad_h, g.pad_w = p.pad_w, g.cstride = p.cstride, g.cp = p.cp;
-    g.bw = p.bw, g.bh = p.bh, g.bn = p.bn, g.tiles_w = p.tiles_w, g.tiles_h = p.tiles_h, g.oh = p.oh, g.ow = p.ow, g.nimg = p.nimg;
-    g.a_tx_bytes = p.a_tx_bytes;
-    g.u8 = p.u8, g.taps = p.taps, g.in_h = p.in_h, g.in_w = p.in_w, g.btab = btab, g.b_signed = p.b_signed, g.cplane = p.cplane;
-    g.fixq = (uint4*)p.fixq, g.fixq_cap = p.fixq_cap, g.out_base = (uint8_t*)p.out, g.ldo = p.ldo, g.m_rows = (int)p.m;
-    g.mt = p.mt;
-    g.num_super = (int)(((p.m_tiles + p.mt - 1) / p.mt) * p.n_tiles);
-    g.bw_rcp = p.conv ? (65536u + (uint32_t)p.bw - 1) / (uint32_t)p.bw : 0;
-    g.bh_rcp = p.conv ? (65536u + (uint32_t)p.bh - 1) / (uint32_t)p.bh : 0;
-    g.block_k = p.block_k, g.stages = p.stages, g.swizzle = p.swizzle, g.oc = p.oc, g.ocp = p.ocp;
-    g.cs = p.cs, g.ngroups = p.ngroups, g.rows_valid = p.rows_valid, g.out_mode = p.out_mode;
-    const int par_ch = p.n_tiles * p.block_n;
-    g.par_all = par_ch <= PAR_MAX ? 1 : 0;
-    const int a_bytes = BLOCK_M * p.block_k, b_bytes = (p.block_n * p.block_k + 1023) & ~1023;
-    g.b_res = p.b_res;
-    const size_t smem = (size_t)p.stages * (a_bytes + (p.b_res ? 0 : b_bytes)) + (p.b_res ? (size_t)p.k_blocks * b_bytes : 0) + (p.cplane ? 4096 : 0) +
-                        (size_t)EPI_WARPS * 2 * 512 * p.cs + sizeof(GemmSmemCtl) +
-                        (size_t)(g.par_all ? par_ch : p.block_n) * 8 + 16 + 128 * (size_t)acc_pitch(p.mt * p.block_n) + 1024;
+    if (p.grid <= 0) return cudaErrorInvalidValue; // plan was never created
     static const bool trace_on = getenv("TB200_GEMM_TRACE") != nullptr;
     const bool launch_dbg = debug_launch();
     static unsigned long long* trace_buf = nullptr;
-    g.trace = nullptr;
+    GemmArgs g = p.g;
     if (trace_on)
     {
         if (!trace_buf) cudaMalloc(&trace_buf, 4 * 1024 * sizeof(unsigned long long));
         cudaMemsetAsync(trace_buf, 0, 4 * 1024 * sizeof(unsigned long long), st);
         g.trace = trace_buf;
     }
-    int grid = (int)(g.num_super < num_sms ? g.num_super : num_sms);
-    if (p.b_res) grid -= grid % p.n_tiles; // a CTA must see one N tile only (num_super is a multiple of n_tiles, so grid >= n_tiles)
-    CUtensorMap ta, tb, to, tt;
-    memcpy(&ta, p.tmap_a, sizeof ta);
-    memcpy(&tb, p.tmap_b, sizeof tb);
-    memcpy(&to, p.tmap_out, sizeof to);
-    memcpy(&tt, p.tmap_out_tail, sizeof tt);
-    const int mode = !e.fast_ok ? 2 : ((!p.u8 && e.fuse_bias) ? 1 : 0);
+    const int grid = p.grid;
+    const size_t smem = (size_t)p.smem_bytes;
     cudaError_t err = cudaErrorInvalidValue;
-    // uint8 border corrections only exist for convolutions with taps that can fall into the padding: any window larger than one
-    // pixel, or a 1x1 window whose last row / column lies past the image (bottom / right padding, e.g. TF-style (0, 1))
-    const bool pad_1x1 = p.pad_h || p.pad_w || (p.oh - 1) * p.cstride >= p.in_h || (p.ow - 1) * p.cstride >= p.in_w;
-    const bool border = p.u8 && p.conv && (p.taps > 1 || pad_1x1);
 #define TB200_GEMM_CASE(U, MD, C, B)                                                                                           \
-    if ((p.u8 != 0) == U && mode == MD && p.cs == C && border == B)                                                            \
+    if ((g.u8 != 0) == U && p.mode == MD && g.cs == C && (p.border != 0) == B)                                                 \
     {                                                                                                                          \
         /* the opt-in is per device AND per context: set it before every launch (launches happen at graph capture only) */ \
         {                                                                                                                      \
@@ -1185,9 +1145,9 @@ cudaError_t launch_gemm_i8(const GemmPlan& p, const EpiParams& e, const int32_t*
         }                                                                                                                      \
         if (launch_dbg)                                                                                                        \
             fprintf(stderr, "tengine_b200: launch gemm_i8_tcgen05_kernel<U8=%d,MODE=%d,CS=%d,BORDER=%d> out_mode=%d conv=%d n_tiles=%d b_res=%d fixq=%d mt=%d par_all=%d\n", \
-                    (int)U, MD, C, (int)B, p.out_mode, p.conv, p.n_tiles, p.b_res, p.fixq != nullptr, p.mt, g.par_all);     \
-        gemm_i8_tcgen05_kernel<U, MD, C, B><<<grid, GEMM_THREADS, smem, st>>>(ta, tb, to, tt, g, e);                                                \
-        if (trace_on) gemm_trace_report(p, g, grid, st);                                                                       \
+                    (int)U, MD, C, (int)B, g.out_mode, g.conv, g.n_tiles, g.b_res, g.fixq != nullptr, g.mt, g.par_all);     \
+        gemm_i8_tcgen05_kernel<U, MD, C, B><<<grid, GEMM_THREADS, smem, st>>>(p.tmap_a, p.tmap_b, p.tmap_out, p.tmap_out_tail, g, p.e); \
+        if (trace_on) gemm_trace_report(g, grid, st);                                                                          \
         err = cudaGetLastError();                                                                                              \
         if (launch_dbg || err != cudaSuccess) gemm_launch_debug((const void*)gemm_i8_tcgen05_kernel<U, MD, C, B>, "launch", err, grid, smem, st); \
         return err;                                                                                                            \

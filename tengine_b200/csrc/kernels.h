@@ -1,5 +1,6 @@
 // kernels.h -- internal launcher interface between the graph executor (engine.cu) and the kernels.
 #pragma once
+#include <cuda.h> // CUtensorMap
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -74,12 +75,18 @@ cudaError_t launch_nhwc_to_nchw(const void* in, void* out, int n, int c, int h, 
 // ---- TMA-staged depthwise 3x3 (dw_tma.cu) ---------------------------------------------------------------
 struct DwPlan
 {
-    alignas(64) unsigned char tmap_in[128]; // CUtensorMap over the NHWC input (C, W, H, N)
-    int valid;
-    int tw, gpr, rows_per_cta, tile_cols, tile_rows, smem_bytes;
+    CUtensorMap tmap_in; // over the NHWC input (C, W, H, N)
+    const uint8_t* w;
+    uint8_t* out;
+    ConvShape s;
+    EpiParams e;
+    int gpr, rows_per_cta, tile_cols, tile_rows, smem_bytes;
+    dim3 grid;
+    int mode; // the epilogue the kernels take at run time (epi_mode), for TB200_DEBUG_LAUNCH
 };
-int dw_plan_create(DwPlan* plan, const void* in, const ConvShape& s, const EpiParams& e);
-cudaError_t launch_conv_dw_tma(const DwPlan& plan, const void* w, void* out, const ConvShape& s, const EpiParams& e, cudaStream_t st);
+// 0, or < 0 when this layer must use the generic depthwise kernel
+int dw_plan_create(DwPlan* plan, const void* in, const void* w, void* out, const ConvShape& s, const EpiParams& e);
+cudaError_t launch_conv_dw_tma(const DwPlan& plan, cudaStream_t st);
 
 // ---- fp32 members of the path (conv_fp32.cu): Winograd F(4x4,3x3) and depthwise 3x3 on NCHW fp32 ---------------
 size_t wino43_workspace_bytes(int n, int c, int oc, int oh, int ow);
@@ -140,49 +147,100 @@ cudaError_t launch_detect_pre(const uint8_t* pixels, const ImageDesc* images, in
                               const float scale[3], float s_in, int zp, bool u8, cudaStream_t st);
 
 // ---- small-Cin convolutions with a TMA-staged input window (conv_window.cu) -----------------------------------
+struct WindowArgs
+{
+    const uint8_t* w; // [OCp][ks*32]; NCHW: k = (c*KH + kh)*KW + kw ; NHWC: k = (kh*3 + kw)*CB + c ; zero padded
+    uint8_t* out;     // NHWC, OCp bytes per pixel
+    int n, c, h, w_in, oh, ow, ocp, oc, stride, ph, pw;
+    unsigned ntiles;
+    int tiles_w, tiles_h;
+    uint32_t tw_magic, th_magic; // floor(2^32 / d) + 1: q = umulhi(x, magic) is x / d for the tile counts that occur (checked by the planner)
+    int box_w, box_h, xoff, in_bytes, ks;
+    uint32_t fill; // uint8: the input zero point replicated x4 (0 for int8: the TMA zero fill already is the padding)
+};
 struct WindowPlan
 {
-    alignas(64) unsigned char tmap_in[128]; // CUtensorMap over the input: NCHW (W, H, C, N) or NHWC (Cp, W, H, N)
-    int valid;
+    CUtensorMap tmap_in; // over the input: NCHW (W, H, C, N) or NHWC (Cp, W, H, N)
+    WindowArgs a;
+    EpiParams e;
+    int smem_bytes;
+    int num_sms; // the grid is as many CTAs as the SMs hold at once, at most one per tile
+    // the instantiation conv_window_tc_kernel<MODE, U8 = e.is_uint8, LAYOUT>
+    int mode;
     int layout; // 0 NCHW 3x3, 1 NCHW 7x7, 2 NHWC 16 B/pixel 3x3, 3 NHWC 32 B/pixel 3x3
-    int box_w, box_h, xoff, in_bytes, ks, smem_bytes;
 };
-int window_plan_create(WindowPlan* plan, const void* in, const ConvShape& s, int nhwc); // < 0: not applicable
+// 0; 1 when the window kernel does not apply (the gather kernel takes the layer); < 0 (TB200_ERR_UNSUPPORTED) when it applies but
+// the layer has more output pixels or tiles than its 32-bit indices address
+int window_plan_create(WindowPlan* plan, const void* in, const void* w, void* out, const ConvShape& s, const EpiParams& e, int nhwc, int num_sms);
 bool window_nhwc_fits(int cp, int ocp, int stride); // a 3x3 conv over an NHWC input of cp bytes per pixel fits the kernel's shared memory
-cudaError_t launch_conv_window(const WindowPlan& plan, const void* w, void* out, const ConvShape& s, const EpiParams& e, int num_sms, cudaStream_t st);
+cudaError_t launch_conv_window(const WindowPlan& plan, cudaStream_t st);
+
 // the same layers without a window plan: every thread gathers its pixel's taps from global memory (NCHW stems, 16-channel NHWC inputs)
-cudaError_t launch_conv_gather_tc(const void* in, const void* w, void* out, const ConvShape& s, const EpiParams& e, int nhwc16, int num_sms,
-                                  cudaStream_t st);
+struct GatherArgs
+{
+    const uint8_t* in;
+    const uint8_t* w; // [OCp][ks*32]; NCHW: k = (c*3 + kh)*3 + kw ; NHWC16: k = (kh*3 + kw)*16 + c ; zero padded
+    uint8_t* out;
+    int n, c, h, w_in, oh, ow, ocp, oc, stride, ph, pw;
+    unsigned npix, ntiles;
+    int ks, nhwc16;
+    uint32_t fill; // byte for taps outside the image, replicated x4 (uint8: the input zero point; int8: 0)
+    uint32_t fill16[4]; // NHWC16: the same for a whole 16-channel tap; pad channels (c >= C) stay 0 like in the tensor itself
+};
+struct GatherPlan
+{
+    GatherArgs a;
+    EpiParams e;
+    int smem_bytes;
+    unsigned grid;
+    int mode, khw; // the instantiation conv_gather_tc_kernel<MODE, U8 = e.is_uint8, KHW>
+};
+void gather_plan_create(GatherPlan* plan, const void* in, const void* w, void* out, const ConvShape& s, const EpiParams& e, int nhwc16, int num_sms);
+cudaError_t launch_conv_gather_tc(const GatherPlan& plan, cudaStream_t st);
 
 // ---- wgmma GEMM (gemm_tcgen05.cu) --------------------------------------------------------------------
 // out[M][ldo] (bytes) = requant( A[M][K] (row pitch lda bytes) . B[OCp][K]^T )
+struct GemmArgs
+{
+    int m_tiles, num_super; // 32-bit on purpose: 64-bit divisions in the tile decode cost ~100 instructions each
+    int k_blocks, n_tiles, block_n, block_k, stages, swizzle;
+    int mt;     // m-tiles (128 rows each) per accumulator stage
+    uint32_t bw_rcp, bh_rcp; // ceil(65536/d): q = (x * rcp) >> 16 is exact for x < 4096, d <= 256
+    int oc, ocp;
+    // conv mode (implicit GEMM): an m-tile is a bw x bh x bn patch of output pixels, a k-block is (tap, channel block)
+    int conv, cblocks, kw_n, pad_h, pad_w, cstride, cp;
+    int bw, bh, bn, tiles_w, tiles_h, oh, ow, nimg;
+    uint32_t a_tx_bytes; // bytes one A load delivers (block_k * rows of the patch)
+    // uint8 (unsigned A): B holds w - 128 as int8 (plain w when zw == 0), so the accumulator is sum x*(w - 128); what is left of
+    // sum x*(w - zw) is cplane * sum(x) with cplane = 128 - zw, and the epilogue adds cplane * sum(x) inside the IADD3 that also
+    // adds the per-channel constant.
+    // sum(x) comes from two extra warps that add up the rows of every A tile in shared memory (cplane != 0 only).
+    int u8, taps, in_h, in_w, b_signed, cplane;
+    // epilogue / stores
+    int cs, ngroups; // 16-column chunks per store group (1 or 2) and groups per m-tile
+    int rows_valid;  // rows of an m-tile that are output pixels (128, or bw*bh*bn of a smaller conv patch)
+    int out_mode;    // coordinates of the output map: 0 (c, row, 0)  1 (c, pixel in image, image)  2 (c, x, image row)
+    int par_all;     // the constants of every channel are resident (loaded once); else reloaded per N tile
+    int b_res;       // the N tile's weights (all k-blocks) are loaded once and stay in smem; the ring carries A only
+    // deferred rare path: a guarded element is queued {m-tile, row, channel, accumulator} and recomputed literally by all threads of the
+    // CTA after its last tile, instead of holding up its epilogue warp (and with it the accumulator stage); null = inline
+    uint4* fixq;
+    int fixq_cap; // entries per CTA
+    uint8_t* out_base;
+    int ldo, m_rows; // output row pitch in bytes; rows of the flat GEMM
+    const int32_t* btab; // uint8 convolutions: [border pattern][OCp] summed corrections of the taps a border pixel misses (engine.cu)
+    unsigned long long* trace; // debug (TB200_GEMM_TRACE): event timeline of CTA 0, see gemm_trace_report
+};
 struct GemmPlan
 {
-    alignas(64) unsigned char tmap_a[128]; // CUtensorMap
-    alignas(64) unsigned char tmap_b[128];
-    alignas(64) unsigned char tmap_out[128];      // (C, rows, outer) over the output, box = 16*cs x 32 rows
-    alignas(64) unsigned char tmap_out_tail[128]; // same with rows_valid % 32 rows (last quarter of a short conv patch)
-    long long m;
-    int k;       // padded K (multiple of 16)
-    int oc, ocp; // logical / padded output channels
-    int ldo;     // output row pitch in bytes
-    int block_n, block_k, stages, k_blocks, n_tiles;
-    int mt; // m-tiles per accumulator stage
-    // conv mode (implicit GEMM over a 4-D tensor map)
-    int conv, cblocks, kw_n, pad_h, pad_w, cstride, cp, bw, bh, bn, tiles_w, tiles_h, oh, ow, nimg;
-    unsigned a_tx_bytes;
-    int u8, taps, in_h, in_w; // uint8: unsigned A operand
-    int b_signed, cplane;     // uint8: B holds w - 128 as int8, the epilogue adds (128 - zw) * sum(x) (gemm_tcgen05.cu)
-    long long m_tiles;
-    int swizzle; // 32 / 64 / 128
-    int cs, ngroups, rows_valid, out_mode; // epilogue store groups, see gemm_tcgen05.cu plan_epilogue
-    int b_res;                             // weights of the N tile resident in smem (ring carries A only)
-    void* out;
-    // deferred rare path (gemm_tcgen05.cu fixq_*): per-context scratch of fixq_cap 16-byte entries per CTA; null = fix inline
-    void* fixq;
-    int fixq_cap;
+    CUtensorMap tmap_a, tmap_b;
+    CUtensorMap tmap_out;      // (C, rows, outer) over the output, box = 16*cs x 32 rows
+    CUtensorMap tmap_out_tail; // same with rows_valid % 32 rows (last quarter of a short conv patch)
+    GemmArgs g;
+    EpiParams e;
+    int grid, smem_bytes;
+    int mode, border; // with g.u8 and g.cs: the instantiation gemm_i8_tcgen05_kernel<U8, MODE, CS, BORDER>
 };
-// Build TMA descriptors for fixed device pointers. Returns 0 or a negative TB200_ERR_*.
 // ordinal of the calling thread's current CUDA device (launchers keep per-device state: cudaFuncSetAttribute is per device)
 static inline int current_device()
 {
@@ -194,9 +252,14 @@ int gemm_block_n(int ocp); // channels of one N tile = rows of one packed B tile
 // TB200_DEBUG_LAUNCH (read once per process): the templated launchers print one stderr line per launch naming the instantiation,
 // "tengine_b200: launch <kernel><ARG=value,...>"; diagnostic only, changes nothing else
 bool debug_launch();
-int gemm_plan_create(GemmPlan* plan, const void* a, long long lda, const void* b, void* out, long long m, int k, int oc, int ocp, int ldo, int u8);
-int gemm_plan_create_conv(GemmPlan* plan, const void* in, const void* w, void* out, const ConvShape& s, int u8);
-cudaError_t launch_gemm_i8(const GemmPlan& plan, const EpiParams& e, const int32_t* btab, int num_sms, cudaStream_t st);
+// Build the TMA descriptors for fixed device pointers and every launch parameter.  Returns 0 or a negative TB200_ERR_*.
+// u8: 0 for int8, 1 + the weight zero point for uint8.  fixq: the deferred rare path's scratch of fixq_cap 16-byte entries per CTA
+// (gemm_tcgen05.cu fixq_*), null = fix inline.  btab: see GemmArgs.
+int gemm_plan_create(GemmPlan* plan, const void* a, long long lda, const void* b, void* out, long long m, int k, int oc, int ocp, int ldo, int u8,
+                     const EpiParams& e, const int32_t* btab, void* fixq, int fixq_cap, int num_sms);
+int gemm_plan_create_conv(GemmPlan* plan, const void* in, const void* w, void* out, const ConvShape& s, int u8, const EpiParams& e,
+                          const int32_t* btab, void* fixq, int fixq_cap, int num_sms);
+cudaError_t launch_gemm_i8(const GemmPlan& plan, cudaStream_t st);
 // measured peak of wgmma m64n128k32 s8 (two warpgroups per SM) on this GPU, in TOP/s: the tensor roofline's denominator
 cudaError_t probe_int8_mma_peak(int num_sms, double* tops, cudaStream_t st);
 

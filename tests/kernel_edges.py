@@ -26,7 +26,7 @@ def cpad(c):
 
 # ---- gemm_tcgen05.cu: plan geometry of the persistent GEMM ------------------------------------------------------------------
 BLOCK_M, ACC_COLS_MAX, PAR_MAX, MAX_STAGES, B_RESIDENT_MAX = 128, 128, 2048, 24, 96 * 1024
-EPI_WARPS, SMEM_CTL = 16, 432  # sizeof(GemmSmemCtl): (2 * MAX_STAGES + 5) uint64, 16-byte aligned
+PLAN_STG_WARPS, SMEM_CTL = 16, 432  # sizeof(GemmSmemCtl): (2 * MAX_STAGES + 5) uint64, 16-byte aligned
 
 
 def _block_n(ocp):
@@ -37,8 +37,8 @@ def _block_n(ocp):
 def gemm_geometry(ocp, u8zp, m=None, k=None, conv=None):
     """The plan of gemm_plan_create (flat: m rows, k = K) or gemm_plan_create_conv (conv = dict(n, h, w, cp, oh, ow, kh, kw,
     stride, ph0, pw0)).  u8zp is the planners' `u8` argument: 0 for int8, 1 + weight zero point for uint8.  Restates
-    gemm_tcgen05.cu gemm_block_n (:823-829), gemm_plan_create (:884-908), gemm_plan_create_conv (:912-979), plan_stage
-    (:835-843), epilogue_smem_bytes / plan_ring (:861-882), and launch_gemm_i8's par_all and BORDER (:1023, :1051)."""
+    gemm_tcgen05.cu gemm_block_n, plan_begin, gemm_plan_create, gemm_plan_create_conv (with its BORDER), plan_stage, and
+    plan_ring with epilogue_smem_bytes (par_all, b_res)."""
     G = dict(ocp=ocp)
     bn = G["block_n"] = _block_n(ocp)
     G["n_tiles"] = n_tiles = (ocp + bn - 1) // bn
@@ -93,7 +93,7 @@ def gemm_geometry(ocp, u8zp, m=None, k=None, conv=None):
     par_ch = n_tiles * bn
     G["par_all"] = 1 if par_ch <= PAR_MAX else 0
     cplane = u8zp > 1
-    epi = EPI_WARPS * 2 * 512 * cs + (par_ch if par_ch <= PAR_MAX else bn) * 8 + SMEM_CTL + 2048 + 128 * (mt * bn * 4 + 16) + 16
+    epi = PLAN_STG_WARPS * 2 * 512 * cs + (par_ch if par_ch <= PAR_MAX else bn) * 8 + SMEM_CTL + 2048 + 128 * (mt * bn * 4 + 16) + 16
     budget = 224 * 1024 - epi - (4096 if cplane else 0)
     a_bytes, b_al = BLOCK_M * bk, (bn * bk + 1023) & ~1023
     b_res = 1 if kb * b_al <= B_RESIDENT_MAX else 0
@@ -103,7 +103,7 @@ def gemm_geometry(ocp, u8zp, m=None, k=None, conv=None):
     return G
 
 
-# ---- dw_tma.cu dw_plan_create (:250-271): the TMA depthwise 3x3 or the generic kernel --------------------------------------
+# ---- dw_tma.cu dw_plan_create: the TMA depthwise 3x3 or the generic kernel ---------------------------------------------------
 DW_CH = 32
 
 
@@ -144,7 +144,7 @@ def window_nhwc_fits(cp, ocp, stride):
 
 def window_geometry(n, c, cp, w, oh, ow, k, stride, pw0, ocp, nhwc):
     """window_plan_create's checks beyond plan_conv's (group 1, no dilation, one stride, square kernel), its box and shared
-    memory, and the tile arithmetic of launch_conv_window: 16 x 8 output pixels per tile, the two tile counts divided by
+    memory, and its tiles: 16 x 8 output pixels per tile, the two tile counts divided by
     multiply-high with a magic number, 0 for a divisor of 1."""
     W = dict(valid=False, layout=None)
     if stride > 2 or ocp > 256:
@@ -175,7 +175,7 @@ def window_geometry(n, c, cp, w, oh, ow, k, stride, pw0, ocp, nhwc):
 
 
 def gather_geometry(n, c, oh, ow, k, nhwc16):
-    """launch_conv_gather_tc: 128 output pixels per tile; ks k-steps of 32 bytes (NHWC16: nine 16-byte taps and a zero half)."""
+    """gather_plan_create: 128 output pixels per tile; ks k-steps of 32 bytes (NHWC16: nine 16-byte taps and a zero half)."""
     npix = n * oh * ow
     return dict(ks=5 if nhwc16 else (c * k * k + 31) // 32, ntiles=(npix + 127) // 128, npix_mod128=npix % 128)
 

@@ -11,7 +11,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "tengine_b200", "csrc")
 LOG = os.path.join(CSRC, "gemm_tcgen05.o.ptxas.log")
 KERNEL = "gemm_i8_tcgen05_kernel"
-VARIANTS = 14  # <U8, MODE, CS, BORDER> combinations launch_gemm_i8 dispatches to
+VARIANTS = 14  # <U8, MODE, CS, BORDER> combinations the GEMM planners can select (launch_gemm_i8's TB200_GEMM_CASE list)
 
 
 def _nvcc():
