@@ -661,6 +661,7 @@ static void fuse_nodes(const tb200_layer_desc* layers, const tb200_tensor_desc* 
         if (!same) continue;
         fused[li].output = R.output, plan[li].post_relu = 1;
         fused[lj].op = TB200_OP_NOP_, fused[lj].num_inputs = 0;
+        if (debug_launch()) fprintf(stderr, "tengine_b200: plan fuse elt_relu layer=%d folded=%d\n", li, lj);
     }
     // (Leaky) ReLU -> max pooling whose output keeps the ReLU's quantisation, the ReLU result having no other reader: the ReLU is
     // a non-decreasing byte table, so max(table(x)) == table(max(x)); the pooling reads the convolution's bytes and applies the
@@ -679,6 +680,7 @@ static void fuse_nodes(const tb200_layer_desc* layers, const tb200_tensor_desc* 
         plan[lj].pool_relu = li;
         fused[lj].inputs[0] = R.inputs[0]; // the pooling reads what the ReLU read
         fused[li].op = TB200_OP_NOP_, fused[li].num_inputs = 0;
+        if (debug_launch()) fprintf(stderr, "tengine_b200: plan fuse relu_pool layer=%d folded=%d\n", lj, li);
     }
     // Sigmoid -> Eltwise-PROD with the Sigmoid's own input (x * sigmoid(x): how an int8 YOLOv5s spells SiLU, SURVEY.md 8(a)): both
     // operands of the product are functions of the same byte of x, so the PAIR is one byte table -- sigmoid's table composed with
@@ -698,6 +700,7 @@ static void fuse_nodes(const tb200_layer_desc* layers, const tb200_tensor_desc* 
         // E is fused[lj], so this compares the rewritten inputs[0]; nothing reads this axis but the pack-cache key
         fused[lj].axis = (E.inputs[0] == S.output) ? 0 : 1;
         fused[li].op = TB200_OP_NOP_, fused[li].num_inputs = 0;
+        if (debug_launch()) fprintf(stderr, "tengine_b200: plan fuse silu layer=%d folded=%d\n", lj, li);
     }
 }
 
@@ -963,6 +966,18 @@ static void plan_activation_arena(Shard* g, std::vector<LayerPlan>& plan)
         if (to.last_use < li && !permanent(to) && !freed[L.output]) release(to.off, to.slot_bytes), freed[L.output] = 1; // dead value
     }
     g->act_bytes = top;
+    if (debug_launch()) // the arena plan, for tests/graph_gen.py (a tensor neither produced nor read has no slot; its off is 0)
+    {
+        for (int i = 0; i < num_tensors; i++)
+        {
+            const TensorInfo& t = g->tensors[i];
+            fprintf(stderr, "tengine_b200: plan tensor %d off=%zu slot=%zu producer=%d last_use=%d\n", i, t.off, t.slot_bytes, t.producer, t.last_use);
+        }
+        for (int li = 0; li < num_layers; li++)
+            if (plan[li].kind == K_RESHAPE)
+                fprintf(stderr, "tengine_b200: plan scratch layer=%d off=%zu slot=%zu\n", li, plan[li].scratch_off,
+                        align_up(g->tensors[g->layers[li].output].nchw_bytes, 1024));
+    }
 }
 
 // The arenas and the NCHW staging buffers of the graph's inputs and outputs.

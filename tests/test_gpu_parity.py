@@ -12,11 +12,12 @@ pytestmark = pytest.mark.gpu
 
 
 def _run_all_layers(ctx, g, x, flags):
+    """x: the graph's one input, or a list of one array per graph input."""
     from tengine_b200 import runtime as rt
 
     gr = rt.Graph(ctx, g, flags | abi.PRERUN_NO_GRAPH)
     try:
-        outs = gr.run([x])
+        outs = gr.run(x if isinstance(x, list) else [x])
         tensors = {t: gr.read_tensor(t) for t in layer_outputs(g)}
         return outs, tensors, gr.layer_kernels()
     finally:
@@ -26,18 +27,16 @@ def _run_all_layers(ctx, g, x, flags):
 FLAGS = [abi.PRERUN_DEFAULT, abi.PRERUN_NO_TENSORCORE]
 
 
-# the KATs of the convolution / FC / pooling tests (single graph input); the glue-op KATs added later pin the oracle on the CPU
-_GPU_KATS = [k for k in kat_graphs() if k[0] in ("uint8_conv3x3_pad1", "uint8_depthwise3x3_pad1", "uint8_fc", "uint8_maxpool3x3s2_const", "int8_conv3x3_bias")]
-
-
 @pytest.mark.parametrize("flags", FLAGS, ids=["tensorcore", "cudacore"])
-@pytest.mark.parametrize("kat", _GPU_KATS, ids=lambda k: k[0])
-def test_reference_kats(ctx, kat, flags):
+@pytest.mark.parametrize("kat", kat_graphs(), ids=lambda k: k[0])
+def test_reference_kats(ctx, oracle, kat, flags):
+    """Every known-answer vector of the reference's op tests, each graph input fed: within the vector's own tolerance of the
+    reference's expected values, and bit-exact against the oracle."""
     name, g, xins, expected, tol = kat
-    xin = xins[0]
-    outs, _, _ = _run_all_layers(ctx, g, xin, flags)
+    outs, _, _ = _run_all_layers(ctx, g, xins, flags)
     real = dequant(g, g.outputs[0], outs[0])
     assert np.abs(real - expected).max() <= tol + 1e-6
+    assert np.array_equal(outs[0], oracle.run(g, xins, uint8_mode=0)[g.outputs[0]])
 
 
 @pytest.mark.parametrize("flags", FLAGS, ids=["tensorcore", "cudacore"])
