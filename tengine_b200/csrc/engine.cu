@@ -484,7 +484,7 @@ static int run_step(const Shard* g, const Step& s, cudaStream_t st)
     case K_POOL: { auto& a = args<PoolArgs>(s); err = launch_pool(a.in, a.out, a.ps, a.u8, st); break; }
     case K_POINTWISE: { auto& a = args<PointwiseArgs>(s); err = launch_pointwise(a.in, a.in2, a.out, a.bytes, a.pp, a.u8, st); break; }
     case K_CONCAT_PART: { auto& a = args<ConcatArgs>(s); err = launch_concat_part(a.in, a.out, a.part, a.u8, st); break; }
-    case K_CONCAT_LUT: { auto& a = args<ConcatArgs>(s); err = launch_concat_lut(a.in, a.out, a.part, st); break; }
+    case K_CONCAT_LUT: { auto& a = args<ConcatArgs>(s); err = launch_concat_lut(a.in, a.out, a.part, a.u8, st); break; }
     case K_LUT: { auto& a = args<ByteLutArgs>(s); err = launch_byte_lut(a.in, a.out, a.lut, a.bytes, a.c, a.cp, st); break; }
     case K_SOFTMAX: { auto& a = args<SoftmaxArgs>(s); err = launch_softmax(a.in, a.out, a.sm, a.u8, st); break; }
     case K_RESHAPE:
@@ -1532,7 +1532,8 @@ static int fill_concat_steps(const Shard* g, int li, const LayerPlan& P, const S
         q.npix = (long long)sl.nb * tin.d.dims[2] * tin.d.dims[3], q.c = tk.d.dims[1], q.cp_in = tk.cp, q.cp_out = tout.cp, q.c_off = coff;
         q.s_in = tk.d.scale, q.z_in = tk.d.zero_point, q.s_out = tout.d.scale, q.z_out = tout.d.zero_point;
         q.c_write = (k + 1 == L.num_inputs) ? tout.cp - coff : tk.d.dims[1];
-        // vectorised table path when everything is 16-channel aligned; identical quantisation -> no table at all
+        // vectorised table path when everything is 16-channel aligned; identical quantisation -> no table at all (a copy, int8
+        // -128 -> +127)
         q.lut = (tk.d.scale == tout.d.scale && tk.d.zero_point == tout.d.zero_point) ? nullptr : g->w_arena + P.blob.w_off + 256 * k;
         const Step p{tk.d.dims[1] % 16 == 0 && coff % 16 == 0 ? K_CONCAT_LUT : K_CONCAT_PART, li, ConcatArgs{sl.dev(tk), sl.dev(tout), q, u8}};
         coff += tk.d.dims[1];

@@ -1144,8 +1144,9 @@ cudaError_t launch_gemm_i8(const GemmPlan& p, cudaStream_t st)
             if (err != cudaSuccess) return err;                                                                                \
         }                                                                                                                      \
         if (launch_dbg)                                                                                                        \
-            fprintf(stderr, "tengine_b200: launch gemm_i8_tcgen05_kernel<U8=%d,MODE=%d,CS=%d,BORDER=%d> out_mode=%d conv=%d n_tiles=%d b_res=%d fixq=%d mt=%d par_all=%d\n", \
-                    (int)U, MD, C, (int)B, g.out_mode, g.conv, g.n_tiles, g.b_res, g.fixq != nullptr, g.mt, g.par_all);     \
+            fprintf(stderr, "tengine_b200: launch gemm_i8_tcgen05_kernel<U8=%d,MODE=%d,CS=%d,BORDER=%d> out_mode=%d conv=%d n_tiles=%d b_res=%d fixq=%d mt=%d par_all=%d block_n=%d b_signed=%d cplane=%d\n", \
+                    (int)U, MD, C, (int)B, g.out_mode, g.conv, g.n_tiles, g.b_res, g.fixq != nullptr, g.mt, g.par_all, g.block_n,           \
+                    (int)g.b_signed, g.cplane);                                                                                        \
         gemm_i8_tcgen05_kernel<U, MD, C, B><<<grid, GEMM_THREADS, smem, st>>>(p.tmap_a, p.tmap_b, p.tmap_out, p.tmap_out_tail, g, p.e); \
         if (trace_on) gemm_trace_report(g, grid, st);                                                                          \
         err = cudaGetLastError();                                                                                              \

@@ -67,7 +67,7 @@ cudaError_t launch_concat_part(const void* in, void* out, const ConcatPart& p, b
 cudaError_t launch_byte_lut(const void* in, void* out, const uint8_t* lut, long long bytes, int c, int cp, cudaStream_t st);
 // softmax over the channel axis (softmax_kernel_ref_int8.c / _uint8.c), one thread per pixel
 cudaError_t launch_softmax(const void* in, void* out, const SoftmaxShape& p, bool u8, cudaStream_t st);
-cudaError_t launch_concat_lut(const void* in, void* out, const ConcatPart& p, cudaStream_t st);
+cudaError_t launch_concat_lut(const void* in, void* out, const ConcatPart& p, bool u8, cudaStream_t st);
 cudaError_t launch_upsample(const void* in, void* out, int n, int h, int w, int cp, int scale, cudaStream_t st);
 cudaError_t launch_nchw_to_nhwc(const void* in, void* out, int n, int c, int h, int w, cudaStream_t st);
 cudaError_t launch_nhwc_to_nchw(const void* in, void* out, int n, int c, int h, int w, cudaStream_t st);

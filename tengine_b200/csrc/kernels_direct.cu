@@ -908,10 +908,11 @@ cudaError_t launch_pointwise(const void* a, const void* b, void* out, long long 
 }
 
 // Vectorised form for 16-channel-aligned inputs: the per-input requantisation of concat_kernel_ref_{int8,uint8}.c is a function of one
-// byte, so it is a 256-entry table (built by engine.cu with the reference's arithmetic; nullptr = identity: equal quantisation).
+// byte, so it is a 256-entry table (built by engine.cu with the reference's arithmetic; nullptr = equal quantisation: a copy,
+// except that int8 -128 becomes +127 as in the reference's clamp, concat_kernel_ref_int8.c:77-78).
 // Thread = 16 channels of one pixel; the last input also clears the output's pad lanes (vectors beyond its channels).
 __global__ void __launch_bounds__(256) concat_lut_kernel(const uint4* __restrict__ in, uint8_t* __restrict__ out, const uint8_t* __restrict__ lut, long long npix,
-                                                         int cv_in, int cv_write, int cp_in, int cp_out, int c_off)
+                                                         int cv_in, int cv_write, int cp_in, int cp_out, int c_off, bool s8)
 {
     __shared__ uint8_t tab[256];
     if (lut)
@@ -936,16 +937,20 @@ __global__ void __launch_bounds__(256) concat_lut_kernel(const uint4* __restrict
                        ((uint32_t)tab[w[j] >> 24] << 24);
             r = make_uint4(w[0], w[1], w[2], w[3]);
         }
+        else if (s8) // 0x80 ^ 0xff = 0x7f; every other byte is left as it is
+            r = make_uint4(r.x ^ __vcmpeq4(r.x, 0x80808080u), r.y ^ __vcmpeq4(r.y, 0x80808080u), r.z ^ __vcmpeq4(r.z, 0x80808080u),
+                           r.w ^ __vcmpeq4(r.w, 0x80808080u));
     }
     *reinterpret_cast<uint4*>(out + (size_t)pix * cp_out + c_off + v * 16) = r;
 }
 
-cudaError_t launch_concat_lut(const void* in, void* out, const ConcatPart& p, cudaStream_t st)
+cudaError_t launch_concat_lut(const void* in, void* out, const ConcatPart& p, bool u8, cudaStream_t st)
 {
     if ((p.c % 16) || (p.c_off % 16) || (p.c_write % 16)) return cudaErrorInvalidValue;
     const long long total = p.npix * (p.c_write / 16);
     TB200_CHECK_32BIT(total * 16);
-    concat_lut_kernel<<<blocks_for(total, 256), 256, 0, st>>>((const uint4*)in, (uint8_t*)out, p.lut, p.npix, p.c / 16, p.c_write / 16, p.cp_in, p.cp_out, p.c_off);
+    concat_lut_kernel<<<blocks_for(total, 256), 256, 0, st>>>((const uint4*)in, (uint8_t*)out, p.lut, p.npix, p.c / 16, p.c_write / 16, p.cp_in, p.cp_out, p.c_off,
+                                                              !u8);
     return cudaGetLastError();
 }
 

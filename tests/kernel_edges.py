@@ -92,9 +92,15 @@ def gemm_geometry(ocp, u8zp, m=None, k=None, conv=None):
     G["cs"] = cs = 2 if nch % 2 == 0 and (mt * (nch // 2)) % 4 == 0 else 1
     par_ch = n_tiles * bn
     G["par_all"] = 1 if par_ch <= PAR_MAX else 0
-    cplane = u8zp > 1
+    # plan_begin: uint8 B holds w - 128 (signed) unless zw == 0, and the epilogue adds cplane * sum(x) with cplane = 128 - zw;
+    # gemm_mma_dispatch<AU, BU = !b_signed> picks the MMA warpgroup's code by (block_n, mt)
+    G["b_signed"] = int(u8zp != 1)
+    G["cplane"] = cplane = 128 - (u8zp - 1) if u8zp > 1 else 0
+    if u8zp:
+        G["u8_operands"] = {1: "unsigned_b", 129: "no_cplane", 2: "cplane_max", 256: "cplane_min"}.get(u8zp, "cplane")
+        G["mma_uu"] = (bn, mt) if u8zp == 1 else None
     epi = PLAN_STG_WARPS * 2 * 512 * cs + (par_ch if par_ch <= PAR_MAX else bn) * 8 + SMEM_CTL + 2048 + 128 * (mt * bn * 4 + 16) + 16
-    budget = 224 * 1024 - epi - (4096 if cplane else 0)
+    budget = 224 * 1024 - epi - (4096 if cplane else 0)  # the row sums' region exists only with cplane != 0
     a_bytes, b_al = BLOCK_M * bk, (bn * bk + 1023) & ~1023
     b_res = 1 if kb * b_al <= B_RESIDENT_MAX else 0
     if b_res and (budget - kb * b_al) // a_bytes < 3:
@@ -321,6 +327,26 @@ def geometry(g, L, no_tc=False):
     return dict(kind=abi.OP_NAMES[L["op"]], c_mod16=C % 16, channels=C)
 
 
+def data_edges(case, e):
+    """What an entry's quantisation and data reach beyond the plan: uint8 input and output zero points (zx, zo), whether a uint8
+    pooling result falls below 0 and wraps (pool_wraps), and whether an int8 graph input holds -128 (in_min_byte)."""
+    g = case.g
+    L = g.layers[e.layer]
+    if g.data_type != abi.DT_UINT8:
+        return dict(in_min_byte=any(bool((np.asarray(x) == -128).any()) for x in case.inputs))
+    D = dict(zx=g.tensors[L["inputs"][0]]["zero_point"], zo=g.tensors[L["output"]]["zero_point"])
+    if L["op"] == abi.OP_POOL and e.ref == "exact":
+        r = ties.exact_run(g, case.inputs)[1][L["output"]]
+        D["pool_wraps"] = bool((ties._round_away(r.t) + r.add < 0).any())
+    return D
+
+
+def reached(case, e):
+    """geometry() of the entry's layer and its data_edges."""
+    no_tc = bool(e.flags & abi.PRERUN_NO_TENSORCORE)
+    return dict(geometry(case.g, case.g.layers[e.layer], no_tc=no_tc), **data_edges(case, e))
+
+
 # ---- the table ------------------------------------------------------------------------------------------------------------
 @dataclass
 class Entry:
@@ -384,11 +410,40 @@ def int8_fc_hw(rng, n, c, h, w, oc, mode=0, m_exps=ties.M_EXPS, tie_frac=0.10):
     return cs
 
 
-def u8_conv_pad(rng, n, c, h, w, oc, k, stride, pad, mode=0, dilation=1):
+def u8_conv_pad(rng, n, c, h, w, oc, k, stride, pad, mode=0, dilation=1, **zps):
     """uint8 conv with a 4-tuple padding (h0, h1, w0, w1) or a dilation: ties.uint8_conv's layer, rebuilt through
-    g.conv(..., pad=..., dilation=...)."""
-    case = ties.uint8_conv(rng, n, c, h, w, oc, k=k, stride=stride, pad=0, mode=mode)
+    g.conv(..., pad=..., dilation=...).  zps: ties.uint8_conv's zero points."""
+    case = ties.uint8_conv(rng, n, c, h, w, oc, k=k, stride=stride, pad=0, mode=mode, **zps)
     return _repad(case, pad, dilation)
+
+
+def u8_far(rng, n, c, h, w, oc, k=1, pad=0, fc=False, zx=255, zw=0, s_out=16.0):
+    """uint8 conv / FC with inputs and weights at the far ends of the byte range from their zero points (|x - zx| and |w - zw| in
+    [235, 255]), so that the accumulator nears 255^2 K (1.6e9 at K = 25088, 3/4 of int32).  The bias takes each channel's median
+    accumulator off (padded: the interior's) and s_out spreads t over about +-40.  Past 2^24 the reference rounds the accumulator
+    to fp32 before it scales it, which ties.exact_layer does not model: compared with the oracle.  MODE 2 (the clamp-range proof
+    fails)."""
+    g = GraphDef(abi.DT_UINT8)
+    s_in, s_w = 2.0 ** -4, 2.0 ** -3
+    x = g.input(n, c, h, w, s_in, zx)
+    kk = c * h * w if fc else c * k * k
+    far = lambda z, shape: ((0 if z > 127 else 235) + rng.integers(0, 21, shape)).astype(np.uint8)  # noqa: E731
+    wq = far(zw, (oc, kk) if fc else (oc, c, k, k))
+    xin = far(zx, (n, c, h, w))
+    L = dict(group=1, stride_h=1, stride_w=1, dilation_h=1, dilation_w=1, pad_h0=pad, pad_h1=pad, pad_w0=pad, pad_w1=pad)
+    acc = ties.conv_acc(xin.reshape(n, 1, 1, -1), wq.reshape(oc, 1, 1, -1), dict(L, pad_h0=0, pad_h1=0, pad_w0=0, pad_w1=0), zx, zw) \
+        if fc else ties.conv_acc(xin, wq, L, zx, zw)
+    b = (-np.rint(np.median(acc, axis=(0, 2, 3))) + rng.integers(-40, 41, oc) * s_out / (s_in * s_w)).astype(np.int32)
+    if fc:
+        y = g.fc(x, wq, b, [s_w], s_out, 128, weight_zero=zw)
+    else:
+        y = g.conv(x, wq, b, [s_w], s_out, 128, pad=pad, weight_zero=zw)
+    g.mark_output(y)
+    cs = ties.Case(f"uint8_far_{'fc' if fc else f'k{k}'}_K{kk}_z{zx}_{zw}", g, [xin])
+    cs.mode = ties.planned_mode(g, g.layers[0])
+    cs.notes["acc_max"] = int(np.abs(acc).max())
+    assert cs.mode == 2, cs.name
+    return cs
 
 
 def i8_conv_pad(rng, n, c, h, w, oc, k, stride, pad, mode=1, dilation=1):
@@ -410,72 +465,101 @@ def _repad(case, pad, dilation=1):
     return case
 
 
-def act_conv(rng, u8, n, c, h, w, oc, activation, recipe, s_out, k=3, stride=1, pad=1, group=1, zo=110, t_mid=0.0):
+def act_conv(rng, u8, n, c, h, w, oc, activation, recipe, s_out, k=3, stride=1, pad=1, group=1, zo=110, t_mid=0.0, zx=ties.U8_ZX,
+             zw=ties.U8_ZW, min_byte=False):
     """A conv whose t = f / s_out lies within a few units of t_mid, so that the activation's clamp cuts it: the clamp bounds over
     a power-of-two s_out (6 / 4 = 1.5, 1 / 2 = 0.5) are half-integers, which the reference rounds away from zero.  M = 2^-1
     (every odd accumulator is a tie); weights +-1 on about six taps per output, inputs in [-2, 2] about the zero point, so t
-    spreads over about +-2 whatever K is."""
+    spreads over about +-2 whatever K is.  uint8 zero points zx, zw, zo: at an end of the byte range the inputs are
+    [0, 4] or [251, 255] (ties._shift) and the weights zw + {0, 1} or zw - {0, 1}; the bias takes the accumulator's mean off."""
     g = GraphDef(abi.DT_UINT8 if u8 else abi.DT_INT8)
     s_in, M = 2.0 ** -4, 0.5
     cg = c // group
     kk = cg * k * k
-    zx, zw = (ties.U8_ZX, ties.U8_ZW) if u8 else (0, 0)
+    zx, zw = (zx, zw) if u8 else (0, 0)
     x = g.input(n, c, h, w, s_in, zx)
     wd = rng.choice(np.array([-1, 1]), (oc, cg, k, k)) * (rng.random((oc, cg, k, k)) < min(1.0, 6.0 / kk))
+    if u8 and ties._shift(zw, -1, 1):
+        wd = np.abs(wd) * (1 if zw < 128 else -1)
     b = (np.round(t_mid / M) + rng.integers(-2, 3, oc)).astype(np.int32)
     s_w = M * s_out / s_in
     if u8:
+        xin = (zx + ties._shift(zx, -2, 2) + rng.integers(-2, 3, (n, c, h, w))).astype(np.uint8)
+        if ties._shift(zx, -2, 2) or ties._shift(zw, -1, 1):
+            L = dict(group=group, stride_h=stride, stride_w=stride, dilation_h=1, dilation_w=1, pad_h0=pad, pad_h1=pad, pad_w0=pad,
+                     pad_w1=pad)
+            b = (b - np.rint(ties.conv_acc(xin, zw + wd, L, zx, zw).mean(axis=(0, 2, 3)))).astype(np.int32)
         y = g.conv(x, (zw + wd).astype(np.uint8), b, [s_w], s_out, zo, stride=stride, pad=pad, group=group,
                    activation=activation, recipe=recipe, weight_zero=zw)
     else:
         y = g.conv(x, wd.astype(np.int8), b, np.full(oc, s_w, np.float32), s_out, stride=stride, pad=pad, group=group,
                    activation=activation, recipe=recipe)
+        xin = rng.integers(-2, 3, (n, c, h, w)).astype(np.int8)
+        if min_byte:
+            xin[rng.random(xin.shape) < ties.MIN_BYTE_FRAC] = -128
     g.mark_output(y)
-    xin = (zx + rng.integers(-2, 3, (n, c, h, w))).astype(np.uint8 if u8 else np.int8)
     cs = ties.Case(("uint8" if u8 else "int8") + f"_act{activation}_r{recipe}_so{s_out}_n{n}c{c}_{h}x{w}_oc{oc}_k{k}", g, [xin],
                    min_tie_frac=0.05)
     cs.mode = ties.planned_mode(g, g.layers[0])
     return cs
 
 
-def concat_n(rng, u8, chans, shape=(2, 5, 7)):
+def concat_n(rng, u8, chans, shape=(2, 5, 7), zps=None, zo=110, ratios=None, min_byte=False):
     """Concat of len(chans) inputs with s_in / s_out = 1/2, 1/4, 1/2, ... (t = q/2, q/4): inputs whose channel count and offset
-    are multiples of 16 take the byte table, the others the bytewise path (engine.cu fill_concat_steps)."""
+    are multiples of 16 take the byte table, the others the bytewise path (engine.cu fill_concat_steps).  zps: the inputs' uint8
+    zero points (default 120, 125, ...); ratios: s_in / s_out per input (1: an input whose quantisation may equal the output's,
+    which the table path copies)."""
     g = GraphDef(abi.DT_UINT8 if u8 else abi.DT_INT8)
     n, h, w = shape
     ins, xs = [], []
     for i, c in enumerate(chans):
-        zp = (120 + 5 * i) if u8 else 0
-        ins.append(g.input(n, c, h, w, 2.0 ** -(5 + i % 2), zp))
-        xs.append(ties._in(rng, u8, (n, c, h, w), -100, 100, zp=zp))
-    g.mark_output(g.concat(ins, 2.0 ** -4, 110 if u8 else 0))
+        zp = ((120 + 5 * i) if zps is None else zps[i]) if u8 else 0
+        s = 2.0 ** -(5 + i % 2) if ratios is None else 2.0 ** -4 * ratios[i]
+        ins.append(g.input(n, c, h, w, s, zp))
+        xs.append(ties._in(rng, u8, (n, c, h, w), -100, 100, zp=zp, min_byte=min_byte))
+    g.mark_output(g.concat(ins, 2.0 ** -4, zo if u8 else 0))
     return ties.Case(("uint8" if u8 else "int8") + "_concat_" + "_".join(map(str, chans)), g, xs, min_tie_frac=0.10)
 
 
-def relu_maxpool(rng, u8, c, slope_exp=None, shape=(2, 9, 11)):
+def relu_maxpool(rng, u8, c, slope_exp=None, shape=(2, 9, 11), zi=128, zo=110, min_byte=False):
     """(Leaky) ReLU, then a 3x3 / 2 max pooling keeping the ReLU's quantisation: the pooling folds the ReLU in as a byte table
     (engine.cu fuse_nodes) when the ReLU's output is read by the pooling alone."""
     g = GraphDef(abi.DT_UINT8 if u8 else abi.DT_INT8)
-    zi, zo = (128, 110) if u8 else (0, 0)
+    zi, zo = (zi, zo) if u8 else (0, 0)
     n, h, w = shape
     x = g.input(n, c, h, w, 2.0 ** -5, zi)
     y = g.relu(x, 2.0 ** -4, zo, negative_slope=0.0 if slope_exp is None else 2.0 ** -slope_exp)
     g.mark_output(g.pool(y, abi.POOL_MAX, 3, 2, 1))
-    xs = [ties._in(rng, u8, (n, c, h, w), -100, 100, zp=zi)]
+    xs = [ties._in(rng, u8, (n, c, h, w), -100, 100, zp=zi, min_byte=min_byte)]
     return ties.Case(("uint8" if u8 else "int8") + f"_relu_maxpool_c{c}", g, xs, min_tie_frac=0.20)
 
 
-def eltwise_relu(rng, u8, c, shape=(2, 9, 11)):
-    """Eltwise SUM, then a ReLU with the sum's own quantisation: folded into the eltwise kernel (engine.cu fuse_nodes)."""
+def eltwise_relu(rng, u8, c, shape=(2, 9, 11), z0=120, z1=130, zo=110, elt=abi.ELT_SUM, min_byte=False):
+    """Eltwise SUM (or PROD), then a ReLU with the eltwise's own quantisation: folded into the eltwise kernel (engine.cu
+    fuse_nodes)."""
     g = GraphDef(abi.DT_UINT8 if u8 else abi.DT_INT8)
-    z0, z1, zo = (120, 130, 110) if u8 else (0, 0, 0)
+    z0, z1, zo = (z0, z1, zo) if u8 else (0, 0, 0)
     n, h, w = shape
-    a = g.input(n, c, h, w, 2.0 ** -4, z0)
-    b = g.input(n, c, h, w, 2.0 ** -5, z1)
-    s = g.eltwise(a, b, 2.0 ** -4, zo, elt_type=abi.ELT_SUM)
+    s0, s1, so, r = (2.0 ** -4, 2.0 ** -5, 2.0 ** -4, 60) if elt == abi.ELT_SUM else (2.0 ** -3, 2.0 ** -3, 2.0 ** -2, 40)
+    a = g.input(n, c, h, w, s0, z0)
+    b = g.input(n, c, h, w, s1, z1)
+    s = g.eltwise(a, b, so, zo, elt_type=elt)
     g.mark_output(g.relu(s))
-    xs = [ties._in(rng, u8, (n, c, h, w), -60, 60, zp=z0), ties._in(rng, u8, (n, c, h, w), -60, 60, zp=z1)]
+    xs = [ties._in(rng, u8, (n, c, h, w), -r, r, zp=z0, min_byte=min_byte), ties._in(rng, u8, (n, c, h, w), -r, r, zp=z1,
+                                                                                     min_byte=min_byte)]
     return ties.Case(("uint8" if u8 else "int8") + f"_eltwise_relu_c{c}", g, xs, min_tie_frac=0.05)
+
+
+def unary(rng, u8, op, c, shape=(2, 9, 11), zi=128, zo=0, min_byte=False):
+    """Sigmoid or hardswish (uint8 only, as in the reference) over the whole byte range of its input: a byte table built at
+    prerun (engine.cu), compared with the oracle."""
+    g = GraphDef(abi.DT_UINT8 if u8 else abi.DT_INT8)
+    zi, zo = (zi, zo) if u8 else (0, 0)
+    n, h, w = shape
+    x = g.input(n, c, h, w, 2.0 ** -4, zi)
+    g.mark_output(g.sigmoid(x, 2.0 ** -8 if u8 else 2.0 ** -7, zo) if op == "sigmoid" else g.hardswish(x, 2.0 ** -4, zo))
+    xs = [ties._in(rng, u8, (n, c, h, w), -127, 127, zp=zi, min_byte=min_byte)]
+    return ties.Case(("uint8" if u8 else "int8") + f"_{op}_c{c}", g, xs)
 
 
 def silu(rng, c, shape=(2, 9, 11)):
@@ -488,20 +572,32 @@ def silu(rng, c, shape=(2, 9, 11)):
     return ties.Case(f"int8_silu_c{c}", g, [ties._in(rng, False, (n, c, h, w), -127, 127)])
 
 
-def softmax(rng, u8, c, h=1, w=1, n=3):
+def relu_same(rng, c, shape=(2, 9, 11)):
+    """int8 ReLU keeping its input's quantisation (max(byte, 0): engine.cu's same-scale kernel) over inputs with -128."""
+    g = GraphDef(abi.DT_INT8)
+    n, h, w = shape
+    x = g.input(n, c, h, w, 2.0 ** -4)
+    g.mark_output(g.relu(x))
+    return ties.Case(f"int8_relu_same_c{c}", g, [ties._in(rng, False, (n, c, h, w), -127, 127, min_byte=True)])
+
+
+def softmax(rng, u8, c, h=1, w=1, n=3, zi=128, min_byte=False):
     g = GraphDef(abi.DT_UINT8 if u8 else abi.DT_INT8)
-    zi = 128 if u8 else 0
+    zi = zi if u8 else 0
     x = g.input(n, c, h, w, 2.0 ** -4, zi)
     g.mark_output(g.softmax(x, 2.0 ** -7 if not u8 else 2.0 ** -8, 0))
-    return ties.Case(("uint8" if u8 else "int8") + f"_softmax_c{c}_{h}x{w}", g, [ties._in(rng, u8, (n, c, h, w), -100, 100, zp=zi)])
+    return ties.Case(("uint8" if u8 else "int8") + f"_softmax_c{c}_{h}x{w}", g,
+                     [ties._in(rng, u8, (n, c, h, w), -100, 100, zp=zi, min_byte=min_byte)])
 
 
-def upsample(rng, u8, c, scale, shape=(2, 5, 6)):
+def upsample(rng, u8, c, scale, shape=(2, 5, 6), zi=128, min_byte=False):
     g = GraphDef(abi.DT_UINT8 if u8 else abi.DT_INT8)
     n, h, w = shape
-    x = g.input(n, c, h, w, 2.0 ** -4, 128 if u8 else 0)
+    zi = zi if u8 else 0
+    x = g.input(n, c, h, w, 2.0 ** -4, zi)
     g.mark_output(g.upsample(x, scale))
-    return ties.Case(("uint8" if u8 else "int8") + f"_upsample{scale}_c{c}", g, [ties._in(rng, u8, (n, c, h, w), -100, 100, zp=128 if u8 else 0)])
+    return ties.Case(("uint8" if u8 else "int8") + f"_upsample{scale}_c{c}", g,
+                     [ties._in(rng, u8, (n, c, h, w), -100, 100, zp=zi, min_byte=min_byte)])
 
 
 G_, I_, D_, DD = "gemm_i8_tcgen05", "conv_igemm_i8_tcgen05", "conv_dw3x3_tma_dp4a", "conv_dw_direct"
@@ -730,6 +826,138 @@ _add("eltwise_relu_i8_c24", lambda r: eltwise_relu(r, False, 24), _F, dict(c_mod
 _add("eltwise_relu_u8_c32", lambda r: eltwise_relu(r, True, 32), _F, dict(c_mod16=0), layer=1, fused=True, tie_layer=0)
 _add("silu_i8_c24", lambda r: silu(r, 24), _F, dict(c_mod16=8), fused=True, ref="oracle", ties=False)
 
+# ---- the ends of the byte range: uint8 zero points 0, 1, 128 and 255 -----------------------------------------------------------
+# The uint8 GEMM's operand regime follows the weight zero point (gemm_tcgen05.cu plan_begin): zw 0 -> B holds the plain weights,
+# unsigned (the u8.u8 MMA), no cplane term; zw 128 -> cplane 0, no row-sum warps; else B holds w - 128 and cplane = 128 - zw adds
+# cplane * sum(x) from the row sums (+127 at zw 1, -127 at zw 255).  Each regime through the 1x1 GEMM, an FC over C % 16 != 0,
+# the implicit GEMM with padding (border table), several N tiles, streamed B (b_res 0), MODE 0 and MODE 2.  The MODE 0 entries
+# keep x about a mid zero point (one-sided x and w would put the bias past the fast path's bound); the MODE 2 ones move x to an
+# end of the byte range too.
+U8_REGIMES = {"zw0": (0, "unsigned_b", 255), "zw128": (128, "no_cplane", 0), "zw1": (1, "cplane_max", 255),
+              "zw255": (255, "cplane_min", 0)}
+for rg, (zw, ops, zx_end) in U8_REGIMES.items():
+    def _r(edges, **kw):
+        return dict(edges, u8_operands=ops, b_signed=int(zw != 0), cplane=0 if zw in (0, 128) else 128 - zw, **kw)
+    _add(f"gemm1x1_u8_{rg}", _u8(2, 64, 9, 7, 40, zw=zw), G_, _r(dict(b_res=1, n_tiles=1)))
+    _add(f"gemm1x1_u8_{rg}_zx{zx_end}_m2", _u8(2, 64, 9, 7, 40, zw=zw, zx=zx_end, mode=2), G_, _r(dict(zx=zx_end)))
+    _add(f"gemm1x1_u8_{rg}_ocp400", _u8(2, 64, 9, 7, 400, zw=zw), G_, _r(dict(n_tiles=4, n_uneven=True)))
+    _add(f"fc_u8_c24_3x3_{rg}", lambda r, zw=zw: ties.uint8_conv(r, 3, 24, 3, 3, 50, fc=True, zw=zw), G_, _r(dict(k_blocks=3)))
+    _add(f"fc_u8_k4608_{rg}_m2", lambda r, zw=zw: ties.uint8_conv(r, 2, 512, 3, 3, 64, fc=True, mode=2, zw=zw), G_,
+         _r(dict(b_res=0, k_blocks=36)))
+    _add(f"igemm3x3_u8_{rg}_m2", _u8(2, 64, 9, 10, 40, k=3, pad=1, mode=2, zw=zw), I_, _r(dict(border=1, taps=9)))
+    _add(f"igemm7x7_u8_{rg}_m2", _u8(1, 64, 13, 12, 40, k=7, pad=3, mode=2, zw=zw), I_, _r(dict(border=1, taps=49)))
+# every (block_n, mt) of gemm_mma_dispatch on the unsigned-B path: one N tile of OCp = block_n channels; mt 2 over 3 m-tiles, mt 4
+# (block_n <= 32) over 5
+MMA_PAIRS = ((16, 1), (16, 2), (16, 4), (32, 1), (32, 2), (32, 4), (48, 1), (48, 2), (64, 1), (64, 2), (80, 1), (96, 1), (112, 1),
+             (128, 1))
+for bn, mt in MMA_PAIRS:
+    shp = {1: (1, 10, 12), 2: (1, 15, 20), 4: (2, 15, 20)}[mt if bn < 80 else 2]
+    _add(f"gemm1x1_u8_zw0_bn{bn}_mt{mt}", _u8(shp[0], 32, shp[1], shp[2], bn, zw=0), G_,
+         dict(mma_uu=(bn, mt), block_n=bn, mt=mt, b_signed=0, cplane=0))
+# the largest accumulators: |x - zx| = |w - zw| in [235, 255] at K = 4608 (3x3x512, padded) and 25088 (VGG fc6), both operand
+# regimes with a non-zero correction term away from zx = 0: unsigned B (zx 255, zw 0) and cplane -127 (zx 0, zw 255)
+for zx, zw in ((255, 0), (0, 255)):
+    _add(f"igemm3x3_u8_far_z{zx}_{zw}", lambda r, zx=zx, zw=zw: u8_far(r, 1, 512, 10, 10, 64, k=3, pad=1, zx=zx, zw=zw, s_out=16.0),
+         I_, dict(k_blocks=36, border=1, zx=zx, b_signed=int(zw != 0)), ref="oracle", ties=False)
+    _add(f"fc_u8_far_z{zx}_{zw}", lambda r, zx=zx, zw=zw: u8_far(r, 2, 512, 7, 7, 64, fc=True, zx=zx, zw=zw, s_out=32.0),
+         G_, dict(k_blocks=196, b_res=0, zx=zx, b_signed=int(zw != 0)), ref="oracle", ties=False)
+# zx = 255: the window and gather kernels fill out-of-image taps with 0xFF, the implicit GEMM's border table holds its largest
+# corrections; zx = 0 likewise
+for zx in (0, 255):
+    _add(f"win3x3s1_u8_c3_zx{zx}", _u8(2, 3, 15, 32, 24, k=3, pad=1, zx=zx), WI, dict(layout=0, zx=zx))
+    _add(f"win7x7s2_u8_c3_zx{zx}", _u8(2, 3, 21, 32, 24, k=7, stride=2, pad=3, zx=zx), WI, dict(layout=1, zx=zx))
+    _add(f"win3x3s1_u8_c16_zx{zx}", _u8(3, 16, 10, 20, 40, k=3, pad=1, zx=zx), WI, dict(layout=2, zx=zx))
+    _add(f"win3x3s2_u8_c24_zx{zx}", _u8(3, 24, 9, 20, 40, k=3, stride=2, pad=1, zx=zx), WI, dict(layout=3, zx=zx))
+    _add(f"gat3x3s1_u8_c3_zx{zx}", _u8(2, 3, 14, 30, 24, k=3, pad=1, zx=zx), GA, dict(ks=1, zx=zx, window_valid=False))
+    _add(f"gat7x7s2_u8_c3_zx{zx}", _u8(2, 3, 16, 24, 40, k=7, stride=2, pad=3, zx=zx), GA, dict(ks=5, zx=zx, window_valid=False))
+    _add(f"igemm3x3_u8_zx{zx}_m2", _u8(2, 64, 9, 10, 40, k=3, pad=1, mode=2, zx=zx), I_, dict(border=1, zx=zx))
+    _add(f"direct3x3_u8_c32_notc_zx{zx}", _u8(2, 32, 7, 9, 32, k=3, pad=1, zx=zx), DR, dict(oct=8, zx=zx), flags=NO_TC)
+    _add(f"dw3x3s1_u8_c32_zx{zx}", _u8(2, 32, 9, 11, 32, k=3, pad=1, group=32, zx=zx), DD, dict(dw_kernel="generic", zx=zx))
+    _add(f"dw3x3s2_u8_c32_zx{zx}", _u8(2, 32, 9, 11, 32, k=3, stride=2, pad=1, group=32, zx=zx), DD, dict(dw_kernel="generic", zx=zx))
+    _add(f"direct3x3d2_u8_c32_zx{zx}", lambda r, zx=zx: u8_conv_pad(r, 2, 32, 12, 16, 24, 3, 1, 2, dilation=2, zx=zx), DR,
+         dict(oct=8, zx=zx))
+# output zero points 0 and 255 under every activation: make_epi saturates the clamp's bounds before it builds the fast
+# epilogue's constants.  t about t_mid; at zo 255 the ReLU-type clamps leave only t <= 0.5, so every byte is 255 (no live ties)
+_ZO_ACTS = dict(ACTS, none=(-1, abi.RECIPE_HCL, 1.0))
+_ZO_SHAPES = {"gemm1x1": (G_, (2, 64, 9, 7, 40, 1, 1, 0, 1)), "win3x3": (WI, (2, 3, 9, 32, 24, 3, 1, 1, 1)),
+              "direct3x3": (DR, (2, 32, 7, 9, 32, 3, 1, 1, 4))}
+for sh, (kern, (n, c, h, w, oc, k, st, pd, gp)) in _ZO_SHAPES.items():
+    for a, (act, rec, so) in _ZO_ACTS.items():
+        for zo in (0, 255):
+            t_mid = {"none": 20.0 if zo == 0 else -20.0, "ref1": 0.0}.get(a, 0.75)
+            dense = zo == 0 or a in ("none", "ref1")
+            _add(f"{sh}_u8_{a}_zo{zo}", lambda r, act=act, rec=rec, so=so, zo=zo, t_mid=t_mid, n=n, c=c, h=h, w=w, oc=oc, k=k, st=st,
+                 pd=pd, gp=gp: act_conv(r, True, n, c, h, w, oc, act, rec, so, k=k, stride=st, pad=pd, group=gp, zo=zo, t_mid=t_mid),
+                 kern, dict(act=a, zo=zo), ties=dense, notes={} if dense else dict(constant_output=True))
+# glue ops at the ends of the byte range
+_PW, _CR, _LUT = "pointwise", "concat_requant", "byte_lut"
+# uint8 pooling has no lower clamp: below 0 (zo < zi) the result wraps
+_add("avgpool2x2s2_u8_wrap", lambda r: ties.pool(r, True, abi.POOL_AVG, 2, 2, zi=255, zo=0), _P, dict(pool_wraps=True, zx=255, zo=0))
+_add("maxpool3x3s2_u8_wrap", lambda r: ties.pool(r, True, abi.POOL_MAX, 3, 2, pad=1, scale_ratio=2, zi=255, zo=0, shape=(2, 20, 9, 10)),
+     _P, dict(pool_wraps=True, zx=255, zo=0))
+_add("avgpool2x2s2_u8_zi0", lambda r: ties.pool(r, True, abi.POOL_AVG, 2, 2, zi=0, zo=60), _P, dict(pool_wraps=False, zx=0))
+_add("maxpool2x3s1_u8_zi255", lambda r: ties.pool(r, True, abi.POOL_MAX, (2, 3), 1, scale_ratio=2, zi=255, zo=255), _P,
+     dict(pool_wraps=False, zx=255))
+# ReLU and leaky ReLU with zi 255 (every input at or below the zero point) or zo 0
+_add("relu_u8_zi255", lambda r: ties.relu(r, True, zi=255, zo=110), _PW, dict(zx=255), ties=False)
+_add("relu_u8_zo0", lambda r: ties.relu(r, True, zi=128, zo=0), _PW, dict(zo=0))
+_add("leaky_relu_u8_zi255", lambda r: ties.relu(r, True, slope_exp=1, zi=255, zo=110), _PW, dict(zx=255))
+_add("leaky_relu_u8_zo0", lambda r: ties.relu(r, True, slope_exp=2, zi=128, zo=0), _PW, dict(zo=0))
+# eltwise sum and product with zero points 0 and 255, and with the folded ReLU
+_add("eltwise_sum_u8_z0_255_zo0", lambda r: ties.eltwise(r, True, abi.ELT_SUM, z0=0, z1=255, zo=0), _PW, dict(zx=0, zo=0))
+_add("eltwise_sum_u8_z255_0_zo255", lambda r: ties.eltwise(r, True, abi.ELT_SUM, z0=255, z1=0, zo=255), _PW, dict(zx=255, zo=255))
+_add("eltwise_prod_u8_z0_255_zo255", lambda r: ties.eltwise(r, True, abi.ELT_PROD, z0=0, z1=255, zo=255), _PW, dict(zx=0, zo=255))
+_add("eltwise_prod_u8_z255_255_zo0", lambda r: ties.eltwise(r, True, abi.ELT_PROD, z0=255, z1=255, zo=0), _PW, dict(zx=255, zo=0))
+_add("eltwise_relu_u8_z0_255_zo0", lambda r: eltwise_relu(r, True, 32, z0=0, z1=255, zo=0), _F, dict(zx=0, zo=0), layer=1, fused=True,
+     tie_layer=0)
+_add("eltwise_prod_relu_u8_z255_255_zo0", lambda r: eltwise_relu(r, True, 32, z0=255, z1=255, zo=0, elt=abi.ELT_PROD), _F,
+     dict(zx=0, zo=0), layer=1, fused=True, tie_layer=0)
+# concat through the byte table and the bytewise kernel, zero points 0 and 255 in and out; an input with the output's quantisation
+# takes the table path without a table (a copy)
+for z in (0, 255):
+    _add(f"concat4_u8_z{z}", lambda r, z=z: concat_n(r, True, (16, 8, 24, 16), zps=(z,) * 4, zo=z), _CR, dict(mixed=True, zx=z, zo=z))
+    _add(f"concat3_aligned_u8_z{z}", lambda r, z=z: concat_n(r, True, (16, 32, 16), zps=(z,) * 3, zo=z), _CR, dict(mixed=False, zx=z, zo=z))
+_add("concat2_aligned_u8_copy_z255", lambda r: concat_n(r, True, (16, 32), zps=(255, 255), zo=255, ratios=(1, 0.5)), _CR,
+     dict(mixed=False, zx=255, zo=255))
+# the ReLU folded into max pooling as a table, at zo 255: a plain ReLU saturates every byte, a leaky one keeps its negative side
+_add("relu_maxpool_u8_c32_zo255", lambda r: relu_maxpool(r, True, 32, zi=128, zo=255), _F, dict(zo=255), fused=True, tie_layer=0,
+     ties=False)
+_add("leaky_relu_maxpool_u8_c32_zi255_zo255", lambda r: relu_maxpool(r, True, 32, slope_exp=1, zi=255, zo=255), _F,
+     dict(zx=255, zo=255), fused=True, tie_layer=0)
+# byte tables and softmax over inputs at zi 255
+_add("sigmoid_u8_c24_zi255", lambda r: unary(r, True, "sigmoid", 24, zi=255), _LUT, dict(zx=255), ref="oracle", ties=False)
+_add("hardswish_u8_c24_zi255", lambda r: unary(r, True, "hardswish", 24, zi=255, zo=128), _LUT, dict(zx=255), ref="oracle",
+     ties=False)
+_add("softmax_c21_5x6_u8_zi255", lambda r: softmax(r, True, 21, 5, 6, zi=255), "softmax", dict(zx=255), ref="oracle", ties=False)
+
+# ---- int8 -128 in a graph input: the reference clamps it to -127 in every op, its concat to +127 (concat_kernel_ref_int8.c:77-78) ----
+_M = dict(in_min_byte=True)
+# concat: an input with the output's quantisation (the table path's copy), the bytewise kernel at the same scale, and rescaled
+_add("concat2_aligned_i8_copy", lambda r: concat_n(r, False, (16, 32), ratios=(1, 0.5)), _CR, dict(in_min_byte=False, mixed=False))
+_add("concat2_aligned_i8_copy_min", lambda r: concat_n(r, False, (16, 32), ratios=(1, 0.5), min_byte=True), _CR, dict(_M, mixed=False))
+_add("concat2_i8_bytewise_same_min", lambda r: concat_n(r, False, (8, 24), ratios=(1, 1), min_byte=True), _CR, dict(_M, mixed=False),
+     ties=False)
+_add("concat3_i8_min", lambda r: concat_n(r, False, (32, 40, 16), min_byte=True), _CR, dict(_M, mixed=True))
+# pooling: max at the same scale (the byte path), max rescaled, average
+_add("maxpool3x3s2_i8_same_min", lambda r: ties.pool(r, False, abi.POOL_MAX, 3, 2, pad=1, shape=(2, 32, 9, 10), min_byte=True), _P,
+     dict(_M), ties=False)
+_add("maxpool2x3s1_i8_min", lambda r: ties.pool(r, False, abi.POOL_MAX, (2, 3), 1, scale_ratio=2, min_byte=True), _P, dict(_M))
+_add("avgpool2x2s2_i8_min", lambda r: ties.pool(r, False, abi.POOL_AVG, 2, 2, min_byte=True), _P, dict(_M))
+# ReLU at the same scale, leaky ReLU, eltwise sum and product, sigmoid (int8 has no hardswish in the reference), softmax, upsample
+_add("relu_same_i8_min", lambda r: relu_same(r, 32), _PW, dict(_M), ties=False)
+_add("leaky_relu_i8_min", lambda r: ties.relu(r, False, slope_exp=2, min_byte=True), _PW, dict(_M))
+_add("eltwise_sum_i8_min", lambda r: ties.eltwise(r, False, abi.ELT_SUM, min_byte=True), _PW, dict(_M))
+_add("eltwise_prod_i8_min", lambda r: ties.eltwise(r, False, abi.ELT_PROD, min_byte=True), _PW, dict(_M))
+_add("sigmoid_i8_c24_min", lambda r: unary(r, False, "sigmoid", 24, min_byte=True), _LUT, dict(_M), ref="oracle", ties=False)
+_add("softmax_c21_5x6_i8_min", lambda r: softmax(r, False, 21, 5, 6, min_byte=True), "softmax", dict(_M), ref="oracle", ties=False)
+_add("upsample2_c24_i8_min", lambda r: upsample(r, False, 24, 2, min_byte=True), "upsample_nearest", dict(_M), ref="oracle", ties=False)
+# convolutions reading the graph input: the stem's window and gather kernels, the GEMM on its NHWC copy, the depthwise kernels
+_add("win3x3s1_i8_c3_min", _i8(2, 3, 15, 32, 24, k=3, pad=1, min_byte=True), WI, dict(_M, layout=0))
+_add("gat3x3s1_i8_c3_min", _i8(2, 3, 14, 30, 24, k=3, pad=1, min_byte=True), GA, dict(_M, window_valid=False))
+_add("gemm1x1_i8_min", _i8(2, 64, 9, 7, 40, mode=1, min_byte=True), G_, dict(_M))
+_add("dw3x3s1_i8_c32_min", _i8(2, 32, 9, 10, 32, k=3, pad=1, group=32, min_byte=True), D_, dict(_M, valid=True))
+_add("dw5x5s1_i8_c32_min", _i8(2, 32, 9, 11, 32, k=5, pad=2, group=32, min_byte=True), DD, dict(_M, dw_kernel="generic"))
+
 # Boundaries: geometry key -> the values that must each be reached by some entry (both sides of every edge)
 BOUNDARIES = {
     "par_all": {0, 1},
@@ -772,6 +1000,13 @@ BOUNDARIES = {
     "act": {"hcl0", "hcl6", "ref1", "ref6"},
     "bound_half": {True, False},
     "bound_beyond_sat": {True, False},
+    # the ends of the byte range
+    "u8_operands": {"unsigned_b", "no_cplane", "cplane_max", "cplane_min"},
+    "mma_uu": set(MMA_PAIRS),
+    "zx": {0, 255},
+    "zo": {0, 255},
+    "pool_wraps": {True, False},
+    "in_min_byte": {True, False},
 }
 
 # Edges no graph can reach, and why (none so far).
@@ -784,6 +1019,22 @@ def gemm_entries():
 
 def uint8_gemm_entries():
     return [n for n in gemm_entries() if "_u8_" in n or n.startswith("fc_u8")]
+
+
+def negative_control_entries():
+    """The uint8 GEMM entries whose output is not one constant byte (a saturated output cannot show a wrong accumulator), and
+    whether the restated plan has a cplane term: without it (TB200_DEBUG_NO_CPLANE) exactly those with one must fail."""
+    out = {}
+    for n in uint8_gemm_entries():
+        if ENTRIES[n].notes.get("constant_output"):
+            continue
+        case = build(n)
+        out[n] = gemm_geometry_of(case, ENTRIES[n])["cplane"] != 0
+    return out
+
+
+def gemm_geometry_of(case, e):
+    return geometry(case.g, case.g.layers[e.layer])
 
 
 def window_entries():

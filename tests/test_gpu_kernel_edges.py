@@ -4,8 +4,8 @@ ops outside ties.exact_layer), with the kernel each entry is meant to reach asse
 Child processes (`python -m tests.test_gpu_kernel_edges <entry>...`) cover what the library reads once per process:
   - TB200_DEBUG_LAUNCH: the printed plans of the GEMM, the window and the gather kernel equal kernel_edges.gemm_geometry,
     window_geometry and gather_geometry for every entry of theirs, so the Python restatement cannot drift from the code unnoticed;
-  - TB200_DEBUG_NO_CPLANE (documented to give wrong uint8 results): the uint8 GEMM entries must FAIL there -- a sweep that passed
-    under a known-wrong kernel would prove nothing."""
+  - TB200_DEBUG_NO_CPLANE (documented to give wrong uint8 results): the uint8 GEMM entries with a cplane term must FAIL there --
+    a sweep that passed under a known-wrong kernel would prove nothing -- and those without one (zw 0 or 128) must pass."""
 import os
 import re
 import subprocess
@@ -75,14 +75,14 @@ def _child(names, env, timeout=900):
 
 
 _LAUNCH = re.compile(r"tengine_b200: launch gemm_i8_tcgen05_kernel<U8=(\d),MODE=(\d),CS=(\d),BORDER=(\d)> out_mode=(\d+) conv=(\d) "
-                     r"n_tiles=(\d+) b_res=(\d) fixq=\d mt=(\d) par_all=(\d)")
+                     r"n_tiles=(\d+) b_res=(\d) fixq=\d mt=(\d) par_all=(\d) block_n=(\d+) b_signed=(\d) cplane=(-?\d+)")
 
 
 def test_gemm_plan_equals_restatement():
     names = ke.gemm_entries()
     r = _child(names, {"TB200_DEBUG_LAUNCH": "1"})
     assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
-    printed, cur = {}, None
+    printed, cur, uu = {}, None, set()
     for line in r.stderr.splitlines():
         if line.startswith(MARK):
             cur = line[len(MARK):].strip()
@@ -95,11 +95,16 @@ def test_gemm_plan_equals_restatement():
         case = ke.build(name)
         geo = ke.geometry(case.g, case.g.layers[ke.ENTRIES[name].layer])
         want = (geo["cs"], geo["border"], geo["out_mode"], int(geo["kind"] == "igemm"), geo["n_tiles"], geo["b_res"], geo["mt"],
-                geo["par_all"])
+                geo["par_all"], geo["block_n"], geo["b_signed"], geo["cplane"])
         got = [(p[2],) + p[3:] for p in printed.get(name, [])]
         if not got or any(x != want for x in got):
-            bad.append(f"{name}: printed (cs, border, out_mode, conv, n_tiles, b_res, mt, par_all) {got}, restated {want}")
+            bad.append(f"{name}: printed (cs, border, out_mode, conv, n_tiles, b_res, mt, par_all, block_n, b_signed, cplane) {got}, "
+                       f"restated {want}")
+        elif geo.get("mma_uu"):
+            uu.add((got[0][8], got[0][6]))
     assert not bad, "\n".join(bad)
+    # the u8.u8 MMA (B unsigned: zw 0) ran in every (block_n, mt) instantiation of gemm_mma_dispatch
+    assert uu == set(ke.MMA_PAIRS), sorted(set(ke.MMA_PAIRS) - uu)
 
 
 _WINDOW = re.compile(r"tengine_b200: launch conv_window_tc_kernel<MODE=\d,U8=\d,LAYOUT=(\d)> layout=(\d) xoff=(\d+) box_w=(\d+) box_h=(\d+) "
@@ -166,12 +171,20 @@ def test_window_entry_on_part_of_the_batch(ctx, name):
 
 
 def test_negative_control_without_the_uint8_correction():
-    """TB200_DEBUG_NO_CPLANE drops the cplane * sum(x) term of the uint8 tensor-core kernels: every uint8 GEMM entry must fail."""
-    names = ke.uint8_gemm_entries()
+    """TB200_DEBUG_NO_CPLANE drops the cplane * sum(x) term of the uint8 tensor-core kernels: every uint8 GEMM entry with a
+    cplane term (zw not 0 or 128) must fail, and every one without it must still pass (entries whose output is one saturated
+    byte cannot show it and are left out)."""
+    want = ke.negative_control_entries()
+    names = list(want)
     r = _child(names, {"TB200_DEBUG_NO_CPLANE": "1"})
     assert r.returncode == 1, r.stdout[-3000:] + r.stderr[-3000:]
-    failed = [ln for ln in r.stdout.splitlines() if ln.startswith("FAIL ")]
-    assert len(failed) == len(names), r.stdout
+    status = {}
+    for ln in r.stdout.splitlines():
+        if ln.startswith("ok "):
+            status[ln[3:].strip()] = False
+        elif ln.startswith("FAIL "):
+            status[ln[5:].split(":", 1)[0]] = True
+    assert status == want, {n: (status.get(n), want[n]) for n in names if status.get(n) != want[n]}
 
 
 def _main(names):

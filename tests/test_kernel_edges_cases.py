@@ -13,7 +13,7 @@ NAMES = list(ke.ENTRIES)
 def _geometry(name):
     e = ke.ENTRIES[name]
     case = ke.build(name)
-    return e, case, ke.geometry(case.g, case.g.layers[e.layer], no_tc=bool(e.flags & ke.abi.PRERUN_NO_TENSORCORE))
+    return e, case, ke.reached(case, e)
 
 
 @pytest.mark.parametrize("name", NAMES)
@@ -88,3 +88,40 @@ def test_gemm_entries_are_listed():
     assert len(ke.gemm_entries()) >= 30
     u8 = ke.uint8_gemm_entries()
     assert u8 and all(ke.build(n).g.data_type == ke.abi.DT_UINT8 for n in u8)
+
+
+FAR = [n for n in NAMES if "_far_" in n]
+
+
+@pytest.mark.parametrize("name", FAR)
+def test_far_end_entries_leave_the_exact_reference(oracle, name):
+    """|x - zx| = |w - zw| near 255 puts the accumulator past 2^24, where the reference rounds it to fp32 before it scales it:
+    ties.exact_layer refuses the layer instead of disagreeing quietly, and the oracle's outputs still spread."""
+    case = ke.build(name)
+    assert case.notes["acc_max"] >= 255 ** 2 * 4608 * 0.8, case.notes
+    with pytest.raises(AssertionError, match="2\\^24"):
+        ties.exact_run(case.g, case.inputs)
+    out = oracle.run(case.g, case.inputs, uint8_mode=0)[case.g.outputs[0]]
+    assert len(np.unique(out)) >= 16, np.unique(out)
+
+
+def test_large_accumulator_entries_are_listed():
+    """At K = 4608 and 25088, with both uint8 operand regimes that carry a correction term."""
+    assert {ke.ENTRIES[n].edges["k_blocks"] for n in FAR} == {36, 196}
+    assert {ke.ENTRIES[n].edges["b_signed"] for n in FAR} == {0, 1}
+
+
+def test_negative_control_splits_on_cplane():
+    """The uint8 GEMM entries of the GPU negative control: some with a cplane term (they must fail without it), some without
+    (zw 0 or 128: they must pass); an entry left out has one output byte only, by its exact reference."""
+    nc = ke.negative_control_entries()
+    assert any(nc.values()) and not all(nc.values())
+    assert {ke.gemm_geometry_of(ke.build(n), ke.ENTRIES[n])["u8_operands"] for n, c in nc.items() if not c} == {"unsigned_b", "no_cplane"}
+    for n in ke.uint8_gemm_entries():
+        case = ke.build(n)
+        if ke.ENTRIES[n].ref != "exact":
+            assert n in nc
+            continue
+        want, _ = ties.exact_run(case.g, case.inputs)
+        constant = len(np.unique(want[case.g.outputs[0]])) == 1
+        assert constant == (n not in nc), (n, constant)

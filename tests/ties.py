@@ -138,6 +138,16 @@ def _pool_windows(L, H, W, OH, OW):
     return out
 
 
+ACC_EXACT = 2 ** 24  # below it an integer is exact in fp32
+
+
+def _check_acc_exact(acc, b):
+    """The reference casts the accumulator and the bias to float before it scales them (tb200_oracle.c conv / fc, common.cuh
+    requant); the float64 arithmetic here equals that only while |acc|, |bias| and |acc + bias| are below 2^24."""
+    worst = max(int(np.abs(acc).max(initial=0)), int(np.abs(b).max(initial=0)), int(np.abs(acc + b).max(initial=0)))
+    assert worst < ACC_EXACT, f"exact reference: |accumulator / bias| reaches {worst} >= 2^24, where fp32 rounds it"
+
+
 def exact_layer(g, L, bufs):
     """Rounding step of layer L (a dict of g.layers) given the int8/uint8 arrays of its inputs in `bufs` (tensor id -> array)."""
     u8 = g.data_type == abi.DT_UINT8
@@ -163,6 +173,7 @@ def exact_layer(g, L, bufs):
             acc = conv_acc(x, L["weight"], L, zi if u8 else 0, L["weight_zero"] if u8 else 0)
         oc = acc.shape[1]
         b = (L["bias"].astype(np.int64) if L["bias"] is not None else np.zeros(oc, np.int64)).reshape(1, oc, 1, 1)
+        _check_acc_exact(acc, b)
         if not u8:
             sw = ws.reshape(1, oc, 1, 1)
             if op == abi.OP_FC:
@@ -268,6 +279,7 @@ def planned_mode(g, L):
 M_EXPS = (1, 1, 1, 2, 2, 3, 4, 5, 6, 7, 8)
 S_IN, S_OUT = 2.0 ** -4, 2.0 ** -6
 X_MAX = 15  # int8 inputs in [-15, 15]
+MIN_BYTE_FRAC = 1 / 16  # min_byte: the share of int8 input bytes set to -128
 
 
 @dataclass
@@ -309,10 +321,10 @@ def _int8_bias(rng, oc, m, mode):
 
 
 def int8_conv(rng, n, c, h, w, oc, k=1, stride=1, pad=0, group=1, activation=-1, recipe=abi.RECIPE_HCL, mode=1, name=None,
-              x_max=X_MAX, m_exps=M_EXPS):
+              x_max=X_MAX, m_exps=M_EXPS, min_byte=False):
     """mode 1: fused bias; 0: one channel with |bias*M| > 100; 2: channel 0 is "hot" (weights +-127 at M = 2^-1: the
     clamp-range bound passes 32000 and the layer takes the exact epilogue; that channel saturates, the rest do not).
-    m_exps: the exponents m of M_c = 2^-m dealt to the channels in turn."""
+    m_exps: the exponents m of M_c = 2^-m dealt to the channels in turn.  min_byte: -128 in about one input byte in sixteen."""
     g = GraphDef(abi.DT_INT8)
     x = g.input(n, c, h, w, S_IN)
     cg = c // group
@@ -326,6 +338,8 @@ def int8_conv(rng, n, c, h, w, oc, k=1, stride=1, pad=0, group=1, activation=-1,
     y = g.conv(x, wq, b, ws, S_OUT, stride=stride, pad=pad, group=group, activation=activation, recipe=recipe)
     g.mark_output(y)
     xin = rng.integers(-x_max, x_max + 1, (n, c, h, w)).astype(np.int8)
+    if min_byte:
+        xin[rng.random(xin.shape) < MIN_BYTE_FRAC] = -128
     cs = Case(name or f"int8_conv_n{n}c{c}_{h}x{w}_oc{oc}_k{k}s{stride}p{pad}g{group}_a{activation}_r{recipe}_m{mode}", g, [xin])
     cs.mode = planned_mode(g, g.layers[0])
     assert cs.mode == mode, (cs.name, cs.mode)
@@ -358,33 +372,59 @@ def int8_fc(rng, n, k, oc, mode=0, name=None):
 U8_ZX, U8_ZW, U8_ZO = 128, 100, 110
 
 
+def _shift(z, lo, hi):
+    """What moves the byte range [z + lo, z + hi] inside [0, 255]: 0 when it lies there already, so that zero points near either
+    end of the byte range draw their data from the side of the zero point that exists (z = 0: [0, hi - lo])."""
+    return max(0, -(z + lo)) - max(0, z + hi - 255)
+
+
 def uint8_conv(rng, n, c, h, w, oc, k=1, stride=1, pad=0, group=1, activation=-1, recipe=abi.RECIPE_HCL, mode=0, fc=False,
-               name=None, s_out=2.0 ** -5):
+               name=None, s_out=2.0 ** -5, zx=U8_ZX, zw=U8_ZW, zo=U8_ZO):
     """Zero points on input, weights and output; t spans about [-100, 100] around the output zero point, so negative ties are as
-    common as positive ones.  mode 2: channel 0's bias has |bias*M| > 250 (that channel saturates)."""
+    common as positive ones.  mode 2: channel 0's bias has |bias*M| > 250 (that channel saturates).
+    Inputs lie within zx +- 10 and weights within zw +- a, moved inside the byte range when a zero point lies near its end (zx = 0:
+    x in [0, 20]); then sum (x - zx)(w - zw) no longer centres on 0, and the bias takes each channel's mean accumulator off again,
+    so that t stays spread about the output zero point."""
     g = GraphDef(abi.DT_UINT8)
     s_in, s_w = 2.0 ** -4, 2.0 ** -3
     M = s_in * s_w / s_out
-    x = g.input(n, c, h, w, s_in, U8_ZX)
+    x = g.input(n, c, h, w, s_in, zx)
     cg = c // group
     kk = (cg * k * k) if not fc else c * h * w
     a = max(1, min(100, int(round(35.0 / (M * np.sqrt(kk) * 6 * 0.58)))))
-    while a > 1 and 255.0 * kk * a * (a + 1) / (2 * a + 1) * M > 28000:  # keep the clamp-range proof (planned_mode) passing
+
+    def w_abs(a, p=1):  # mean |w - zw|^p over the weights' range
+        d = np.arange(-a, a + 1) + _shift(zw, -a, a)
+        return np.mean(np.abs(d) ** p)
+
+    # keep the clamp-range proof (planned_mode) passing, and t's spread when the weights lie on one side of zw
+    while a > 1 and (255.0 * kk * w_abs(a) * M > 28000 or (_shift(zw, -a, a) and np.sqrt(w_abs(a, 2) * kk) * 6 * M > 40)):
         a -= 1
     shape = (oc, kk) if fc else (oc, cg, k, k)
-    wq = (U8_ZW + rng.integers(-a, a + 1, shape)).astype(np.uint8)
+    wq = (zw + _shift(zw, -a, a) + rng.integers(-a, a + 1, shape)).astype(np.uint8)
     b = (rng.integers(-40, 41, oc) / M + rng.integers(-3, 4, oc)).astype(np.int32)
     if mode == 2:
         b[0] = int(260 / M)
+    xin = (zx + _shift(zx, -10, 10) + rng.integers(-10, 11, (n, c, h, w))).astype(np.uint8)
+    if _shift(zx, -10, 10) or _shift(zw, -a, a):
+        L = dict(group=1 if fc else group, stride_h=stride, stride_w=stride, dilation_h=1, dilation_w=1, pad_h0=pad, pad_h1=pad,
+                 pad_w0=pad, pad_w1=pad)
+        xa, wa = (xin.reshape(n, 1, 1, -1), wq.reshape(oc, 1, 1, -1)) if fc else (xin, wq)
+        if fc:
+            L.update(stride_h=1, stride_w=1, pad_h0=0, pad_h1=0, pad_w0=0, pad_w1=0)
+        mean = np.rint(conv_acc(xa, wa, L, zx, zw).mean(axis=(0, 2, 3)))
+        if mode == 2:
+            mean[0] = 0  # the saturating channel keeps |bias*M| > 250
+        b = (b - mean).astype(np.int32)
     if fc:
-        y = g.fc(x, wq, b, [s_w], s_out, U8_ZO, weight_zero=U8_ZW)
+        y = g.fc(x, wq, b, [s_w], s_out, zo, weight_zero=zw)
     else:
-        y = g.conv(x, wq, b, [s_w], s_out, U8_ZO, stride=stride, pad=pad, group=group, activation=activation, recipe=recipe,
-                   weight_zero=U8_ZW)
+        y = g.conv(x, wq, b, [s_w], s_out, zo, stride=stride, pad=pad, group=group, activation=activation, recipe=recipe,
+                   weight_zero=zw)
     g.mark_output(y)
-    xin = (U8_ZX + rng.integers(-10, 11, (n, c, h, w))).astype(np.uint8)
     kind = "fc" if fc else f"conv_k{k}s{stride}p{pad}g{group}_a{activation}_r{recipe}"
-    cs = Case(name or f"uint8_{kind}_n{n}c{c}_{h}x{w}_oc{oc}_m{mode}", g, [xin])
+    zps = "" if (zx, zw, zo) == (U8_ZX, U8_ZW, U8_ZO) else f"_z{zx}_{zw}_{zo}"
+    cs = Case(name or f"uint8_{kind}_n{n}c{c}_{h}x{w}_oc{oc}_m{mode}{zps}", g, [xin])
     cs.mode = planned_mode(g, g.layers[0])
     assert cs.mode == mode, (cs.name, cs.mode)
     cs.min_tie_frac = 0.05 if activation >= 0 else 0.10
@@ -392,63 +432,71 @@ def uint8_conv(rng, n, c, h, w, oc, k=1, stride=1, pad=0, group=1, activation=-1
 
 
 # ---- glue ops -------------------------------------------------------------------------------------------------------------
-def _in(rng, u8, shape, lo=-60, hi=60, zp=0):
+def _in(rng, u8, shape, lo=-60, hi=60, zp=0, min_byte=False):
+    """Bytes within [lo, hi] about the zero point (uint8: moved inside the byte range, see _shift).  int8 min_byte: about one byte
+    in sixteen becomes -128, which the reference's ops clamp to -127 (its concat to +127)."""
     if u8:
-        return (zp + rng.integers(lo, hi + 1, shape)).astype(np.uint8)
-    return rng.integers(lo, hi + 1, shape).astype(np.int8)
+        return (zp + _shift(zp, lo, hi) + rng.integers(lo, hi + 1, shape)).astype(np.uint8)
+    x = rng.integers(lo, hi + 1, shape).astype(np.int8)
+    if min_byte:
+        x[rng.random(shape) < MIN_BYTE_FRAC] = -128
+    return x
 
 
-def eltwise(rng, u8, elt, shape=(2, 24, 9, 11)):
-    """SUM: t = a + b/2 (ties at odd b); PROD: t = a*b/16 (ties at a*b = 8 mod 16)."""
+def eltwise(rng, u8, elt, shape=(2, 24, 9, 11), z0=120, z1=130, zo=110, min_byte=False):
+    """SUM: t = a + b/2 (ties at odd b); PROD: t = a*b/16 (ties at a*b = 8 mod 16).  z0, z1, zo: the uint8 zero points."""
     g = GraphDef(abi.DT_UINT8 if u8 else abi.DT_INT8)
-    z0, z1, zo = (120, 130, 110) if u8 else (0, 0, 0)
+    z0, z1, zo = (z0, z1, zo) if u8 else (0, 0, 0)
     s0, s1, so = (2.0 ** -4, 2.0 ** -5, 2.0 ** -4) if elt == abi.ELT_SUM else (2.0 ** -3, 2.0 ** -3, 2.0 ** -2)
     a = g.input(*shape, s0, z0)
     b = g.input(*shape, s1, z1)
     g.mark_output(g.eltwise(a, b, so, zo, elt_type=elt))
     r = (-60, 60) if elt == abi.ELT_SUM else (-40, 40)
-    xs = [_in(rng, u8, shape, *r, zp=z0), _in(rng, u8, shape, *r, zp=z1)]
+    xs = [_in(rng, u8, shape, *r, zp=z0, min_byte=min_byte), _in(rng, u8, shape, *r, zp=z1, min_byte=min_byte)]
     name = ("uint8" if u8 else "int8") + "_eltwise_" + ("sum" if elt == abi.ELT_SUM else "prod")
     return Case(name, g, xs, min_tie_frac=0.10 if elt == abi.ELT_SUM else 0.05)
 
 
-def relu(rng, u8, slope_exp=None, shape=(2, 40, 7, 9)):
+def relu(rng, u8, slope_exp=None, shape=(2, 40, 7, 9), zi=128, zo=110, min_byte=False):
     """s_out = 2 s_in: t = x/2 on the positive side (ties at odd x); leaky slope 2^-k: t = x/2^(k+1) below zero.
-    uint8 adds the zero point inside round() (relu_kernel_ref_uint8.c:85)."""
+    uint8 adds the zero point inside round() (relu_kernel_ref_uint8.c:85).  zi, zo: the uint8 zero points."""
     g = GraphDef(abi.DT_UINT8 if u8 else abi.DT_INT8)
-    zi, zo = (128, 110) if u8 else (0, 0)
+    zi, zo = (zi, zo) if u8 else (0, 0)
     x = g.input(*shape, 2.0 ** -5, zi)
     slope = 0.0 if slope_exp is None else 2.0 ** -slope_exp
     g.mark_output(g.relu(x, 2.0 ** -4, zo, negative_slope=slope))
-    xs = [_in(rng, u8, shape, -100, 100, zp=zi)]
+    xs = [_in(rng, u8, shape, -100, 100, zp=zi, min_byte=min_byte)]
     name = ("uint8" if u8 else "int8") + ("_relu" if slope_exp is None else f"_leaky_relu_2^-{slope_exp}")
     return Case(name, g, xs, min_tie_frac=0.20)
 
 
-def pool(rng, u8, method, kernel, stride, pad=0, caffe=0, global_pool=False, shape=(2, 20, 8, 10), scale_ratio=1):
+def pool(rng, u8, method, kernel, stride, pad=0, caffe=0, global_pool=False, shape=(2, 20, 8, 10), scale_ratio=1, zi=128, zo=100,
+         min_byte=False):
     """Average pooling over power-of-two window areas (every divisor, also at padded borders, is 1, 2 or 4 for 2x2 windows; global
-    pooling over 4x4 with s_out = s_in/4: t = sum/4); max pooling with s_out = 2 s_in (t = max/2)."""
+    pooling over 4x4 with s_out = s_in/4: t = sum/4); max pooling with s_out = 2 s_in (t = max/2).  zi, zo: the uint8 zero points
+    (below zo - zi the uint8 result wraps: the reference has no lower clamp)."""
     g = GraphDef(abi.DT_UINT8 if u8 else abi.DT_INT8)
-    zi, zo = (128, 100) if u8 else (0, 0)
+    zi, zo = (zi, zo) if u8 else (0, 0)
     x = g.input(*shape, 2.0 ** -4, zi)
     so = 2.0 ** -4 * scale_ratio
     y = g.pool(x, method, kernel, stride, pad, out_scale=so, out_zero=zo, global_pool=global_pool, caffe_flavor=caffe)
     g.mark_output(y)
-    xs = [_in(rng, u8, shape, -90, 90, zp=zi)]
+    xs = [_in(rng, u8, shape, -90, 90, zp=zi, min_byte=min_byte)]
     name = (("uint8" if u8 else "int8") + ("_maxpool" if method == abi.POOL_MAX else "_avgpool") +
             (f"_global{shape[2]}x{shape[3]}" if global_pool else f"_k{kernel}s{stride}p{pad}_caffe{caffe}") + f"_r{scale_ratio}")
     return Case(name, g, xs, min_tie_frac=0.10)
 
 
-def concat(rng, u8, shape=(2, 16, 6, 7), c2=32):
-    """Two inputs with s_in / s_out = 1/2 and 1/4 (t = q/2, q/4)."""
+def concat(rng, u8, shape=(2, 16, 6, 7), c2=32, z0=120, z1=135, zo=110, min_byte=False):
+    """Two inputs with s_in / s_out = 1/2 and 1/4 (t = q/2, q/4).  z0, z1, zo: the uint8 zero points."""
     g = GraphDef(abi.DT_UINT8 if u8 else abi.DT_INT8)
-    z0, z1, zo = (120, 135, 110) if u8 else (0, 0, 0)
+    z0, z1, zo = (z0, z1, zo) if u8 else (0, 0, 0)
     n, c, h, w = shape
     a = g.input(n, c, h, w, 2.0 ** -5, z0)
     b = g.input(n, c2, h, w, 2.0 ** -6, z1)
     g.mark_output(g.concat([a, b], 2.0 ** -4, zo))
-    xs = [_in(rng, u8, (n, c, h, w), -100, 100, zp=z0), _in(rng, u8, (n, c2, h, w), -100, 100, zp=z1)]
+    xs = [_in(rng, u8, (n, c, h, w), -100, 100, zp=z0, min_byte=min_byte), _in(rng, u8, (n, c2, h, w), -100, 100, zp=z1,
+                                                                              min_byte=min_byte)]
     return Case(("uint8" if u8 else "int8") + f"_concat_c{c}_{c2}", g, xs, min_tie_frac=0.10)
 
 
