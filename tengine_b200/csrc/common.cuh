@@ -240,45 +240,54 @@ __device__ __forceinline__ uint32_t requant_fast4_i8(const int32_t (&acc)[4], co
     return __byte_perm(p01, p23, 0x6420);
 }
 
-// Eight consecutive channels, instruction order pinned stage by stage (asm volatile keeps its order): the four channel
-// pairs advance through the dependent chain fma -> +MAGIC -> -MAGIC -> t-(..) together, so every instruction has three
-// independent neighbours.  ptxas on its own schedules the chains one after the other, and with only four epilogue warps
-// per scheduler the fixed-latency stalls then halve the issue rate (ncu: stall_wait 2.2 per issue).
-// w0/w1: the two packed words (before requant_byte_fix); g0/g1: max |d| of each word for the tie guard.
-template <bool FUSE>
-__device__ __forceinline__ void requant_fast8_i8(const int32_t (&a)[8], const float4 (&p)[4], const EpiParams& e, uint32_t& w0, uint32_t& w1,
-                                                 float& g0, float& g1)
+// N words of four consecutive channels each, instruction order written stage by stage: the 2N channel pairs advance
+// through the dependent chain fma -> +MAGIC -> -MAGIC -> t-(..) together, so every instruction has 2N-1 independent
+// neighbours.  ptxas on its own schedules the chains one after the other, and with only two epilogue warps per scheduler
+// the fixed-latency stalls then dominate.  Word j uses the constants f[j] (NP == N) or all words share f[0] (NP == 1: one
+// lane walking one channel word down several rows).
+// w[j]: the packed word (before requant_byte_fix); g[j]: max |d| of word j for the tie guard.
+template <bool FUSE, int N, int NP>
+__device__ __forceinline__ void requant_fast_words_i8(const int32_t (&a)[N][4], const FastPar4 (&f)[NP], const EpiParams& e, uint32_t (&w)[N],
+                                                      float (&g)[N])
 {
+    static_assert(NP == 1 || NP == N, "one constant set per word, or one for all");
     const uint64_t mg = f2_pack(TB200_MAGIC, TB200_MAGIC);
-    uint64_t x[4], t[4], r[4], s[4], d[4];
+    uint64_t x[2 * N], t[2 * N], r[2 * N], s[2 * N], d[2 * N];
+    // pair k: word k / 2, channels 2 (k & 1) + {0, 1} of it, constants p(k)
+    auto p = [&](int k) -> const float4& { const FastPar4& fp = f[NP == 1 ? 0 : k >> 1]; return (k & 1) ? fp.b : fp.a; };
 #pragma unroll
-    for (int k = 0; k < 4; k++)
+    for (int k = 0; k < 2 * N; k++)
     {
-        const int32_t a0 = FUSE ? a[2 * k] : a[2 * k] + __float_as_int(p[k].z), a1 = FUSE ? a[2 * k + 1] : a[2 * k + 1] + __float_as_int(p[k].w);
+        const int32_t* ak = &a[k >> 1][2 * (k & 1)];
+        const int32_t a0 = FUSE ? ak[0] : ak[0] + __float_as_int(p(k).z), a1 = FUSE ? ak[1] : ak[1] + __float_as_int(p(k).w);
         x[k] = f2_pack((float)a0, (float)a1);
     }
 #pragma unroll
-    for (int k = 0; k < 4; k++)
+    for (int k = 0; k < 2 * N; k++)
     {
-        if (FUSE) t[k] = f2_fma(x[k], f2_pack(p[k].x, p[k].y), f2_pack(p[k].z, p[k].w));
-        else t[k] = f2_mul(x[k], f2_pack(p[k].x, p[k].y));
+        if (FUSE) t[k] = f2_fma(x[k], f2_pack(p(k).x, p(k).y), f2_pack(p(k).z, p(k).w));
+        else t[k] = f2_mul(x[k], f2_pack(p(k).x, p(k).y));
     }
 #pragma unroll
-    for (int k = 0; k < 4; k++) r[k] = f2_add(t[k], mg);
+    for (int k = 0; k < 2 * N; k++) r[k] = f2_add(t[k], mg);
 #pragma unroll
-    for (int k = 0; k < 4; k++) s[k] = f2_sub(r[k], mg);
+    for (int k = 0; k < 2 * N; k++) s[k] = f2_sub(r[k], mg);
 #pragma unroll
-    for (int k = 0; k < 4; k++) d[k] = f2_sub(t[k], s[k]);
-    float dl[4], dh[4];
-    uint32_t rl[4], rh[4];
+    for (int k = 0; k < 2 * N; k++) d[k] = f2_sub(t[k], s[k]);
 #pragma unroll
-    for (int k = 0; k < 4; k++) f2_unpack(d[k], dl[k], dh[k]), f2_unpack_bits(r[k], rl[k], rh[k]);
-    g0 = fmaxf(fmaxf(fabsf(dl[0]), fabsf(dh[0])), fmaxf(fabsf(dl[1]), fabsf(dh[1])));
-    g1 = fmaxf(fmaxf(fabsf(dl[2]), fabsf(dh[2])), fmaxf(fabsf(dl[3]), fabsf(dh[3])));
-    uint32_t q[4];
+    for (int j = 0; j < N; j++)
+    {
+        float dl[2], dh[2];
+        uint32_t rl[2], rh[2], q[2];
 #pragma unroll
-    for (int k = 0; k < 4; k++) q[k] = __viaddmin_s16x2_relu(__byte_perm(rl[k], rh[k], 0x5410), e.q_add2, e.q_max2);
-    w0 = __byte_perm(q[0], q[1], 0x6420), w1 = __byte_perm(q[2], q[3], 0x6420);
+        for (int h = 0; h < 2; h++)
+        {
+            f2_unpack(d[2 * j + h], dl[h], dh[h]), f2_unpack_bits(r[2 * j + h], rl[h], rh[h]);
+            q[h] = __viaddmin_s16x2_relu(__byte_perm(rl[h], rh[h], 0x5410), e.q_add2, e.q_max2);
+        }
+        g[j] = fmaxf(fmaxf(fabsf(dl[0]), fabsf(dh[0])), fmaxf(fabsf(dl[1]), fabsf(dh[1])));
+        w[j] = __byte_perm(q[0], q[1], 0x6420);
+    }
 }
 
 // bytes += q_byte_add (mod 256, no carries between bytes): only layers whose lower clamp is not 0 (warp-uniform test)

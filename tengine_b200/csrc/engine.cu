@@ -423,7 +423,7 @@ static EpiParams make_epi(const tb200_layer_desc& L, const tb200_tensor_desc& ti
     {
         e.fast_lo = (float)(0 - tout.zero_point), e.fast_hi = (float)(255 - tout.zero_point);
         e.fast_r = 1.0f / so;
-        // integer-domain clip + zero point + saturation (common.cuh requant_fast8_i8, the int8 form the uint8 tensor-core epilogues
+        // integer-domain clip + zero point + saturation (common.cuh requant_fast_words_i8, the int8 form the uint8 tensor-core epilogues
         // use): the activation bounds become the integers the reference's own division and round() give for them;
         // q' = max(min(q + zp - L, H - L), 0), byte = q' + L
         int q_lo = -30000, q_hi = 30000;

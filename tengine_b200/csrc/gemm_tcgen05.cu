@@ -17,14 +17,16 @@
 //                   32-row quarter q is written by two MMA warps as soon as its two epilogue warps have read the previous stage
 //                   out of it (mbarriers img_empty[q] / img_full[q]), so no warp waits for the whole CTA at the hand-over.
 //   WG2-3, warps 8-15: epilogue.  Two warps per 32-row quarter of the image; a warp owns whole "store groups" = 32 rows x
-//                   16/32 channels: image -> registers -> requant_fast4_i8 -> bytes -> its own swizzled smem buffer -> ONE
-//                   TMA store per group (cp.async.bulk.tensor, double-buffered).  No address arithmetic for the stores,
-//                   rows outside the tensor are clipped by the TMA unit.
+//                   16 cs channels (cs = 1 or 2): image -> registers -> requant_fast_words_i8 -> bytes -> its own swizzled
+//                   smem buffer -> ONE TMA store per group (cp.async.bulk.tensor, double-buffered).  Inside a group each lane
+//                   owns one 4-channel word of 4 cs rows: its constants stay in registers, and its 4 cs words are requantised
+//                   side by side.  No address arithmetic for the stores, rows outside the tensor are clipped by the TMA unit.
 // So the tensor cores multiply stage s+1 while the epilogue requantises stage s: the registers are the second accumulator
 // buffer.  Registers per thread (setmaxnreg): WG0 40, MMA 200 (at most 128 accumulators), epilogue 136.
 // The producer runs ahead through the ring, so the next tile's operands are resident when its MMAs start.  K is small
-// (32..1024), so these layers are bound by the epilogue's ALU-pipe issue rate, not by the tensor pipe: see common.cuh
-// (requant_fast4_i8) for the instruction budget.
+// (32..1024), so the epilogue sets the pace of these layers, not the tensor pipe.  With only two epilogue warps per scheduler
+// it is bound by latency unless each lane has many independent chains in flight: hence 4 cs words per lane, their image
+// loads issued together and their fp32 chains interleaved (common.cuh, requant_fast_words_i8).
 #include <cuda.h>
 
 #include "common.cuh"
@@ -119,21 +121,22 @@ struct FixQueue
 };
 __shared__ FixQueue s_fixq;
 
-__device__ __forceinline__ bool fixq_push(uint32_t mtile, int oc, int32_t acc)
+// row: the element's image row = its row of the m-tile (0..127)
+__device__ __forceinline__ bool fixq_push(uint32_t mtile, uint32_t row, int oc, int32_t acc)
 {
     if (!s_fixq.q) return false;
     const uint32_t slot = atomicAdd(&s_fixq.count, 1u);
     if (slot >= s_fixq.cap) return false;
-    const uint32_t row = ((threadIdx.x >> 5) & 3u) * 32u + (threadIdx.x & 31u); // image row of this thread = row of the m-tile
     s_fixq.q[slot] = make_uint4(mtile, row | ((uint32_t)oc << 8), (uint32_t)acc, 0u);
     return true;
 }
 
-// One guarded word (final fast bytes in `word`): find the elements that really sit in the band, queue them (or fix them here).
+// One guarded word (final fast bytes in `word`) of image row `row`: find the elements that really sit in the band, queue them
+// (or fix them here).
 // a[j]: what the fast path converted to float -- int8: the raw accumulator (y is added inside), uint8: accumulator + sum(x) term + y.
 template <bool U8, bool FUSE>
 __device__ __noinline__ uint32_t gemm_fix_word(uint32_t word, int32_t a0, int32_t a1, int32_t a2, int32_t a3, int oc0, int oc_limit, uint32_t mtile,
-                                               const EpiParams& e)
+                                               uint32_t row, const EpiParams& e)
 {
     const FastPar4 f = fast_par4_ldg(e, oc0);
     const int32_t a[4] = {a0, a1, a2, a3};
@@ -146,7 +149,7 @@ __device__ __noinline__ uint32_t gemm_fix_word(uint32_t word, int32_t a0, int32_
         const float d = __fsub_rn(t, __fsub_rn(r, TB200_MAGIC));
         if (fabsf(d) > 0.5f - TB200_TIE_EPS && oc0 + j < oc_limit)
         {
-            if (!fixq_push(mtile, oc0 + j, a[j]))
+            if (!fixq_push(mtile, row, oc0 + j, a[j]))
             {
                 // the literal arithmetic wants the accumulator without the bias (uint8: y holds it)
                 const int32_t acc = a[j] - ((U8 && e.has_bias) ? __ldg(e.bias + oc0 + j) : 0);
@@ -186,140 +189,119 @@ __device__ __forceinline__ void fixq_drain(const GemmArgs& g, const EpiParams& e
     }
 }
 
-// 16 accumulator columns of one row -> 16 output bytes into the warp's staging buffer (int8, fast path).
-template <bool FUSE>
-__device__ __forceinline__ void epilogue_unit_fast(const uint32_t (&v)[16], uint32_t par_addr, uint32_t dst_addr, int oc0, uint32_t mtile, const EpiParams& e)
+// Exact mode, one word: the literal arithmetic for each of its real channels (uint8: y from the constants in shared memory, the
+// bias taken off again, the padding taps' corrections added).  Not inlined: the lane's other words then stay in registers across
+// the requant() calls instead of spilling.
+template <bool U8, bool BORDER>
+__device__ __noinline__ uint32_t epilogue_word_exact(uint32_t v0, uint32_t v1, uint32_t v2, uint32_t v3, int32_t rowc, uint32_t pad, uint32_t par_addr,
+                                                     int oc0, int oc_limit, int ocp, const int32_t* btab, const EpiParams& e)
 {
-    uint32_t w[4];
-    float gw[4];
+    const uint32_t v[4] = {v0, v1, v2, v3};
+    uint32_t w = 0;
 #pragma unroll
-    for (int h = 0; h < 2; h++)
+    for (int j = 0; j < 4; j++)
     {
-        float4 p[4];
-#pragma unroll
-        for (int k = 0; k < 4; k++) p[k] = lds_f4(par_addr + h * 64 + k * 16);
-        const int32_t a8[8] = {(int32_t)v[h * 8], (int32_t)v[h * 8 + 1], (int32_t)v[h * 8 + 2], (int32_t)v[h * 8 + 3],
-                               (int32_t)v[h * 8 + 4], (int32_t)v[h * 8 + 5], (int32_t)v[h * 8 + 6], (int32_t)v[h * 8 + 7]};
-        requant_fast8_i8<FUSE>(a8, p, e, w[2 * h], w[2 * h + 1], gw[2 * h], gw[2 * h + 1]);
+        const int oc = oc0 + j;
+        if (oc < oc_limit)
+        {
+            int32_t acc = (int32_t)v[j];
+            if (U8)
+            {
+                const float4 pp = lds_f4(par_addr + (j >> 1) * 16);
+                acc += rowc + __float_as_int((j & 1) ? pp.w : pp.z) - (e.has_bias ? __ldg(e.bias + oc) : 0);
+                if (BORDER && pad) acc += __ldg(btab + (size_t)pad * ocp + oc);
+            }
+            w |= ((uint32_t)requant(acc, oc, e) & 0xffu) << (8 * j);
+        }
     }
-    if (e.q_byte_add)
-    {
-#pragma unroll
-        for (int j = 0; j < 4; j++) w[j] = requant_byte_fix(w[j], e);
-    }
-    if (fmaxf(fmaxf(gw[0], gw[1]), fmaxf(gw[2], gw[3])) > 0.5f - TB200_TIE_EPS)
-    {
-        // rare (2.4e-4 of the elements): exact recomputation of the guarded bytes
-#pragma unroll
-        for (int j = 0; j < 4; j++)
-            if (gw[j] > 0.5f - TB200_TIE_EPS)
-                w[j] = gemm_fix_word<false, FUSE>(w[j], (int32_t)v[j * 4], (int32_t)v[j * 4 + 1], (int32_t)v[j * 4 + 2], (int32_t)v[j * 4 + 3], oc0 + j * 4, 0x7fffffff /* pad channels have M = y = 0: never guarded */, mtile, e);
-    }
-    sts_u4(dst_addr, w[0], w[1], w[2], w[3]);
+    return w;
 }
 
-// degenerate scales / accumulators that could leave the 16-bit clamp range: literal arithmetic for every element
-__device__ __forceinline__ void epilogue_unit_exact(const uint32_t (&v)[16], uint32_t dst_addr, int oc0, int oc_limit, const EpiParams& e)
-{
-    uint32_t w[4];
-#pragma unroll
-    for (int k = 0; k < 16; k++)
-    {
-        if ((k & 3) == 0) w[k >> 2] = 0;
-        if (oc0 + k < oc_limit) w[k >> 2] |= ((uint32_t)requant((int32_t)v[k], oc0 + k, e) & 0xffu) << (8 * (k & 3));
-    }
-    sts_u4(dst_addr, w[0], w[1], w[2], w[3]);
-}
-
-// uint8 flavour: v = sum x*w over in-bounds taps (raw bytes), sx = sum x.  The true accumulator is
-//   sum (x-zx)(w-zw) = v - zw*sx + corr[oc] + sum_{padding taps t} btab[t][oc]
-// with corr[oc] = -zx*sum_k w + taps*Cin*zx*zw (interior pixels) folded into the per-channel constants.
+// One lane's share of a store group: channel word oc0..oc0+3 of the 4*CS rows row0 + k*(8/CS) of the image (row0: the lane's
+// first row of the m-tile), v[k] their accumulators -> 4*CS output words, one 32-bit store each into the warp's staging buffer
+// (dst[k & 1] + 128 k: the CS == 2 swizzle flips chunk bit 4 on the rows with bit 2 set, i.e. on odd k).  All 4*CS words go
+// through the fast requantisation together, so each lane has 4*CS independent chains in flight; f: the word's constants,
+// held in registers by the caller (fast modes), par_addr: the same in shared memory (exact mode).
 // uint8 flavour: v = sum x*w over in-bounds taps (raw bytes), sx = sum x.  The true accumulator is
 //   sum (x-zx)(w-zw) = v - zw*sx + corr[oc] + sum_{padding taps t} btab[t][oc]
 // with corr[oc] = -zx*sum_k w + taps*Cin*zx*zw (interior pixels).  The per-channel constants are in the int8 layout
-// { M[2k], M[2k+1], y[2k], y[2k+1] } with y = corr + bias (an integer), so the fast path IS the int8 one on a' = v + rowc + y:
-// t = fl((float)a' * M), exact up to the tie guard under the bound engine.cu proves per layer (|bias*M| <= 250).
-
-template <bool EXACT, bool BORDER>
-__device__ __forceinline__ void epilogue_unit_u8(const uint32_t (&v)[16], int32_t rowc, uint32_t pad_mask_in, const GemmArgs& g, uint32_t par_addr,
-                                                 uint32_t dst_addr, int oc0, uint32_t mtile, const EpiParams& e)
+// { M[2k], M[2k+1], y[2k], y[2k+1] } with y = corr + bias (an integer), so the fast path IS the int8 one on
+// a' = v + rowc[k] + btab[pad[k]] (BORDER only) + y: t = fl((float)a' * M), exact up to the tie guard under the bound engine.cu
+// proves per layer (|bias*M| <= 250).  rowc[k] = cplane * sx of row k.
+// MODE: 0 fast, 1 fast with the bias fused into the FMA (int8 only), 2 exact (literal arithmetic for every element: degenerate
+// scales, or accumulators that could leave the 16-bit clamp range).
+template <bool U8, int MODE, int CS, bool BORDER>
+__device__ __forceinline__ void epilogue_words(const uint32_t (&v)[4 * CS][4], const int32_t (&rowc)[4 * CS], const uint32_t (&pad)[4 * CS],
+                                               const FastPar4& f, uint32_t par_addr, int oc0, uint32_t row0, const uint32_t (&dst)[2],
+                                               uint32_t mtile, const GemmArgs& g, const EpiParams& e)
 {
-    const uint32_t pad_mask = BORDER ? pad_mask_in : 0u; // BORDER == false (1x1 / FC, unpadded convs): the correction code compiles away
-    uint32_t w[4];
-    if (!EXACT)
+    constexpr int W = 4 * CS, RPI = 8 / CS;
+    constexpr bool FUSE = !U8 && MODE == 1;
+    uint32_t w[W];
+    if (MODE != 2)
     {
-        float gw[4];
+        const int32_t y[4] = {__float_as_int(f.a.z), __float_as_int(f.a.w), __float_as_int(f.b.z), __float_as_int(f.b.w)}; // uint8: integers
+        int32_t a[W][4];
 #pragma unroll
-        for (int h = 0; h < 2; h++)
+        for (int k = 0; k < W; k++)
+#pragma unroll
+            for (int j = 0; j < 4; j++) a[k][j] = (int32_t)v[k][j] + (U8 ? rowc[k] : 0); // (+ y inside requant_fast_words_i8<false>)
+        if (U8 && BORDER && oc0 < g.ocp) // (channels of an N tile past ocp have no table entries; they come out 0)
         {
-            float4 p[4];
 #pragma unroll
-            for (int k = 0; k < 4; k++) p[k] = lds_f4(par_addr + h * 64 + k * 16);
-            int32_t a8[8];
-#pragma unroll
-            for (int k = 0; k < 8; k++) a8[k] = (int32_t)v[h * 8 + k] + rowc; // (+ y inside requant_fast8_i8<false>: one IADD3)
-            if (pad_mask)
-            {
-                // border row: the summed corrections of its missing taps, one 16-byte load per four channels
-                const int4* pt = reinterpret_cast<const int4*>(g.btab + (size_t)pad_mask * g.ocp + oc0 + h * 8);
-                const int4 c0 = __ldg(pt), c1 = __ldg(pt + 1);
-                a8[0] += c0.x, a8[1] += c0.y, a8[2] += c0.z, a8[3] += c0.w, a8[4] += c1.x, a8[5] += c1.y, a8[6] += c1.z, a8[7] += c1.w;
-            }
-            requant_fast8_i8<false>(a8, p, e, w[2 * h], w[2 * h + 1], gw[2 * h], gw[2 * h + 1]);
+            for (int k = 0; k < W; k++)
+                if (pad[k])
+                {
+                    // border row: the summed corrections of its missing taps, one 16-byte load per word
+                    const int4 c = __ldg(reinterpret_cast<const int4*>(g.btab + (size_t)pad[k] * g.ocp + oc0));
+                    a[k][0] += c.x, a[k][1] += c.y, a[k][2] += c.z, a[k][3] += c.w;
+                }
         }
+        float gw[W];
+        const FastPar4 fp[1] = {f};
+        requant_fast_words_i8<FUSE, W, 1>(a, fp, e, w, gw);
         if (e.q_byte_add)
         {
 #pragma unroll
-            for (int j = 0; j < 4; j++) w[j] = requant_byte_fix(w[j], e);
+            for (int k = 0; k < W; k++) w[k] = requant_byte_fix(w[k], e);
         }
-        if (fmaxf(fmaxf(gw[0], gw[1]), fmaxf(gw[2], gw[3])) > 0.5f - TB200_TIE_EPS)
+        float gmax = gw[0];
+#pragma unroll
+        for (int k = 1; k < W; k++) gmax = fmaxf(gmax, gw[k]);
+        if (gmax > 0.5f - TB200_TIE_EPS)
         {
-            // rare (2.4e-4 of the elements): the guarded words again -- requant_fix_word_u8 finds the elements inside the band and
-            // runs the literal reference arithmetic on exactly those
+            // rare (2.4e-4 of the elements): the guarded words again -- gemm_fix_word finds the elements inside the band and queues
+            // them for the literal reference arithmetic
 #pragma unroll
-            for (int j = 0; j < 4; j++)
-                if (gw[j] > 0.5f - TB200_TIE_EPS)
+            for (int k = 0; k < W; k++)
+                if (gw[k] > 0.5f - TB200_TIE_EPS)
                 {
-                    int32_t a[4];
-#pragma unroll
-                    for (int t = 0; t < 4; t++)
-                    {
-                        const float4 pp = lds_f4(par_addr + ((j * 4 + t) >> 1) * 16);
-                        a[t] = (int32_t)v[j * 4 + t] + rowc + __float_as_int((t & 1) ? pp.w : pp.z);
-                    }
-                    if (pad_mask && oc0 + j * 4 < g.ocp)
-                    {
-                        const int4 c = __ldg(reinterpret_cast<const int4*>(g.btab + (size_t)pad_mask * g.ocp + oc0 + j * 4));
-                        a[0] += c.x, a[1] += c.y, a[2] += c.z, a[3] += c.w;
-                    }
-                    w[j] = gemm_fix_word<true, false>(w[j], a[0], a[1], a[2], a[3], oc0 + j * 4, g.oc, mtile, e);
+                    const uint32_t row = row0 + (uint32_t)(k * RPI);
+                    if (U8)
+                        w[k] = gemm_fix_word<true, false>(w[k], a[k][0] + y[0], a[k][1] + y[1], a[k][2] + y[2], a[k][3] + y[3], oc0, g.oc, mtile, row, e);
+                    else
+                        w[k] = gemm_fix_word<false, FUSE>(w[k], a[k][0], a[k][1], a[k][2], a[k][3], oc0,
+                                                          0x7fffffff /* pad channels have M = y = 0: never guarded */, mtile, row, e);
                 }
         }
-        if (oc0 + 16 > g.oc)
+        if (U8 && oc0 + 4 > g.oc)
         {
             // pad lanes of uint8 tensors hold 0, not the zero point
 #pragma unroll
-            for (int k = 0; k < 16; k++)
-                if (oc0 + k >= g.oc) w[k >> 2] &= ~(0xffu << (8 * (k & 3)));
+            for (int j = 0; j < 4; j++)
+                if (oc0 + j >= g.oc)
+#pragma unroll
+                    for (int k = 0; k < W; k++) w[k] &= ~(0xffu << (8 * j));
         }
     }
     else
     {
 #pragma unroll
-        for (int k = 0; k < 16; k++)
-        {
-            if ((k & 3) == 0) w[k >> 2] = 0;
-            const int oc = oc0 + k;
-            if (oc < g.oc)
-            {
-                const float4 pp = lds_f4(par_addr + (k >> 1) * 16);
-                int32_t a = (int32_t)v[k] + rowc + __float_as_int((k & 1) ? pp.w : pp.z) - (e.has_bias ? __ldg(e.bias + oc) : 0);
-                if (pad_mask) a += __ldg(g.btab + (size_t)pad_mask * g.ocp + oc);
-                w[k >> 2] |= ((uint32_t)requant(a, oc, e) & 0xffu) << (8 * (k & 3));
-            }
-        }
+        for (int k = 0; k < W; k++)
+            w[k] = epilogue_word_exact<U8, BORDER>(v[k][0], v[k][1], v[k][2], v[k][3], rowc[k], pad[k], par_addr, oc0, g.oc, g.ocp, g.btab, e);
     }
-    sts_u4(dst_addr, w[0], w[1], w[2], w[3]);
+#pragma unroll
+    for (int k = 0; k < W; k++) sts_b32(dst[k & 1] + 128u * k, w[k]);
 }
 
 // border pattern of output pixel r of m-tile mt (0 = every tap inside the image): how many rows / columns of the filter window are
@@ -636,11 +618,25 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
         // ===================== epilogue (warps 8..15) =====================
         // Image quarter q (rows 32q..32q+31) is served by the two warps {8 + q, 12 + q}.  The work of an accumulator stage is cut
         // into store groups (m-tile i, columns [grp*16*cs, (grp+1)*16*cs)) of 32 rows each, dealt round-robin to the quarter's
-        // warps.  A warp requantises its group chunk by chunk (16 columns per load, the next chunk's load in flight), writes the
-        // bytes to its own swizzled staging buffer and hands the buffer to the TMA unit with one store.  It releases its quarter
-        // of the image to the MMA warpgroup (img_empty[q]) as soon as it has issued its last load of the stage; a warp with no group
-        // in the stage, or whose quarter has no valid rows, arrives at the end of the stage, so each warp arrives once per stage.
+        // warps.  Inside a group lane L owns channel word w = L % (4 cs) (channels cg0 + 4w .. +3) of the 4 cs rows
+        // L / (4 cs) + k * (8 / cs), k = 0 .. 4 cs - 1: it issues the 4 cs image loads of its rows first, then requantises the
+        // 4 cs words together with the word's constants in registers, and writes each word with one 32-bit store into the warp's
+        // own swizzled staging buffer, which it hands to the TMA unit with one store.  It releases its quarter of the image to
+        // the MMA warpgroup (img_empty[q]) as soon as it has issued its last load of the stage; a warp with no group in the
+        // stage, or whose quarter has no valid rows, arrives at the end of the stage, so each warp arrives once per stage.
+        // Shared-memory banks (a 16-byte access is served eight lanes at a time, 128 bytes per wavefront):
+        //   image loads, cs 2: the eight lanes of a quarter-warp read the 8 words = 128 contiguous bytes of one row: one
+        //     wavefront each, 4 per instruction (512 bytes), the minimum.
+        //   image loads, cs 1: a quarter-warp reads 64 contiguous bytes of each of two rows, one pitch apart; the pitch
+        //     (cols * 4 + 16, cols a multiple of 16) is 16 or 80 modulo 128, so the two 64-byte runs share banks: 2 wavefronts
+        //     per quarter-warp.  Only the cs 1 plans (N tiles of an odd number of 16-channel chunks, which MobileNet-v1 has
+        //     none of) pay it; a pitch of 64 modulo 128 would cost every plan 6 KB of ring and the MMA warps' conflict-free
+        //     fragment stores.
+        //   staging stores: instruction k writes rows 4k / 8k .. of the buffer, i.e. bytes [128 k, 128 k + 128) (permuted by
+        //     the swizzle inside), 4 bytes per lane: one wavefront.
+        //   constants: the lanes of one word read the same 32 bytes (broadcast), 4 cs distinct 16-byte addresses: one wavefront.
         setmaxnreg_inc<REG_EPI>();
+        constexpr int WPR = 4 * CS, RPI = 8 / CS; // words per group row, rows per warp-wide load
         const int ew = warp - EPI_WARP0; // epilogue warp 0..7
         const int q = warp & 3;
         const int sub = ew >> 2;
@@ -650,12 +646,18 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
         qrows = qrows < 0 ? 0 : (qrows > 32 ? 32 : qrows);
         const CUtensorMap* tm_out = (qrows == 32) ? &tmap_out : &tmap_out_tail;
         const uint32_t buf0 = stg_base + (uint32_t)ew * 2u * buf_bytes;
-        // swizzle of the staging buffer = the output map's swizzle: 16-byte chunk index ^= row bit 2 (Swizzle<1,4,3>, CS 2 only)
-        const uint32_t xl = CS == 2 ? (uint32_t)((lane >> 2) & 1) << 4 : 0u;
-        const uint32_t row_off = (uint32_t)lane * 16u * CS;
+        const int lw = lane % WPR, lr = lane / WPR; // this lane's word and first row of a group
+        const uint32_t img_lane = img_base + (uint32_t)(q * 32 + lr) * img_pitch + 16u * (uint32_t)lw;
+        // staging offsets of word lw in rows lr + RPI k: even k, and odd k, whose row has bit 2 set, so that the output map's
+        // swizzle (16-byte chunk index ^= row bit 2, Swizzle<1,4,3>, CS 2 only) flips the chunk
+        uint32_t st_off[2];
+        st_off[0] = (uint32_t)lr * (16u * CS) + 4u * (uint32_t)lw;
+        st_off[1] = CS == 2 ? st_off[0] ^ 16u : st_off[0];
         uint32_t ucount = 0; // groups this warp has stored (buffer parity)
         const int par_ch = g.n_tiles * g.block_n;
         const bool fast = MODE != 2;
+        FastPar4 f = {};       // fast modes: this lane's word's constants ...
+        uint32_t par_at = ~0u; // ... from this shared-memory address (~0: none)
         if (g.par_all)
         {
             // per-channel fast-path constants of every N tile, once; pad / overhanging channels get (0, 0)
@@ -681,21 +683,18 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
                     sts_f2(par_base + c * 8, (n0 + c < g.ocp && (fast || U8)) ? __ldg(e.fast_par + n0 + c) : make_float2(0.f, 0.f));
                 epilogue_bar_sync();
                 par_s = par_base;
+                par_at = ~0u; // the registers hold the previous tile's constants
             }
             mbar_wait(&ctl->img_full[q], iphase); // this warp's quarter of the image holds this stage
             iphase ^= 1;
             if (U8 && g.cplane) mbar_wait(&ctl->sx_full[as], aphase); // the row sums of this stage
             TLOG_E(0);
-            const uint32_t tbase = img_base + (uint32_t)(q * 32 + lane) * img_pitch;
             bool released = false; // this warp has arrived on img_empty for this stage
             if (qrows > 0)
             {
                 // groups of this warp: flattened index u = i * ngroups + grp, u = sub, sub + 2, ...
-                uint32_t v0[16], v1[16];
                 int i = 0, grp = sub;
                 while (grp >= ngroups) grp -= ngroups, i++;
-                if (CS > 1 && i < mtc)
-                    acc_ld16(tbase + 4u * (i * g.block_n + grp * (CS * 16)), reinterpret_cast<uint32_t(&)[16]>(v0));
                 while (i < mtc)
                 {
                     int i2 = i, g2 = grp + 2; // the group after this one
@@ -704,60 +703,56 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
                     // the store issued two groups ago has finished reading this buffer
                     if (lane == 0) bulk_wait_read<1>();
                     __syncwarp();
-                    uint32_t pad = 0;
-                    int32_t rowc = 0;
+                    const int cg0 = grp * (CS * 16); // first column of the group inside the N tile
+                    const int c = cg0 + 4 * lw;      // first channel of this lane's word inside the N tile
+                    // the accumulators of this lane's rows, all loads in flight before the first is used
+                    uint32_t v[WPR][4];
+                    const uint32_t src = img_lane + 4u * (uint32_t)(i * g.block_n + cg0);
+#pragma unroll
+                    for (int k = 0; k < WPR; k++)
+                    {
+                        const uint4 u = lds_u4(src + (uint32_t)(k * RPI) * img_pitch);
+                        v[k][0] = u.x, v[k][1] = u.y, v[k][2] = u.z, v[k][3] = u.w;
+                    }
+                    TLOG_E(3);
+                    if (i2 >= mtc)
+                    {
+                        // the last image loads of the stage are issued: (release) the MMA warpgroup may overwrite the image
+                        __syncwarp();
+                        if (lane == 0) mbar_arrive(&ctl->img_empty[q]);
+                        released = true;
+                    }
+                    const uint32_t pa = par_s + (uint32_t)c * 8u; // the word's constants in shared memory
+                    if (MODE != 2 && pa != par_at) f.a = lds_f4(pa), f.b = lds_f4(pa + 16u), par_at = pa; // (the group's columns changed)
+                    int32_t rowc[WPR];
+                    uint32_t pad[WPR];
+#pragma unroll
+                    for (int k = 0; k < WPR; k++) rowc[k] = 0, pad[k] = 0;
                     if (U8)
                     {
-                        // the pixel's sum(x), once per group
                         if (g.cplane)
                         {
-                            int32_t sx;
-                            asm volatile("ld.shared.b32 %0, [%1];" : "=r"(sx) : "r"(sx_base + (uint32_t)(((as * 4 + i) * 128 + q * 32 + lane) * 4)));
-                            rowc = g.cplane * sx;
-                        }
-                        if (BORDER) pad = padding_taps(g, mt0 + i, q * 32 + lane);
-                    }
-                    const uint32_t tg = tbase + 4u * (i * g.block_n + grp * (CS * 16));
-                    const int cg0 = grp * (CS * 16); // first column of the group inside the N tile
-                    const uint32_t sdst = buf + row_off;
-                    auto unit = [&](const uint32_t (&v)[16], int k)
-                    {
-                        const int c = cg0 + k * 16;
-                        const uint32_t dst = sdst + (((uint32_t)k << 4) ^ xl);
-                        if (U8) epilogue_unit_u8<MODE == 2, BORDER>(v, rowc, pad, g, par_s + c * 8, dst, n0 + c, (uint32_t)(mt0 + i), e);
-                        else if (MODE == 2) epilogue_unit_exact(v, dst, n0 + c, g.oc, e);
-                        else epilogue_unit_fast<MODE == 1>(v, par_s + c * 8, dst, n0 + c, (uint32_t)(mt0 + i), e);
-                    };
-                    // after the last image load of the stage: (release) the MMA warpgroup may overwrite the image
-                    auto release = [&]()
-                    {
-                        if (i2 >= mtc)
-                        {
-                            __syncwarp();
-                            if (lane == 0) mbar_arrive(&ctl->img_empty[q]);
-                            released = true;
-                        }
-                    };
-                    if (CS == 1)
-                    {
-                        acc_ld16(tg, reinterpret_cast<uint32_t(&)[16]>(v0));
-                        release();
-                        unit(reinterpret_cast<const uint32_t(&)[16]>(v0), 0);
-                    }
-                    else
-                    {
+                            // the rows' sum(x) terms
+                            const uint32_t sx = sx_base + (uint32_t)(((as * 4 + i) * 128 + q * 32 + lr) * 4);
 #pragma unroll
-                        for (int k = 0; k < CS; k++)
+                            for (int k = 0; k < WPR; k++)
+                            {
+                                int32_t s;
+                                asm volatile("ld.shared.b32 %0, [%1];" : "=r"(s) : "r"(sx + (uint32_t)(k * RPI * 4)));
+                                rowc[k] = g.cplane * s;
+                            }
+                        }
+                        if (BORDER)
                         {
-                            TLOG_E(3);
-                            // the next chunk's accumulators are in flight while this one is requantised
-                            if (k + 1 < CS) acc_ld16(tg + (k + 1) * 64, reinterpret_cast<uint32_t(&)[16]>(*((k & 1) ? v0 : v1)));
-                            else if (i2 < mtc) acc_ld16(tbase + 4u * (i2 * g.block_n + g2 * (CS * 16)), reinterpret_cast<uint32_t(&)[16]>(v0));
-                            if (k + 1 == CS) release();
-                            unit(reinterpret_cast<const uint32_t(&)[16]>(*((k & 1) ? v1 : v0)), k);
-                            TLOG_E(4);
+                            // border pattern of row `lane` of the quarter, then each lane fetches those of its own rows
+                            const uint32_t pl = padding_taps(g, mt0 + i, q * 32 + lane);
+#pragma unroll
+                            for (int k = 0; k < WPR; k++) pad[k] = __shfl_sync(0xffffffffu, pl, lr + k * RPI);
                         }
                     }
+                    const uint32_t dst[2] = {buf + st_off[0], buf + st_off[1]};
+                    epilogue_words<U8, MODE, CS, BORDER>(v, rowc, pad, f, pa, n0 + c, (uint32_t)(q * 32 + lr), dst, (uint32_t)(mt0 + i), g, e);
+                    TLOG_E(4);
                     fence_proxy_async_smem(); // generic-proxy writes -> visible to the TMA unit
                     __syncwarp();
                     if (lane == 0)

@@ -175,13 +175,19 @@ __device__ __forceinline__ void sts_u4(uint32_t addr, uint32_t a, uint32_t b, ui
 {
     asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
 }
+__device__ __forceinline__ void sts_b32(uint32_t addr, uint32_t a)
+{
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(a) : "memory");
+}
 __device__ __forceinline__ void sts_f2(uint32_t addr, float2 v)
 {
     asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(v.x), "f"(v.y) : "memory");
 }
 
 // ---- accumulator image: the s32 accumulators of a 128-row tile as [row][pitch bytes] in shared memory --------------------
-// The MMA warpgroups write their fragments here; the epilogues read one row per thread, 16 consecutive columns at a time.
+// The MMA warpgroups write their fragments here.  The window convolutions' epilogue (conv_window.cu) reads one row per thread,
+// 16 consecutive columns at a time (acc_ld16); the persistent GEMM's epilogue reads one 4-column word of several rows per
+// thread, 8 / CS rows per warp-wide 16-byte load (gemm_tcgen05.cu).
 __device__ __forceinline__ void frag_to_image(const uint32_t (&d)[8], uint32_t img, uint32_t pitch, int row0, int col0)
 {
     const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;

@@ -94,13 +94,16 @@ __device__ __forceinline__ void tc_unit16(const uint32_t (&v)[16], int32_t rowc,
 #pragma unroll
     for (int h = 0; h < 2; h++)
     {
-        float4 p[4];
+        FastPar4 p[2];
 #pragma unroll
-        for (int k = 0; k < 4; k++) p[k] = lds_f4(par_addr + h * 64 + k * 16);
-        int32_t a8[8];
+        for (int k = 0; k < 2; k++) p[k].a = lds_f4(par_addr + h * 64 + k * 32), p[k].b = lds_f4(par_addr + h * 64 + k * 32 + 16);
+        int32_t a8[2][4];
 #pragma unroll
-        for (int k = 0; k < 8; k++) a8[k] = (int32_t)v[h * 8 + k] + (U8 ? rowc : 0);
-        requant_fast8_i8<FUSE>(a8, p, e, w[2 * h], w[2 * h + 1], gw[2 * h], gw[2 * h + 1]);
+        for (int k = 0; k < 8; k++) a8[k >> 2][k & 3] = (int32_t)v[h * 8 + k] + (U8 ? rowc : 0);
+        uint32_t w2[2];
+        float g2[2];
+        requant_fast_words_i8<FUSE, 2, 2>(a8, p, e, w2, g2);
+        w[2 * h] = w2[0], w[2 * h + 1] = w2[1], gw[2 * h] = g2[0], gw[2 * h + 1] = g2[1];
     }
     if (e.q_byte_add)
     {
