@@ -7,7 +7,8 @@ of the oracle); ops that `ties.exact_layer` does not cover (softmax, upsample, s
 `gemm_geometry`, `dw_geometry`, `window_geometry`, `gather_geometry`, `epi_clamp` and `conv_kind` restate the C planners line by
 line (cited at each function).  They only describe what the library decides -- no plan logic lives here -- so that the CPU test
 can show every entry reaches the geometry it is meant to, and the GPU test can tie the restatement to the library
-(TB200_DEBUG_LAUNCH prints the plans of the GEMM, the window and the gather kernel).
+(TB200_DEBUG_LAUNCH prints the plans of the GEMM, the window and the gather kernel).  `conv_recipe` restates the device glue's
+choice of float recipe, the one the unmodified reference would run: every conv entry has it, or is marked `abi_only`.
 
 Every boundary is probed from both sides: an entry per side, listed in `BOUNDARIES`.
 """
@@ -209,6 +210,24 @@ def epi_clamp(g, L):
                 bound_beyond_sat=any(ties._round_away(b) < lo or ties._round_away(b) > hi for b in bounds))
 
 
+# ---- b200_device.cc conv_recipe: the recipe Tengine's CPU device would run a convolution with ---------------------------------
+def conv_recipe(g, L):
+    """Group 1: HCL (conv_hcl_x86 / conv_direct_hcl_int8_x86).  A depthwise conv: HCL only for int8 at batch 1, 3x3, one stride of
+    1 or 2, no dilation and each axis padded alike on both sides (conv_dw_hcl_x86.c:508-543); every other grouped conv, and every
+    uint8 depthwise, runs conv_ref: REF.  A layer with the other recipe can only come from a C-ABI caller."""
+    n, C = g.tensors[L["inputs"][0]]["dims"][:2]
+    OC = g.tensors[L["output"]]["dims"][1]
+    grp = L["group"]
+    if grp == 1:
+        return abi.RECIPE_HCL
+    dw = grp == C and grp == OC
+    if (dw and g.data_type == abi.DT_INT8 and n == 1 and L["kernel_h"] == 3 and L["kernel_w"] == 3 and L["stride_h"] == L["stride_w"]
+            and L["stride_h"] in (1, 2) and L["dilation_h"] == 1 and L["dilation_w"] == 1 and L["pad_h0"] == L["pad_h1"]
+            and L["pad_w0"] == L["pad_w1"]):
+        return abi.RECIPE_HCL
+    return abi.RECIPE_REF
+
+
 # ---- engine.cu plan_conv and fill_conv_step: the kernel of a convolution ----------------------------------------------------
 def _window_of(g, L, nhwc):
     n, C, _, W = g.tensors[L["inputs"][0]]["dims"]
@@ -360,6 +379,8 @@ class Entry:
     fused: bool = False    # run under the default plan (node fusion on); only the graph output is compared
     ties: bool = True      # built tie-dense (ties.check_not_vacuous applies)
     flags: int = 0         # prerun flags ORed into the run's (PRERUN_NO_TENSORCORE: the CUDA-core kernels)
+    abi_only: bool = False  # a conv whose recipe is not conv_recipe's for its shape: only a C-ABI caller can ask for it, so the
+    #                         unmodified reference (which picks its own) is no judge of it: not run through it
     notes: dict = field(default_factory=dict)
 
 
@@ -471,12 +492,14 @@ def act_conv(rng, u8, n, c, h, w, oc, activation, recipe, s_out, k=3, stride=1, 
     a power-of-two s_out (6 / 4 = 1.5, 1 / 2 = 0.5) are half-integers, which the reference rounds away from zero.  M = 2^-1
     (every odd accumulator is a tie); weights +-1 on about six taps per output, inputs in [-2, 2] about the zero point, so t
     spreads over about +-2 whatever K is.  uint8 zero points zx, zw, zo: at an end of the byte range the inputs are
-    [0, 4] or [251, 255] (ties._shift) and the weights zw + {0, 1} or zw - {0, 1}; the bias takes the accumulator's mean off."""
+    [0, 4] or [251, 255] (ties._shift) and the weights zw + {0, 1} or zw - {0, 1}; the bias takes the accumulator's mean off.
+    pad: an int or the 4-tuple (h0, h1, w0, w1)."""
     g = GraphDef(abi.DT_UINT8 if u8 else abi.DT_INT8)
     s_in, M = 2.0 ** -4, 0.5
     cg = c // group
     kk = cg * k * k
     zx, zw = (zx, zw) if u8 else (0, 0)
+    ph0, ph1, pw0, pw1 = pad if isinstance(pad, tuple) else (pad,) * 4
     x = g.input(n, c, h, w, s_in, zx)
     wd = rng.choice(np.array([-1, 1]), (oc, cg, k, k)) * (rng.random((oc, cg, k, k)) < min(1.0, 6.0 / kk))
     if u8 and ties._shift(zw, -1, 1):
@@ -486,8 +509,8 @@ def act_conv(rng, u8, n, c, h, w, oc, activation, recipe, s_out, k=3, stride=1, 
     if u8:
         xin = (zx + ties._shift(zx, -2, 2) + rng.integers(-2, 3, (n, c, h, w))).astype(np.uint8)
         if ties._shift(zx, -2, 2) or ties._shift(zw, -1, 1):
-            L = dict(group=group, stride_h=stride, stride_w=stride, dilation_h=1, dilation_w=1, pad_h0=pad, pad_h1=pad, pad_w0=pad,
-                     pad_w1=pad)
+            L = dict(group=group, stride_h=stride, stride_w=stride, dilation_h=1, dilation_w=1, pad_h0=ph0, pad_h1=ph1, pad_w0=pw0,
+                     pad_w1=pw1)
             b = (b - np.rint(ties.conv_acc(xin, zw + wd, L, zx, zw).mean(axis=(0, 2, 3)))).astype(np.int32)
         y = g.conv(x, (zw + wd).astype(np.uint8), b, [s_w], s_out, zo, stride=stride, pad=pad, group=group,
                    activation=activation, recipe=recipe, weight_zero=zw)
@@ -602,6 +625,7 @@ def upsample(rng, u8, c, scale, shape=(2, 5, 6), zi=128, min_byte=False):
 
 G_, I_, D_, DD = "gemm_i8_tcgen05", "conv_igemm_i8_tcgen05", "conv_dw3x3_tma_dp4a", "conv_dw_direct"
 LOW_M = (2, 2, 3, 4, 5)  # M_c >= 2^-2: the fast-path proof holds up to K ~ 1000
+REF = abi.RECIPE_REF  # conv_recipe's for grouped convs, batched int8 and every uint8 depthwise
 
 # ---- flat GEMM ------------------------------------------------------------------------------------------------------------
 # epilogue constants reloaded per N tile (par_all 0) past PAR_MAX = 2048 channels, resident up to it
@@ -670,35 +694,39 @@ _add("igemm1x1s2_u8_nopad", _u8(2, 64, 13, 15, 40, k=1, stride=2), I_, dict(taps
 
 # ---- depthwise 3x3 -------------------------------------------------------------------------------------------------------
 # the last 32-channel chunk half outside the tensor (cp % 32 == 16): MobileNet-v2's 144 channels
-_add("dw3x3s1_i8_c144", _i8(2, 144, 13, 14, 144, k=3, pad=1, group=144, mode=1), D_, dict(valid=True, cp_mod32=16))
-_add("dw3x3s2_i8_c48", _i8(2, 48, 13, 14, 48, k=3, stride=2, pad=1, group=48, mode=0), D_, dict(valid=True, cp_mod32=16))
-_add("dw3x3s1_i8_c40", _i8(2, 40, 9, 10, 40, k=3, pad=1, group=40, mode=2), D_, dict(valid=True, cp_mod32=16))
-_add("dw3x3s1_i8_c64", _i8(2, 64, 9, 10, 64, k=3, pad=1, group=64, mode=1), D_, dict(valid=True, cp_mod32=0))
-_add("dw3x3s1_u8_c144", _u8(1, 144, 9, 10, 144, k=3, pad=1, group=144), DD, dict(valid=False, cp_mod32=16))
+_add("dw3x3s1_i8_c144", _i8(2, 144, 13, 14, 144, k=3, pad=1, group=144, mode=1, recipe=REF), D_, dict(valid=True, cp_mod32=16))
+_add("dw3x3s2_i8_c48", _i8(2, 48, 13, 14, 48, k=3, stride=2, pad=1, group=48, mode=0, recipe=REF), D_, dict(valid=True, cp_mod32=16))
+_add("dw3x3s1_i8_c40", _i8(2, 40, 9, 10, 40, k=3, pad=1, group=40, mode=2, recipe=REF), D_, dict(valid=True, cp_mod32=16))
+_add("dw3x3s1_i8_c64", _i8(2, 64, 9, 10, 64, k=3, pad=1, group=64, mode=1, recipe=REF), D_, dict(valid=True, cp_mod32=0))
+_add("dw3x3s1_u8_c144", _u8(1, 144, 9, 10, 144, k=3, pad=1, group=144, recipe=REF), DD, dict(valid=False, cp_mod32=16))
 # the row limit: 16 pixel groups (ow 128 at stride 1, 64 at stride 2); one more pixel takes the generic kernel
 _add("dw3x3s1_i8_ow128", _i8(1, 48, 4, 128, 48, k=3, pad=1, group=48, mode=1), D_, dict(valid=True, gpr=16, stride=1))
 _add("dw3x3s1_i8_ow129", _i8(1, 48, 4, 129, 48, k=3, pad=1, group=48, mode=1), DD, dict(valid=False, gpr=17, stride=1))
 _add("dw3x3s2_i8_ow64", _i8(1, 48, 6, 128, 48, k=3, stride=2, pad=1, group=48, mode=1), D_, dict(valid=True, gpr=16, stride=2))
 _add("dw3x3s2_i8_ow65", _i8(1, 48, 6, 129, 48, k=3, stride=2, pad=1, group=48, mode=1), DD, dict(valid=False, gpr=17, stride=2))
 # fewer output rows than rows_per_cta
-_add("dw3x3s1_i8_oh3_capped", _i8(2, 32, 3, 8, 32, k=3, pad=1, group=32, mode=1), D_, dict(valid=True, rows_capped=True, rows_per_cta=3))
-_add("dw3x3s1_i8_oh1_capped", _i8(3, 32, 1, 20, 32, k=3, pad=1, group=32, mode=0), D_, dict(valid=True, rows_capped=True, rows_per_cta=1))
-_add("dw3x3s2_i8_oh2_capped", _i8(2, 48, 3, 30, 48, k=3, stride=2, pad=1, group=48, mode=1), D_, dict(valid=True, rows_capped=True))
+_add("dw3x3s1_i8_oh3_capped", _i8(2, 32, 3, 8, 32, k=3, pad=1, group=32, mode=1, recipe=REF), D_,
+     dict(valid=True, rows_capped=True, rows_per_cta=3))
+_add("dw3x3s1_i8_oh1_capped", _i8(3, 32, 1, 20, 32, k=3, pad=1, group=32, mode=0, recipe=REF), D_,
+     dict(valid=True, rows_capped=True, rows_per_cta=1))
+_add("dw3x3s2_i8_oh2_capped", _i8(2, 48, 3, 30, 48, k=3, stride=2, pad=1, group=48, mode=1, recipe=REF), D_,
+     dict(valid=True, rows_capped=True))
 _add("dw3x3s1_i8_oh17_full", _i8(1, 32, 17, 30, 32, k=3, pad=1, group=32, mode=1), D_, dict(valid=True, rows_capped=False, rows_per_cta=4))
 
 # ---- NCHW stems: the window kernel (W % 16 == 0, stride 1 / 2) and the gather kernel -----------------------------------------
 WI, GA, ST, DR = "conv_window_tcgen05", "conv_gather_tcgen05", "conv_stem_nchw_dp4a", "conv_direct_dp4a"
+CONV_KERNELS = (G_, I_, D_, DD, WI, GA, ST, DR)  # FC layers run the GEMM too, and are never abi_only
 NO_TC = abi.PRERUN_NO_TENSORCORE
 
 
-def _both(name, n, c, h, w, oc, k, stride, pad, kernel, edges, group=1, **kw):
+def _both(name, n, c, h, w, oc, k, stride, pad, kernel, edges, group=1, recipe=abi.RECIPE_HCL, **kw):
     """The int8 and the uint8 entry of one conv shape (pad: an int or the 4-tuple (h0, h1, w0, w1)); modes as ties' defaults."""
     if isinstance(pad, tuple):
         _add(name.format("i8"), lambda r: i8_conv_pad(r, n, c, h, w, oc, k, stride, pad), kernel, edges, **kw)
         _add(name.format("u8"), lambda r: u8_conv_pad(r, n, c, h, w, oc, k, stride, pad), kernel, edges, **kw)
     else:
-        _add(name.format("i8"), _i8(n, c, h, w, oc, k=k, stride=stride, pad=pad, group=group), kernel, edges, **kw)
-        _add(name.format("u8"), _u8(n, c, h, w, oc, k=k, stride=stride, pad=pad, group=group), kernel, edges, **kw)
+        _add(name.format("i8"), _i8(n, c, h, w, oc, k=k, stride=stride, pad=pad, group=group, recipe=recipe), kernel, edges, **kw)
+        _add(name.format("u8"), _u8(n, c, h, w, oc, k=k, stride=stride, pad=pad, group=group, recipe=recipe), kernel, edges, **kw)
 
 
 # 7x7 over 1 and 2 channels: 2 and 4 k-steps of A in shared memory (of the 5 a 147-byte row could fill), B right after them
@@ -746,13 +774,14 @@ _add("gat3x3s3_u8_c12", _u8(2, 12, 10, 13, 40, k=3, stride=3, pad=1), GA, dict(k
 _add("win3x3s2_u8_c24", _u8(3, 24, 9, 20, 40, k=3, stride=2, pad=1), WI, dict(layout=3, ks=9))
 
 # ---- CUDA-core kernels: grouped direct conv (OCT 8 / 4), generic depthwise, the int8 depthwise 3x3 without a TMA plan -------
-_both("direct3x3_{}_g4_og8", 2, 32, 7, 9, 32, 3, 1, 1, DR, dict(oct=8), group=4)
-_both("direct3x3_{}_g4_og12", 2, 32, 7, 9, 48, 3, 2, 1, DR, dict(oct=4), group=4)
-_add("dw5x5s1_i8_c32", _i8(2, 32, 9, 11, 32, k=5, pad=2, group=32), DD, dict(valid=False, dw_kernel="generic"))
-_add("dw3x3s2_u8_c32", _u8(2, 32, 9, 11, 32, k=3, stride=2, pad=1, group=32), DD, dict(valid=False, dw_kernel="generic"))
-_add("dw3x3s1_i8_c32_notc", _i8(2, 32, 7, 13, 32, k=3, pad=1, group=32), DD, dict(dw_kernel="dw3x3_i8", dw_ow_tail=5), flags=NO_TC)
-_add("dw3x3s2_i8_c48_notc", _i8(2, 48, 9, 13, 48, k=3, stride=2, pad=1, group=48, mode=0), DD, dict(dw_kernel="dw3x3_i8", dw_ow_tail=3),
+_both("direct3x3_{}_g4_og8", 2, 32, 7, 9, 32, 3, 1, 1, DR, dict(oct=8), group=4, recipe=REF)
+_both("direct3x3_{}_g4_og12", 2, 32, 7, 9, 48, 3, 2, 1, DR, dict(oct=4), group=4, recipe=REF)
+_add("dw5x5s1_i8_c32", _i8(2, 32, 9, 11, 32, k=5, pad=2, group=32, recipe=REF), DD, dict(valid=False, dw_kernel="generic"))
+_add("dw3x3s2_u8_c32", _u8(2, 32, 9, 11, 32, k=3, stride=2, pad=1, group=32, recipe=REF), DD, dict(valid=False, dw_kernel="generic"))
+_add("dw3x3s1_i8_c32_notc", _i8(2, 32, 7, 13, 32, k=3, pad=1, group=32, recipe=REF), DD, dict(dw_kernel="dw3x3_i8", dw_ow_tail=5),
      flags=NO_TC)
+_add("dw3x3s2_i8_c48_notc", _i8(2, 48, 9, 13, 48, k=3, stride=2, pad=1, group=48, mode=0, recipe=REF), DD,
+     dict(dw_kernel="dw3x3_i8", dw_ow_tail=3), flags=NO_TC)
 _add("dw3x3s1_i8_c32_w16_notc", _i8(1, 32, 5, 16, 32, k=3, pad=1, group=32), DD, dict(dw_kernel="dw3x3_i8", dw_ow_tail=0), flags=NO_TC)
 
 # ---- activation clamps in the epilogues: ReLU and ReLU6 (HCL), [-1, 1] and ReLU6 (REF) ------------------------------------------
@@ -767,6 +796,8 @@ _ACT_SHAPES = {  # kernel, (n, c, h, w, oc, k, stride, pad, group), dtypes
     "gemm1x1": (G_, (2, 64, 9, 7, 40, 1, 1, 0, 1), ("i8", "u8")),
     "dw3x3": (D_, (2, 32, 9, 10, 32, 3, 1, 1, 32), ("i8",)),
 }
+# Every recipe on every kernel, so also the ones Tengine never picks for the shape (conv_recipe: HCL for group 1, REF for the
+# batched depthwise): those are abi_only.
 for sh, (kern, (n, c, h, w, oc, k, st, pd, gp), dts) in _ACT_SHAPES.items():
     for a, (act, rec, so) in ACTS.items():
         for d in dts:
@@ -774,7 +805,8 @@ for sh, (kern, (n, c, h, w, oc, k, st, pd, gp), dts) in _ACT_SHAPES.items():
             if kern == D_:
                 edges["valid"] = True
             _add(f"{sh}_{d}_{a}", lambda r, d=d, act=act, rec=rec, so=so, n=n, c=c, h=h, w=w, oc=oc, k=k, st=st, pd=pd, gp=gp:
-                 act_conv(r, d == "u8", n, c, h, w, oc, act, rec, so, k=k, stride=st, pad=pd, group=gp, t_mid=0.75), kern, edges)
+                 act_conv(r, d == "u8", n, c, h, w, oc, act, rec, so, k=k, stride=st, pad=pd, group=gp, t_mid=0.75), kern, edges,
+                 abi_only=(rec == REF) == (gp == 1))
 # bounds beyond the byte range: ReLU6 at t = 192 > 127 (int8); uint8 output zero points 254 (ReLU6's 2 + 254 > 255) and 0
 # ([-1, 1]'s -1 + 0 < 0)
 _add("win3x3_i8_hcl6_sat", lambda r: act_conv(r, False, 2, 3, 9, 32, 24, 6, abi.RECIPE_HCL, 2.0 ** -5, t_mid=126.5), WI,
@@ -782,9 +814,9 @@ _add("win3x3_i8_hcl6_sat", lambda r: act_conv(r, False, 2, 3, 9, 32, 24, 6, abi.
 _add("win3x3_u8_hcl6_zo254", lambda r: act_conv(r, True, 2, 3, 9, 32, 24, 6, abi.RECIPE_HCL, 4.0, zo=254, t_mid=0.75), WI,
      dict(act="hcl6", bound_half=True, bound_beyond_sat=True))
 _add("gat3x3_u8_ref1_zo0", lambda r: act_conv(r, True, 2, 3, 9, 30, 24, 1, abi.RECIPE_REF, 2.0, zo=0), GA,
-     dict(act="ref1", bound_half=True, bound_beyond_sat=True))
+     dict(act="ref1", bound_half=True, bound_beyond_sat=True), abi_only=True)
 _add("stem3x3_u8_ref6_zo254", lambda r: act_conv(r, True, 2, 4, 9, 11, 24, 6, abi.RECIPE_REF, 4.0, zo=254, t_mid=0.75), ST,
-     dict(act="ref6", bound_beyond_sat=True))
+     dict(act="ref6", bound_beyond_sat=True), abi_only=True)
 # ---- glue ----------------------------------------------------------------------------------------------------------------
 _P = "pool"
 for d, u in (("i8", False), ("u8", True)):
@@ -872,8 +904,10 @@ for zx in (0, 255):
     _add(f"gat7x7s2_u8_c3_zx{zx}", _u8(2, 3, 16, 24, 40, k=7, stride=2, pad=3, zx=zx), GA, dict(ks=5, zx=zx, window_valid=False))
     _add(f"igemm3x3_u8_zx{zx}_m2", _u8(2, 64, 9, 10, 40, k=3, pad=1, mode=2, zx=zx), I_, dict(border=1, zx=zx))
     _add(f"direct3x3_u8_c32_notc_zx{zx}", _u8(2, 32, 7, 9, 32, k=3, pad=1, zx=zx), DR, dict(oct=8, zx=zx), flags=NO_TC)
-    _add(f"dw3x3s1_u8_c32_zx{zx}", _u8(2, 32, 9, 11, 32, k=3, pad=1, group=32, zx=zx), DD, dict(dw_kernel="generic", zx=zx))
-    _add(f"dw3x3s2_u8_c32_zx{zx}", _u8(2, 32, 9, 11, 32, k=3, stride=2, pad=1, group=32, zx=zx), DD, dict(dw_kernel="generic", zx=zx))
+    _add(f"dw3x3s1_u8_c32_zx{zx}", _u8(2, 32, 9, 11, 32, k=3, pad=1, group=32, zx=zx, recipe=REF), DD,
+         dict(dw_kernel="generic", zx=zx))
+    _add(f"dw3x3s2_u8_c32_zx{zx}", _u8(2, 32, 9, 11, 32, k=3, stride=2, pad=1, group=32, zx=zx, recipe=REF), DD,
+         dict(dw_kernel="generic", zx=zx))
     _add(f"direct3x3d2_u8_c32_zx{zx}", lambda r, zx=zx: u8_conv_pad(r, 2, 32, 12, 16, 24, 3, 1, 2, dilation=2, zx=zx), DR,
          dict(oct=8, zx=zx))
 # output zero points 0 and 255 under every activation: make_epi saturates the clamp's bounds before it builds the fast
@@ -883,12 +917,40 @@ _ZO_SHAPES = {"gemm1x1": (G_, (2, 64, 9, 7, 40, 1, 1, 0, 1)), "win3x3": (WI, (2,
               "direct3x3": (DR, (2, 32, 7, 9, 32, 3, 1, 1, 4))}
 for sh, (kern, (n, c, h, w, oc, k, st, pd, gp)) in _ZO_SHAPES.items():
     for a, (act, rec, so) in _ZO_ACTS.items():
+        if a == "none":
+            rec = abi.RECIPE_HCL if gp == 1 else REF  # no clamp: the recipe Tengine gives the shape (conv_recipe)
         for zo in (0, 255):
             t_mid = {"none": 20.0 if zo == 0 else -20.0, "ref1": 0.0}.get(a, 0.75)
             dense = zo == 0 or a in ("none", "ref1")
             _add(f"{sh}_u8_{a}_zo{zo}", lambda r, act=act, rec=rec, so=so, zo=zo, t_mid=t_mid, n=n, c=c, h=h, w=w, oc=oc, k=k, st=st,
                  pd=pd, gp=gp: act_conv(r, True, n, c, h, w, oc, act, rec, so, k=k, stride=st, pad=pd, group=gp, zo=zo, t_mid=t_mid),
-                 kern, dict(act=a, zo=zo), ties=dense, notes={} if dense else dict(constant_output=True))
+                 kern, dict(act=a, zo=zo), ties=dense, notes={} if dense else dict(constant_output=True), abi_only=(rec == REF) == (gp == 1))
+# The REF clamps where Tengine itself runs conv_ref (conv_recipe): grouped direct convs (OCT 8 and 4), the uint8 generic
+# depthwise, and int8 depthwise convs at batch 1 that conv_dw_hcl_x86 turns down (one-sided padding on one axis, a 5x5 kernel).
+# Tie-dense at the half-integer bounds, so that the reference itself says where a clamped value rounds.
+_REF_SHAPES = {  # name ({} = dtype), kernel, (n, c, h, w, oc, k, stride, pad, group), dtypes, edges
+    "direct3x3_{}_g4_og8": (DR, (2, 32, 7, 9, 32, 3, 1, 1, 4), ("i8", "u8"), dict(oct=8)),
+    "direct3x3_{}_g4_og12": (DR, (2, 32, 7, 9, 48, 3, 2, 1, 4), ("i8", "u8"), dict(oct=4)),
+    "dw3x3s1_{}_c32": (DD, (2, 32, 9, 11, 32, 3, 1, 1, 32), ("u8",), dict(dw_kernel="generic")),
+    "dw3x3s2_{}_c32": (DD, (2, 32, 9, 11, 32, 3, 2, 1, 32), ("u8",), dict(dw_kernel="generic")),
+    "dw3x3s1_{}_n1_pad0111": (D_, (1, 32, 9, 11, 32, 3, 1, (0, 1, 1, 1), 32), ("i8",), dict(valid=True)),
+    "dw5x5s1_{}_n1": (DD, (1, 32, 9, 11, 32, 5, 1, 2, 32), ("i8",), dict(dw_kernel="generic")),
+}
+for sh, (kern, (n, c, h, w, oc, k, st, pd, gp), dts, edges) in _REF_SHAPES.items():
+    for a in ("ref1", "ref6"):
+        act, _, so = ACTS[a]
+        for d in dts:
+            _add(sh.format(d) + "_" + a, lambda r, d=d, act=act, so=so, n=n, c=c, h=h, w=w, oc=oc, k=k, st=st, pd=pd, gp=gp:
+                 act_conv(r, d == "u8", n, c, h, w, oc, act, REF, so, k=k, stride=st, pad=pd, group=gp, t_mid=0.75), kern,
+                 dict(edges, act=a, bound_half=True, bound_beyond_sat=False))
+# and [-1, 1] at uint8 output zero points 0 and 255 (t about 0: both bounds live)
+for sh in ("direct3x3_{}_g4_og12", "dw3x3s2_{}_c32"):
+    kern, (n, c, h, w, oc, k, st, pd, gp), _, edges = _REF_SHAPES[sh]
+    for zo in (0, 255):
+        _add(sh.format("u8") + f"_ref1_zo{zo}", lambda r, zo=zo, n=n, c=c, h=h, w=w, oc=oc, k=k, st=st, pd=pd, gp=gp:
+             act_conv(r, True, n, c, h, w, oc, 1, REF, 2.0, k=k, stride=st, pad=pd, group=gp, zo=zo, t_mid=0.0), kern,
+             dict(edges, act="ref1", zo=zo, bound_beyond_sat=True))
+
 # glue ops at the ends of the byte range
 _PW, _CR, _LUT = "pointwise", "concat_requant", "byte_lut"
 # uint8 pooling has no lower clamp: below 0 (zo < zi) the result wraps
@@ -955,8 +1017,8 @@ _add("upsample2_c24_i8_min", lambda r: upsample(r, False, 24, 2, min_byte=True),
 _add("win3x3s1_i8_c3_min", _i8(2, 3, 15, 32, 24, k=3, pad=1, min_byte=True), WI, dict(_M, layout=0))
 _add("gat3x3s1_i8_c3_min", _i8(2, 3, 14, 30, 24, k=3, pad=1, min_byte=True), GA, dict(_M, window_valid=False))
 _add("gemm1x1_i8_min", _i8(2, 64, 9, 7, 40, mode=1, min_byte=True), G_, dict(_M))
-_add("dw3x3s1_i8_c32_min", _i8(2, 32, 9, 10, 32, k=3, pad=1, group=32, min_byte=True), D_, dict(_M, valid=True))
-_add("dw5x5s1_i8_c32_min", _i8(2, 32, 9, 11, 32, k=5, pad=2, group=32, min_byte=True), DD, dict(_M, dw_kernel="generic"))
+_add("dw3x3s1_i8_c32_min", _i8(2, 32, 9, 10, 32, k=3, pad=1, group=32, min_byte=True, recipe=REF), D_, dict(_M, valid=True))
+_add("dw5x5s1_i8_c32_min", _i8(2, 32, 9, 11, 32, k=5, pad=2, group=32, min_byte=True, recipe=REF), DD, dict(_M, dw_kernel="generic"))
 
 # Boundaries: geometry key -> the values that must each be reached by some entry (both sides of every edge)
 BOUNDARIES = {
@@ -1007,10 +1069,26 @@ BOUNDARIES = {
     "zo": {0, 255},
     "pool_wraps": {True, False},
     "in_min_byte": {True, False},
+    # a conv entry whose recipe only a C-ABI caller can ask for (Entry.abi_only), and one with the recipe Tengine picks
+    "abi_only": {True, False},
 }
 
 # Edges no graph can reach, and why (none so far).
 UNREACHABLE = {}
+
+# Entries on which the device's arithmetic (the oracle's uint8 mode 0: the exact integer sum) and the unmodified reference differ
+# by more than 1 LSB: entry -> (layer, the largest difference in LSB, why).  The reference's fp32 simulation (oracle mode 1) equals
+# the reference on every one of them.
+REFERENCE_DIVERGENCES = {
+    name: (0, 15, "K = 25088 and |x - zx| = |w - zw| >= 235: the reference sums the products in fp32, which rounds once the sum "
+                  "passes 2^24 (|acc| ~ 1.5e9 here); the device keeps the exact integer sum")
+    for name in ("fc_u8_far_z255_0", "fc_u8_far_z0_255")
+}
+
+
+def reference_entries():
+    """The entries the unmodified reference can judge: every one but the abi_only convs."""
+    return [n for n, e in ENTRIES.items() if not e.abi_only]
 
 
 def gemm_entries():

@@ -34,8 +34,51 @@ def test_every_boundary_is_reached_on_each_side():
         for k, v in e.edges.items():
             if k in seen:
                 seen[k].add(v)
+        if e.kernel in ke.CONV_KERNELS:
+            seen["abi_only"].add(e.abi_only)
     missing = {k: sorted(map(str, want - seen[k])) for k, want in ke.BOUNDARIES.items() if want - seen[k]}
     assert not missing, f"boundary sides no entry reaches: {missing}"
+
+
+@pytest.mark.parametrize("name", NAMES)
+def test_entry_has_the_recipe_tengine_picks_unless_abi_only(name):
+    """A conv entry carries the recipe b200_device.cc conv_recipe gives its shape (what the unmodified reference runs), or is
+    marked abi_only: a recipe that only a C-ABI caller can ask for."""
+    e = ke.ENTRIES[name]
+    case = ke.build(name)
+    L = case.g.layers[e.layer]
+    if L["op"] != ke.abi.OP_CONV:
+        assert not e.abi_only, f"{name}: abi_only on a layer that is not a convolution"
+        return
+    tengine = ke.conv_recipe(case.g, L)
+    assert (L["recipe"] != tengine) == e.abi_only, \
+        f"{name}: recipe {L['recipe']}, conv_recipe gives {tengine}, abi_only={e.abi_only}"
+
+
+def test_conv_recipe_restates_the_device_glue():
+    """Group 1 is HCL; a depthwise conv is HCL only for int8 at batch 1, 3x3, stride 1 or 2, each axis padded alike on both
+    sides (pad_h may differ from pad_w); every other grouped conv, and every uint8 one, is REF."""
+    from tengine_b200.graphdef import GraphDef
+
+    def recipe(dtype, n, c, oc, k, stride, pad, group, dilation=1):
+        g = GraphDef(dtype)
+        u8 = dtype == ke.abi.DT_UINT8
+        x = g.input(n, c, 12, 12, 0.5, 128 if u8 else 0)
+        w = np.zeros((oc, c // group, k, k), np.uint8 if u8 else np.int8)
+        g.conv(x, w, None, [0.5] * (1 if u8 else oc), 0.5, 128 if u8 else 0, stride=stride, pad=pad, group=group, dilation=dilation)
+        return ke.conv_recipe(g, g.layers[0])
+
+    H, R, I8, U8 = ke.abi.RECIPE_HCL, ke.abi.RECIPE_REF, ke.abi.DT_INT8, ke.abi.DT_UINT8
+    assert recipe(I8, 4, 16, 32, 3, 1, 1, 1) == H and recipe(U8, 4, 16, 32, 5, 2, 0, 1) == H
+    assert recipe(I8, 1, 32, 32, 3, 1, 1, 32) == H and recipe(I8, 1, 32, 32, 3, 2, (1, 1, 0, 0), 32) == H
+    assert recipe(I8, 2, 32, 32, 3, 1, 1, 32) == R  # batched
+    assert recipe(U8, 1, 32, 32, 3, 1, 1, 32) == R  # uint8
+    assert recipe(I8, 1, 32, 32, 5, 1, 2, 32) == R  # 5x5
+    assert recipe(I8, 1, 32, 32, 3, 3, 1, 32) == R  # stride 3
+    assert recipe(I8, 1, 32, 32, 3, 1, 2, 32, dilation=2) == R
+    assert recipe(I8, 1, 32, 32, 3, 1, (0, 1, 1, 1), 32) == R  # one-sided padding
+    assert recipe(I8, 1, 32, 32, 3, 1, 1, 4) == R  # grouped, not depthwise
+    assert recipe(I8, 1, 32, 64, 3, 1, 1, 32) == R  # group == C but OC != C
 
 
 def test_par_all_boundary_sits_at_par_max():
